@@ -115,10 +115,14 @@ class DCGANTrainer:
                 out["%s.%s" % (tag, k)] = v.detach()
         return out
 
+    def _engine_kwargs(self):
+        """extra DcganEngine arguments of a subclass (e.g. the critic's output activation)"""
+        return {}
+
     def _engine_synced(self):
         m = self.model
         if self._engine is None:
-            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant)
+            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, **self._engine_kwargs())
             self._dirty = True
         if self._dirty:
             self._engine.load_torch_weights(self._sd())
@@ -134,7 +138,7 @@ class DCGANTrainer:
             for tag, mod in (("G", self.model.G), ("D", self.model.D)):
                 for k, v in mod.named_parameters():
                     v.copy_(tw["%s.%s" % (tag, k)].to(v.device))
-                for i, bn in ((1, getattr(mod, "bn1", None)), (2, mod.bn2), (3, mod.bn3), (4, mod.bn4)):
+                for i, bn in ((i, getattr(mod, "bn%d" % i, None)) for i in range(1, 5)):       # a critic may have none
                     run = (self._engine.run_G.get(i - 1) if tag == "G" else self._engine.run_D.get(i - 1))
                     if bn is not None and run is not None:
                         bn.running_mean.copy_(run[0].cpu())

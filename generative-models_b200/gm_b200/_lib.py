@@ -135,6 +135,10 @@ def lib():
     L.gm_stage_images.argtypes = [vp, vp, i, vp, vp, i, i, i, vp]
     L.gm_noise_rows.argtypes = [vp, vp, vp, i, i, i, u64, u64, vp]
     L.gm_loss_rows.argtypes = [vp, i, i, vp, i, i, f, vp, vp, vp, vp]
+    L.gm_gp_interp_rows.argtypes = [vp, vp, i, vp, i, i, i, i, vp, vp, u64, u64, vp, i, vp]
+    L.gm_gp_penalty.argtypes = [vp, vp, i, i, i, i, f, f, f, vp, i, vp, vp, vp]
+    L.gm_im2col_k4s2_lrelu_mask.argtypes = [vp, vp, i, i, i, i, i, vp, i, f, vp, i, vp]
+    L.gm_lrelu_mask_rows.argtypes = [vp, vp, i, vp, i, ll, i, f, vp, i, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]

@@ -7,6 +7,7 @@
 // statistics) and the activations are column-statistics + elementwise kernels over the same matrices.  All HBM-bound:
 // 16-byte accesses, grids sized in multiples of the SM count, deterministic two-stage reductions.
 #pragma once
+#include <curand_kernel.h>
 #include "ptx.cuh"
 
 namespace gm {
@@ -486,6 +487,148 @@ __global__ void pack_col0_kernel(const float* __restrict__ v, int rows, __nv_bfl
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= (long long)rows * ld) return;
   out[i] = __float2bfloat16_rn((i % ld) == 0 ? v[i / ld] : 0.f);
+}
+
+// ---------------------------------------------------------------- WGAN-GP on the batch-norm-free conv critic (DESIGN.md §6b)
+// The critic is piecewise linear, so the penalty's double backward is closed form: an input-gradient chain at x_hat, a
+// per-image norm, a forward-mode (tangent) pass under the same LeakyReLU masks, and one weight-gradient GEMM per layer.
+// The kernels below are the parts of that which are not already an im2col / col2im / GEMM.
+
+// per-image eps: the caller's eps_in[b], else Philox U(0,1] with subsequence b of stream (seed, stream_id)
+__device__ __forceinline__ float gp_eps(const float* __restrict__ eps_in, uint32_t b, unsigned long long seed, unsigned long long stream_id) {
+  if (eps_in) return eps_in[b];
+  curandStatePhilox4_32_10_t st;
+  curand_init(seed ^ 0x9E3779B97F4A7C15ull, (unsigned long long)b, stream_id * 256ull, &st);
+  return curand_uniform(&st);   // (0,1]; torch.rand is [0,1)
+}
+
+// x_hat = eps x + (1 - eps) fake per image (src/w_gp_gan.py:197-201) over NHWC rows [B*HW, C].  The two products and the sum
+// are rounded separately (no FMA contraction): bit-identical to torch's eps * x + (1 - eps) * fake in fp32, then bf16.
+// eps_out[b] (nullable) receives the eps used.  One thread per value, grid-stride.
+__global__ void __launch_bounds__(256) gp_interp_kernel(const __nv_bfloat16* __restrict__ xr, int ldr, const __nv_bfloat16* __restrict__ xf,
+                                                        int ldf, uint32_t HW, uint32_t C, uint32_t total, const float* __restrict__ eps_in,
+                                                        float* __restrict__ eps_out, unsigned long long seed, unsigned long long stream_id,
+                                                        __nv_bfloat16* __restrict__ out, int ldo) {
+  griddep_sync();
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const uint32_t pix = i / C, c = i - pix * C, b = pix / HW;
+    const float e = gp_eps(eps_in, b, seed, stream_id);
+    const float a = __bfloat162float(xr[size_t(pix) * ldr + c]), f = __bfloat162float(xf[size_t(pix) * ldf + c]);
+    out[size_t(pix) * ldo + c] = __float2bfloat16_rn(__fadd_rn(__fmul_rn(e, a), __fmul_rn(__fsub_rn(1.f, e), f)));
+    if (eps_out && c == 0 && pix == b * HW) eps_out[b] = e;
+  }
+}
+
+// One block per image b of the image gradient g [B*HW, C]: norm_b = ||g_b||_2 (fp32 per thread, fixed reduction tree),
+// k_b = 2 lambda inv_grad (norm_b - 1) / norm_b, or 0 when norm_b == 0 (torch's subgradient, DESIGN.md §4), and the tangent
+// seed r_b = k_b g_b = dP/dg_b in bf16.  norm_out[b] = norm_b.
+constexpr int kGpThreads = 256;
+__global__ void __launch_bounds__(kGpThreads) gp_penalty_kernel(const __nv_bfloat16* __restrict__ g, int ldg, int HW, int C, float lambda,
+                                                                float inv_grad, __nv_bfloat16* __restrict__ r, int ldr, float* __restrict__ norm_out) {
+  griddep_sync();
+  __shared__ double sh[kGpThreads / 32];
+  const int n = HW * C;
+  const __nv_bfloat16* gb = g + size_t(blockIdx.x) * HW * ldg;
+  __nv_bfloat16* rb = r + size_t(blockIdx.x) * HW * ldr;
+  float ss = 0.f;
+  for (int i = threadIdx.x; i < n; i += kGpThreads) {
+    const int pix = i / C, c = i - pix * C;
+    const float v = __bfloat162float(gb[size_t(pix) * ldg + c]);
+    ss = fmaf(v, v, ss);
+  }
+  const float norm = sqrtf(float(block_sum<kGpThreads>(double(ss), sh)));
+  const float k = norm > 0.f ? 2.f * lambda * inv_grad * (norm - 1.f) / norm : 0.f;
+  for (int i = threadIdx.x; i < n; i += kGpThreads) {
+    const int pix = i / C, c = i - pix * C;
+    rb[size_t(pix) * ldr + c] = __float2bfloat16_rn(k * __bfloat162float(gb[size_t(pix) * ldg + c]));
+  }
+  if (threadIdx.x == 0) norm_out[blockIdx.x] = norm;
+}
+// loss[0] += lambda inv_loss sum_b (norm_b - 1)^2 (src/w_gp_gan.py:215,218); one block, fixed order
+__global__ void __launch_bounds__(kGpThreads) gp_loss_kernel(const float* __restrict__ norms, int B, float lambda, float inv_loss,
+                                                             float* __restrict__ loss) {
+  griddep_sync();
+  __shared__ double sh[kGpThreads / 32];
+  double t = 0.0;
+  for (int b = threadIdx.x; b < B; b += kGpThreads) {
+    const double d = double(norms[b]) - 1.0;
+    t += d * d;
+  }
+  t = block_sum<kGpThreads>(t, sh);
+  if (threadIdx.x == 0) loss[0] += float(double(lambda) * double(inv_loss) * t);
+}
+
+// im2col of the masked tensor x * LeakyReLU'(m) (m: the layer's activation, whose sign is the mask): the tangent
+// t_l = phi'_l(y_l) * u_l of the penalty's forward-mode pass, gathered straight into the column matrix that both the next
+// tangent GEMM and the penalty's weight-gradient GEMM read.  C % 8 == 0; the item mapping is im2col_k4s2_kernel<true>'s
+// plus one 16-byte load of m per item.  The product is rounded once (fp32 -> bf16).
+__global__ void __launch_bounds__(256) im2col_k4s2_lrelu_mask_kernel(const __nv_bfloat16* __restrict__ x, int H, int W, int C, int ldx,
+                                                                     const __nv_bfloat16* __restrict__ m, int ldm, float slope,
+                                                                     __nv_bfloat16* __restrict__ col, int ldc, uint32_t total, FastDiv dcg,
+                                                                     FastDiv dwo, FastDiv dho) {
+  griddep_sync();
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x; t0 < total; t0 += stride * kConvUnroll) {
+    uint4 v[kConvUnroll], mv[kConvUnroll];
+    __nv_bfloat16* dst[kConvUnroll];
+    bool live[kConvUnroll];
+#pragma unroll
+    for (int u = 0; u < kConvUnroll; ++u) {
+      const uint32_t t = t0 + u * stride;
+      live[u] = t < total && t >= t0;
+      uint32_t r, g;
+      fdivmod(t, dcg, r, g);
+      const uint32_t tap = r & 15u;
+      r >>= 4;
+      uint32_t q, wo, b, ho;
+      fdivmod(r, dwo, q, wo);
+      fdivmod(q, dho, b, ho);
+      const int iy = 2 * int(ho) - 1 + int(tap >> 2), ix = 2 * int(wo) - 1 + int(tap & 3u);
+      const bool ok = live[u] && iy >= 0 && iy < H && ix >= 0 && ix < W;
+      const size_t p = (size_t(b) * H + iy) * W + ix;
+      dst[u] = col + size_t(r) * ldc + tap * C + g * 8;
+      v[u] = make_uint4(0, 0, 0, 0);
+      mv[u] = make_uint4(0, 0, 0, 0);
+      if (ok) {
+        v[u] = __ldg(reinterpret_cast<const uint4*>(x + p * ldx + g * 8));
+        mv[u] = __ldg(reinterpret_cast<const uint4*>(m + p * ldm + g * 8));
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kConvUnroll; ++u) {
+      if (!live[u]) continue;
+      const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w}, mw[4] = {mv[u].x, mv[u].y, mv[u].z, mv[u].w};
+      float o[8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        o[2 * q] = bf16_lo(mw[q]) > 0.f ? bf16_lo(w[q]) : slope * bf16_lo(w[q]);
+        o[2 * q + 1] = bf16_hi(mw[q]) > 0.f ? bf16_hi(w[q]) : slope * bf16_hi(w[q]);
+      }
+      store_bf16x8(dst[u], o, 0);
+    }
+  }
+}
+
+// out = x * LeakyReLU'(m) over rows [rows, C], C % 8 == 0 (the 4x4 layer in front of the 1-logit conv, where the masked
+// im2col degenerates to an elementwise mask).  out may alias x or m: every thread reads its 16 bytes before writing them.
+__global__ void __launch_bounds__(256) lrelu_mask_rows_kernel(const __nv_bfloat16* x, int ldx, const __nv_bfloat16* m, int ldm, uint32_t groups,
+                                                              uint32_t total, float slope, __nv_bfloat16* out, int ldo) {
+  griddep_sync();
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const uint32_t r = i / groups, g = i - r * groups;
+    const uint4 v = *reinterpret_cast<const uint4*>(x + size_t(r) * ldx + g * 8);
+    const uint4 mv = *reinterpret_cast<const uint4*>(m + size_t(r) * ldm + g * 8);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w}, mw[4] = {mv.x, mv.y, mv.z, mv.w};
+    float o[8];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      o[2 * q] = bf16_lo(mw[q]) > 0.f ? bf16_lo(w[q]) : slope * bf16_lo(w[q]);
+      o[2 * q + 1] = bf16_hi(mw[q]) > 0.f ? bf16_hi(w[q]) : slope * bf16_hi(w[q]);
+    }
+    store_bf16x8(out + size_t(r) * ldo + g * 8, o, 0);
+  }
 }
 
 }  // namespace gm

@@ -12,6 +12,10 @@ README cites (Radford et al. 2015) with the reference's sigmoid outputs:
   D: Conv(3, h, 4, 2, 1) LeakyReLU(0.2) -> Conv(h, 2h) BN LReLU -> Conv(2h, 4h) BN LReLU -> Conv(4h, 8h) BN LReLU
        -> Conv(8h, 1, 4, 1, 0) -> sigmoid                                   [B, 1]
 
+variant="wgp" (WGAN-GP, src/w_gp_gan.py:177-239) trains D as a critic without BatchNorm — LeakyReLU on conv 1-4, output
+relu(s) (src/w_gp_gan.py:61) or s (d_out_act="none") — and adds the gradient penalty at x_hat = eps x + (1 - eps) G(z),
+whose double backward is closed form because the critic is piecewise linear (_d_grad_wgp, DESIGN.md §6b).
+
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
 same matrices, the loss is the MLP path's loss kernel on the conv D's logits (gm_loss_rows), Adam is gm_adam_step.
@@ -24,7 +28,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import GmError, VARIANTS, check, lib, _ptr, _stream, gemm_bf16, adam_step
+from ._lib import GmError, OUT_ACTS, VARIANTS, check, lib, _ptr, _stream, gemm_bf16, adam_step
 
 SLOPE = 0.2
 BN_EPS = 1e-5
@@ -42,6 +46,18 @@ def _col2im(col, B, Hi, Wi, Cc, y, mode=C2I_NONE, aux=None):
     h = _lib.ctx()
     check(h, lib().gm_col2im_k4s2(h, _ptr(col), col.stride(0), B, Hi, Wi, Cc, _ptr(y), y.stride(0), mode, _ptr(aux),
                                   aux.stride(0) if aux is not None else 0, SLOPE, _stream()))
+
+
+def _im2col_lrelu_mask(x, B, H, W, Cc, m, col):
+    h = _lib.ctx()
+    check(h, lib().gm_im2col_k4s2_lrelu_mask(h, _ptr(x), B, H, W, Cc, x.stride(0), _ptr(m), m.stride(0), SLOPE, _ptr(col), col.stride(0),
+                                             _stream()))
+
+
+def _lrelu_mask(x, m, out):
+    h = _lib.ctx()
+    check(h, lib().gm_lrelu_mask_rows(h, _ptr(x), x.stride(0), _ptr(m), m.stride(0), x.shape[0], x.shape[1], SLOPE, _ptr(out),
+                                      out.stride(0), _stream()))
 
 
 def _bn_fwd(x, gamma, beta, act, y, stats, running):
@@ -101,16 +117,27 @@ class _Net:
 class DcganEngine:
     """One DCGAN (64x64xchannels images) on one GPU; see the module docstring."""
 
-    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None):
+    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None, d_out_act=None):
         if not torch.cuda.is_available():
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*)")
+        if variant not in ("ns", "mm", "w", "ls", "wgp") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*) and wgp")
+        if variant == "wgp":
+            # WGAN-GP critic: no BatchNorm (one sample's input gradient must not depend on the batch, WGAN-GP paper §4),
+            # output relu(s) as src/w_gp_gan.py:61 or the linear s
+            d_out_act = "relu" if d_out_act is None else d_out_act
+            if d_out_act not in ("relu", "none"):
+                raise GmError("the WGAN-GP conv critic's output is relu or none")
+        elif d_out_act not in (None, "sigmoid"):
+            raise GmError("the conv discriminator of the row-wise losses ends in a sigmoid")
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         self.h = _lib.ctx(self.device.index)
         self.hd, self.z, self.ch, self.variant = hidden_dim, z_dim, channels, variant
+        self.d_out_act = d_out_act or "sigmoid"
+        self.d_bn = variant != "wgp"                             # BatchNorm in D's layers 2-4
+        self.gp_lambda = 10.0                                    # LAMBDA of src/w_gp_gan.py:177
         self.zp = (z_dim + 1 + 7) // 8 * 8                       # noise rows: [z | 1 | pad], 16-byte rows
         hd = hidden_dim
         self.gc = [8 * hd, 4 * hd, 2 * hd, hd, channels]        # generator channels after each layer
@@ -124,11 +151,11 @@ class DcganEngine:
         for i in range(1, 4):
             d_shapes.append(("l%d.weight" % (i + 1), (self.dc[i], 16 * self.dc[i - 1])))
         d_shapes.append(("l5.weight", (16, 16 * self.dc[3])))   # 1 real output channel (row 0), padded to the MMA's N = 16
-        for i in range(1, 4):
+        for i in range(1, 4) if self.d_bn else ():
             d_shapes += [("bn%d.weight" % (i + 1), (self.dc[i],)), ("bn%d.bias" % (i + 1), (self.dc[i],))]
         self.G, self.D = _Net(g_shapes, self.device), _Net(d_shapes, self.device)
         self.run_G = {i: torch.zeros(2, self.gc[i], device=self.device) for i in range(4)}
-        self.run_D = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4)}
+        self.run_D = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4) if self.d_bn}
         for r in list(self.run_G.values()) + list(self.run_D.values()):
             r[1].fill_(1.0)
         self.loss_buf = torch.zeros(2, device=self.device)
@@ -250,8 +277,8 @@ class DcganEngine:
             _im2col(x, n, 2 * hw, 2 * hw, cin, col)
             c = self._buf(tag + "c%d" % i, n * hw * hw, dc[i])
             sv["col%d" % i] = col
-            if i == 0:
-                gemm_bf16(col, self.D.bf["l1.weight"], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU in the epilogue
+            if i == 0 or not self.d_bn:
+                gemm_bf16(col, self.D.bf["l%d.weight" % (i + 1)], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU epilogue
                 y = c
             else:
                 gemm_bf16(col, self.D.bf["l%d.weight" % (i + 1)], c, "nt")
@@ -274,6 +301,12 @@ class DcganEngine:
         check(self.h, lib().gm_pack_col0(self.h, _ptr(ds), n, _ptr(dy5), 16, _stream()))
         if need_wgrad:
             gemm_bf16(dy5, sv["flat"], D.view("l5.weight", grads), "tn")                  # [16, 128h]
+        if not self.d_bn:
+            betas = self._betas(sv, dy5, tag)
+            if need_wgrad:
+                for i in range(4):
+                    gemm_bf16(betas[i], sv["col%d" % i], D.view("l%d.weight" % (i + 1), grads), "tn")
+            return self._dimg(sv, betas[0], tag) if need_dimg else None
         dflat = self._buf(tag + "dflat", n, 16 * dc[3])
         gemm_bf16(dy5, D.bf_t["l5.weight"], dflat, "nt", K=16)
         d, hw = dflat.view(n * 16, dc[3]), 4
@@ -296,11 +329,34 @@ class DcganEngine:
             gemm_bf16(d, sv["col0"], D.view("l1.weight", grads), "tn")                    # [h, 16 ch]
         if not need_dimg:
             return None
-        dcol = self._buf(tag + "dcol0", sv["col0"].shape[0], sv["col0"].shape[1])
-        gemm_bf16(d, D.bf_t["l1.weight"], dcol, "nt")
-        dpre = self._buf(tag + "dpre", n * 4096, self.ch)
-        _col2im(dcol, n, 32, 32, self.ch, dpre, C2I_SIGMOID_GRAD, sv["img"])
+        return self._dimg(sv, d, tag)
+
+    def _dimg(self, sv, d, tag, mode=C2I_SIGMOID_GRAD):
+        """d = dL/d(conv 1 output) -> dL/d(image) (mode C2I_NONE) or dL/d(pre-sigmoid generator output) (C2I_SIGMOID_GRAD)"""
+        n = d.shape[0] // 1024
+        dcol = self._buf(tag + "dcol0", d.shape[0], 16 * self.ch)
+        gemm_bf16(d, self.D.bf_t["l1.weight"], dcol, "nt")
+        dpre = self._buf(tag + ("dpre" if mode == C2I_SIGMOID_GRAD else "dimg"), n * 4096, self.ch)
+        _col2im(dcol, n, 32, 32, self.ch, dpre, mode, sv["img"] if mode == C2I_SIGMOID_GRAD else None)
         return dpre
+
+    def _betas(self, sv, dy5, tag):
+        """Input-gradient chain of the batch-norm-free critic: dy5 [rows, 16] (column 0 = dL/dlogit per image) -> the
+        pre-activation gradients [beta_1, .., beta_4] of conv 1..4 as NHWC rows (beta_l = LReLU'(y_l) * W_{l+1}^T beta_{l+1})."""
+        n, dc, D = sv["n"], self.dc, self.D
+        dflat = self._buf(tag + "dflat", n, 16 * dc[3])
+        gemm_bf16(dy5, D.bf_t["l5.weight"], dflat, "nt", K=16)
+        betas = [None, None, None, self._buf(tag + "beta3", n * 16, dc[3])]
+        _lrelu_mask(dflat.view(n * 16, dc[3]), sv["y3"], betas[3])
+        hw = 4
+        for i in range(3, 0, -1):
+            col = sv["col%d" % i]
+            dcol = self._buf(tag + "dcol%d" % i, col.shape[0], col.shape[1])
+            gemm_bf16(betas[i], D.bf_t["l%d.weight" % (i + 1)], dcol, "nt")
+            betas[i - 1] = self._buf(tag + "beta%d" % (i - 1), n * 4 * hw * hw, dc[i - 1])
+            _col2im(dcol, n, hw, hw, dc[i - 1], betas[i - 1], C2I_LRELU_GRAD, sv["y%d" % (i - 1)])
+            hw *= 2
+        return betas
 
     # ------------------------------------------------------------------ the train step (src/ns_gan.py:126-156)
     def stage_images(self, images):
@@ -310,10 +366,18 @@ class DcganEngine:
         x = images.view(n, self.ch, 64, 64).permute(0, 2, 3, 1).to(torch.bfloat16).contiguous()
         return x.view(n * 4096, self.ch)
 
-    def d_grad(self, img_real, n, noise=None, inv_global_batch=None, seed=0, step=0):
-        """train_D + backward (src/ns_gan.py:172-194,138): img_real NHWC rows of n images (stage_images).  Writes the flat
-        D gradient (self.D.grads) and loss_buf[0]."""
+    def _loss_rows(self, logits, n, g_step, inv, ds, loss):
+        variant = VARIANTS["w" if self.variant == "wgp" else self.variant]       # WGAN-GP's rows are W's; the penalty is separate
+        check(self.h, lib().gm_loss_rows(self.h, variant, OUT_ACTS[self.d_out_act], _ptr(logits), n, g_step, inv, _ptr(ds), None,
+                                         loss, _stream()))
+
+    def d_grad(self, img_real, n, noise=None, inv_global_batch=None, seed=0, step=0, gp_lambda=None, eps=None):
+        """train_D + backward (src/ns_gan.py:172-194,138; src/w_gp_gan.py:177-220 for variant wgp): img_real NHWC rows of n
+        images (stage_images).  Writes the flat D gradient (self.D.grads) and loss_buf[0].  WGAN-GP only: gp_lambda (None =
+        self.gp_lambda) and eps [n] fp32 (None = on-device Philox keyed by (seed, step))."""
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
+        if self.variant == "wgp":
+            return self._d_grad_wgp(img_real, n, noise, inv, seed, step, self.gp_lambda if gp_lambda is None else float(gp_lambda), eps)
         fake, gsv = self.g_forward(n, noise, seed, 2 * step)
         lr_, lf_ = self._buf("logits_r", 16, n, torch.float32), self._buf("logits_f", 16, n, torch.float32)
         sr = self.d_forward(img_real, n, lr_, "dr")
@@ -333,6 +397,65 @@ class DcganEngine:
         self.scores_ = logits
         return self.loss_buf[0]
 
+    def _d_grad_wgp(self, img_real, n, noise, inv, seed, step, lam, eps):
+        """D_loss = mean(D(G(z))) - mean(D(x)) + lam mean_b (||grad D(x_hat_b)|| - 1)^2 and its D gradient (src/w_gp_gan.py:
+        186-218), the penalty's double backward in closed form (DESIGN.md §6b).  The critic has no BatchNorm, so real, fake
+        and x_hat images go through ONE forward and ONE input-gradient chain as 3n stacked images."""
+        fake, _ = self.g_forward(n, noise, seed, 2 * step)
+        return self.wgp_critic_grad(img_real, fake, n, inv, lam, eps, seed, step)
+
+    def wgp_critic_grad(self, img_real, fake, n, inv, lam, eps=None, seed=0, step=0):
+        """The critic half of _d_grad_wgp for given real and generated NHWC image rows (data-parallel splits, tests)."""
+        dc, D, ch = self.dc, self.D, self.ch
+        R = n * 4096
+        x3 = self._buf("gp_x3", 3 * R, ch)                                  # NHWC rows [real | fake | x_hat]
+        x3[:R].copy_(img_real)
+        x3[R:2 * R].copy_(fake)
+        eps_used = self._buf("gp_eps", 1, n, torch.float32)[0]
+        if eps is not None:
+            eps = eps.reshape(n).float().contiguous()
+        check(self.h, lib().gm_gp_interp_rows(self.h, _ptr(x3), ch, _ptr(x3[R:]), ch, n, 4096, ch, _ptr(eps), _ptr(eps_used),
+                                              int(seed), int(2 * step), _ptr(x3[2 * R:]), ch, _stream()))
+        # 1. primal forward of the 3n images; the LeakyReLU outputs y_l carry the masks
+        logits = self._buf("gp_logits", 16, 3 * n, torch.float32)
+        sv = self.d_forward(x3, 3 * n, logits, "dw")
+        # 2. upstream dL/dlogit: the W rows for real / fake (loss_buf[0] = mean(DG) - mean(DX)), and the penalty's seed
+        #    1[s > 0] (relu output) or 1 for x_hat: the loss kernel's train_G row (-d, gradient -act'(s) * inv) with inv = -1
+        ds = self._buf("gp_ds", 1, 3 * n, torch.float32)[0]
+        self._loss_rows(logits[0], n, 0, inv, ds, _ptr(self.loss_buf))
+        self._loss_rows(logits[0, 2 * n:], n, 1, -1.0, ds[2 * n:], _ptr(self._buf("gp_seed_loss", 1, 4, torch.float32)))
+        dy5 = self._buf("dwdy5", 3 * n, 16)
+        check(self.h, lib().gm_pack_col0(self.h, _ptr(ds), 3 * n, _ptr(dy5), 16, _stream()))
+        betas = self._betas(sv, dy5, "dw")
+        # 2b. image gradient g at x_hat and 3. the penalty: loss_buf[0] += lam mean (||g|| - 1)^2, tangent seed r = dP/dg
+        g = self._dimg(sv, betas[0][2 * n * 1024:], "gp", C2I_NONE)
+        r = self._buf("gp_r", R, ch)
+        norms = self._buf("gp_norm", 1, n, torch.float32)[0]
+        check(self.h, lib().gm_gp_penalty(self.h, _ptr(g), ch, n, 4096, ch, lam, inv, 1.0 / n, _ptr(r), ch, _ptr(norms),
+                                          _ptr(self.loss_buf), _stream()))
+        # 4. tangent pass t_0 = r, t_l = LReLU'(y_l) * conv_l(t_{l-1}) under x_hat's masks.  im2col(t_{l-1}) overwrites
+        #    x_hat's rows of the saved column matrices (and t_4 x_hat's rows of y_4 = the last layer's input), so that
+        # 5. each layer's weight gradient is ONE GEMM over the 3n images: W part (activations) + penalty (tangents).
+        _im2col(r, n, 64, 64, ch, sv["col0"][2 * n * 1024:])
+        hw = 32
+        for i in range(4):
+            off = 2 * n * hw * hw
+            u = self._buf("gp_u%d" % i, n * hw * hw, dc[i])
+            gemm_bf16(sv["col%d" % i][off:], D.bf["l%d.weight" % (i + 1)], u, "nt")
+            y_hat = sv["y%d" % i][off:]
+            if i < 3:
+                _im2col_lrelu_mask(u, n, hw, hw, dc[i], y_hat, sv["col%d" % (i + 1)][2 * n * (hw // 2) ** 2:])
+            else:
+                _lrelu_mask(u, y_hat, y_hat)
+            hw //= 2
+        D.grads.zero_()
+        gemm_bf16(dy5, sv["flat"], D.view("l5.weight", D.grads), "tn")
+        for i in range(4):
+            gemm_bf16(betas[i], sv["col%d" % i], D.view("l%d.weight" % (i + 1), D.grads), "tn")
+        self.scores_ = logits[0, :2 * n]
+        self.gp_norms_, self.gp_eps_ = norms, eps_used                      # per-image ||g|| and eps of this step
+        return self.loss_buf[0]
+
     def g_grad(self, n, noise=None, inv_global_batch=None, seed=0, step=0):
         """train_G + backward (src/ns_gan.py:196-216,155): G gradients only."""
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
@@ -340,8 +463,7 @@ class DcganEngine:
         logits = self._buf("logits_g", 16, n, torch.float32)
         sf = self.d_forward(fake, n, logits, "df")
         ds = self._buf("ds_g", 1, n, torch.float32)[0]
-        check(self.h, lib().gm_loss_rows(self.h, VARIANTS[self.variant], 0, _ptr(logits), n, 1, inv, _ptr(ds), None,
-                                         C.c_void_p(self.loss_buf.data_ptr() + 4), _stream()))
+        self._loss_rows(logits, n, 1, inv, ds, C.c_void_p(self.loss_buf.data_ptr() + 4))
         dpre = self.d_backward(sf, ds, None, need_wgrad=False, need_dimg=True, tag="df")
         self.g_backward(gsv, dpre)
         return self.loss_buf[1]
@@ -358,4 +480,5 @@ class DcganEngine:
         n = images.shape[0]
         logits = self._buf("logits_i", 16, n, torch.float32)
         self.d_forward(self.stage_images(images), n, logits, "di")
-        return torch.sigmoid(logits[0, :n]).view(n, 1)
+        s = logits[0, :n].view(n, 1)
+        return torch.sigmoid(s) if self.d_out_act == "sigmoid" else (torch.relu(s) if self.d_out_act == "relu" else s.clone())

@@ -326,6 +326,21 @@ int gm_noise_rows(gm_ctx* ctx, const float* noise_dev, void* out_dev, int rows, 
  * row-wise variants only (NS, MM, W, LS, f-GAN) */
 int gm_loss_rows(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, int g_step, float inv_global_batch,
                  float* ds_dev, float* d_out_dev, float* loss_dev, gm_stream stream);
+/* WGAN-GP on the batch-norm-free conv critic (src/w_gp_gan.py:197-218; gm_b200/dcgan.py sequences it).
+ * x_hat = eps x_real + (1 - eps) x_fake per image over NHWC rows [B*HW, C]; eps_dev [B] fp32, or NULL for Philox U(0,1]
+ * keyed by (seed, stream_id); eps_out_dev [B] (nullable) receives the eps used. */
+int gm_gp_interp_rows(gm_ctx* ctx, const void* xr_dev, int ldr, const void* xf_dev, int ldf, int B, int HW, int C, const float* eps_dev,
+                      float* eps_out_dev, uint64_t seed, uint64_t stream_id, void* out_dev, int ldo, gm_stream stream);
+/* per image b of the image gradient g [B*HW, C]: norm_dev[b] = ||g_b||, r_dev = 2 lambda inv_grad (||g_b|| - 1) / ||g_b|| g_b
+ * (0 when ||g_b|| = 0) as bf16, and loss_dev[0] += lambda inv_loss sum_b (||g_b|| - 1)^2 (loss_dev nullable) */
+int gm_gp_penalty(gm_ctx* ctx, const void* g_dev, int ldg, int B, int HW, int C, float lambda, float inv_grad, float inv_loss,
+                  void* r_dev, int ldr, float* norm_dev, float* loss_dev, gm_stream stream);
+/* gm_im2col_k4s2 of x * LeakyReLU'(m) (the sign of m selects slope 1 or `slope`); C a multiple of 8 */
+int gm_im2col_k4s2_lrelu_mask(gm_ctx* ctx, const void* x_dev, int B, int H, int W, int C, int ldx, const void* m_dev, int ldm, float slope,
+                              void* col_dev, int ldc, gm_stream stream);
+/* out = x * LeakyReLU'(m) over rows [rows, C]; C a multiple of 8; out may alias x or m */
+int gm_lrelu_mask_rows(gm_ctx* ctx, const void* x_dev, int ldx, const void* m_dev, int ldm, long long rows, int C, float slope,
+                       void* out_dev, int ldo, gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);

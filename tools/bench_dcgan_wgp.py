@@ -1,0 +1,98 @@
+"""Conv NSGAN step vs conv WGAN-GP step (D_steps = 1) on one GPU, in one process.
+
+    python tools/bench_dcgan_wgp.py [--batch 1024] [--steps 20] [--warmup 5]
+
+Both engines run the DCGAN of bench.py's dcgan workload (64x64x3, hidden 64, z 100) on device-resident synthetic images.
+The two steps alternate (rounds of one NSGAN step then one WGAN-GP step, each timed with its own CUDA events after the
+warm-up), so clock or thermal drift hits both alike.  Prints one JSON line: device name, power limit, images/s, library
+launches per step and achieved TFLOP/s from FLOPs counted from the shapes (bench.py's _dcgan_flop_per_img for NSGAN;
+the penalty adds one critic forward, one input-gradient chain to the image, one tangent forward and one weight-gradient
+pass = 4 critic forwards).  Writes nothing but stdout.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "generative-models_b200")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+
+def critic_flop_per_img(hd=64, ch=3):
+    dc = [hd, 2 * hd, 4 * hd, 8 * hd]
+    d_l = [1024 * dc[0] * 16 * ch, 256 * dc[1] * 16 * dc[0], 64 * dc[2] * 16 * dc[1], 16 * dc[3] * 16 * dc[2], 16 * dc[3]]
+    return 2.0 * sum(d_l)
+
+
+def power_limit(index):
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        return float(out.splitlines()[0])
+    except Exception:
+        return None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=1024)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    a = ap.parse_args()
+    import torch
+    import gm_b200
+    from bench import _dcgan_flop_per_img
+    dev = torch.cuda.current_device()
+    B = a.batch
+    g = torch.Generator(device="cuda").manual_seed(77)
+    pool = (torch.rand(2 * B * 4096, 3, device="cuda", generator=g) < 0.3).to(torch.bfloat16)
+    engines = {"ns": gm_b200.DcganEngine(64, 100, 3, variant="ns"), "wgp": gm_b200.DcganEngine(64, 100, 3, variant="wgp")}
+    hps = {"ns": (gm_b200.AdamHP.make(2e-4), gm_b200.AdamHP.make(2e-4)), "wgp": (gm_b200.AdamHP.make(1e-4), gm_b200.AdamHP.make(1e-4))}
+
+    def step(name, s):
+        eng, (hpG, hpD) = engines[name], hps[name]
+        x = pool[(s % 2) * B * 4096:(s % 2 + 1) * B * 4096]
+        eng.d_grad(x, B, seed=1000, step=s)
+        eng.apply(1, hpD)
+        eng.g_grad(B, seed=1000, step=s)
+        eng.apply(0, hpG)
+
+    launches = {}
+    for name in engines:
+        step(name, 0)
+        torch.cuda.synchronize()
+        gm_b200.launch_count(reset=True)
+        step(name, 1)
+        torch.cuda.synchronize()
+        launches[name] = gm_b200.launch_count(reset=True)
+    for s in range(a.warmup):
+        for name in engines:
+            step(name, 2 + s)
+    torch.cuda.synchronize()
+    ms = {name: [] for name in engines}
+    for s in range(a.steps):
+        for name in engines:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            step(name, 100 + s)
+            e1.record()
+            e1.synchronize()
+            ms[name].append(e0.elapsed_time(e1))
+    loss = {name: [float(v) for v in engines[name].loss_buf.tolist()] for name in engines}
+    flop = {"ns": _dcgan_flop_per_img(), "wgp": _dcgan_flop_per_img() + 4 * critic_flop_per_img()}
+    out = {"device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit(dev), "batch": B, "steps": a.steps,
+           "warmup": a.warmup}
+    for name in engines:
+        med = sorted(ms[name])[len(ms[name]) // 2]
+        out[name] = {"median_ms": round(med, 3), "min_ms": round(min(ms[name]), 3), "images_per_s": round(B / med * 1e3, 1),
+                     "launches_per_step": launches[name], "gflop_per_image": round(flop[name] / 1e9, 3),
+                     "tflops": round(flop[name] * B / med / 1e9, 1), "last_losses": loss[name]}
+    out["wgp_over_ns_images_per_s"] = round(out["wgp"]["images_per_s"] / out["ns"]["images_per_s"], 3)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
