@@ -157,6 +157,9 @@ class DCGANTrainer:
             for net in (eng.G, eng.D):
                 dist.broadcast(net.params, src=0)
                 net.refresh()
+        # batch statistics (RaNS / Fisher loss moments, DRAGAN's image std) run over the global batch: NCCL SUM between passes
+        eng.stats_reduce = par.sum_gradients if world > 1 else None
+        self._pre_train(eng)
         seed = par.rank_seed(self._seed, rank)
         epoch_steps = int(np.ceil(len(self.train_iter) / D_steps))
         for epoch in range(1, num_epochs + 1):
@@ -167,7 +170,8 @@ class DCGANTrainer:
                     images = self.process_batch(self.train_iter)
                     n = images.shape[0]
                     inv = par.inv_global_batch(n, world)
-                    ring[k, i] = eng.d_grad(eng.stage_images(images), n, inv_global_batch=inv, seed=seed, step=self._step * D_steps + k)
+                    ring[k, i] = eng.d_grad(eng.stage_images(images), n, inv_global_batch=inv, seed=seed, step=self._step * D_steps + k,
+                                            stat_batch=n * world)
                     par.sum_gradients(eng.D.grads)                  # NCCL SUM of the flat D gradient (no-op on one GPU)
                     eng.apply(1, hpD)
                 ring[D_steps, i] = eng.g_grad(n, inv_global_batch=inv, seed=seed, step=self._step)
@@ -180,6 +184,9 @@ class DCGANTrainer:
             print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
             self.num_epochs += 1
         self._pull()
+
+    def _pre_train(self, eng):
+        """per-train() state of a subclass (e.g. Fisher GAN's multiplier), after the optimizers are reset"""
 
     def _loss(self, net, loss_val):
         eng = self._engine

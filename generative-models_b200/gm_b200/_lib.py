@@ -139,6 +139,11 @@ def lib():
     L.gm_gp_penalty.argtypes = [vp, vp, i, i, i, i, f, f, f, vp, i, vp, vp, vp]
     L.gm_im2col_k4s2_lrelu_mask.argtypes = [vp, vp, i, i, i, i, i, vp, i, f, vp, i, vp]
     L.gm_lrelu_mask_rows.argtypes = [vp, vp, i, vp, i, ll, i, f, vp, i, vp]
+    L.gm_loss_stats.argtypes = [vp, i, i, vp, i, ll, i, vp, vp, vp]
+    L.gm_loss_rows_stats.argtypes = [vp, i, i, vp, i, f, vp, ll, vp, vp, vp, vp, vp]
+    L.gm_dra_std_sums.argtypes = [vp, vp, i, i, i, vp, vp]
+    L.gm_dra_xhat_rows.argtypes = [vp, vp, i, i, i, vp, C.c_double, f, vp, u64, u64, vp, i, vp]
+    L.gm_dra_penalty.argtypes = [vp, vp, i, vp, i, vp, i, i, i, f, f, f, f, vp, i, vp, vp, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]

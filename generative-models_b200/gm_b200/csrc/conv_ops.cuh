@@ -559,6 +559,66 @@ __global__ void __launch_bounds__(kGpThreads) gp_loss_kernel(const float* __rest
   if (threadIdx.x == 0) loss[0] += float(double(lambda) * double(inv_loss) * t);
 }
 
+// ---- DRAGAN on the sigmoid conv critic (src/dra_gan.py:174-225, DESIGN.md §6b)
+// (sum x, sum x^2) of the per-block partials of moments_kernel -> out[2] (doubles, fixed order): the local sums of
+// images.std() that data-parallel ranks add before xhat_kernel reads them
+__global__ void __launch_bounds__(256) moments_sum_kernel(const double* __restrict__ part, int nblk, double* __restrict__ out) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  double s1 = 0, s2 = 0;
+  for (int i = threadIdx.x; i < nblk; i += 256) { s1 += part[2 * i]; s2 += part[2 * i + 1]; }
+  s1 = block_sum<256>(s1, sh);
+  s2 = block_sum<256>(s2, sh);
+  if (threadIdx.x == 0) { out[0] = s1; out[1] = s2; }
+}
+
+// One block per x_hat image b.  J [HW*C] = image gradient of the logit s_b (the beta chain seeded with 1), xh the image.
+// sigma = sigmoid(s_b), sigma' = sigma (1 - sigma), ||g|| = sigma' ||J|| (the gradient of D's sigmoid output),
+// k = 2 lambda inv_grad (||g|| - K); the tangent seed of the penalty's double backward is
+//   r = k sigma' [J / ||J|| + (1 - 2 sigma) ||J|| xh]      (0 when ||J|| = 0)
+// whose tangent pass carries both sigma'' ||J|| ds/dtheta (the forward activations of xh are its own tangent: no biases,
+// LeakyReLU positively homogeneous) and sigma' (J/||J||) dJ/dtheta.  norm_out[b] = ||g||, r in bf16.
+__global__ void __launch_bounds__(kGpThreads) dra_penalty_kernel(const __nv_bfloat16* __restrict__ J, int ldj, const __nv_bfloat16* __restrict__ xh,
+                                                                 int ldx, const float* __restrict__ logits, int HW, int C, float lambda, float K,
+                                                                 float inv_grad, __nv_bfloat16* __restrict__ r, int ldr, float* __restrict__ norm_out) {
+  griddep_sync();
+  __shared__ double sh[kGpThreads / 32];
+  const int n = HW * C;
+  const __nv_bfloat16* jb = J + size_t(blockIdx.x) * HW * ldj;
+  const __nv_bfloat16* xb = xh + size_t(blockIdx.x) * HW * ldx;
+  __nv_bfloat16* rb = r + size_t(blockIdx.x) * HW * ldr;
+  float ss = 0.f;
+  for (int i = threadIdx.x; i < n; i += kGpThreads) {
+    const int pix = i / C, c = i - pix * C;
+    const float v = __bfloat162float(jb[size_t(pix) * ldj + c]);
+    ss = fmaf(v, v, ss);
+  }
+  const float nj = sqrtf(float(block_sum<kGpThreads>(double(ss), sh)));
+  const float sg = 1.f / (1.f + expf(-logits[blockIdx.x])), sp = sg * (1.f - sg);
+  const float ng = sp * nj;
+  const float k = 2.f * lambda * inv_grad * (ng - K) * sp;
+  const float a = nj > 0.f ? k / nj : 0.f, b = nj > 0.f ? k * (1.f - 2.f * sg) * nj : 0.f;
+  for (int i = threadIdx.x; i < n; i += kGpThreads) {
+    const int pix = i / C, c = i - pix * C;
+    const float jv = __bfloat162float(jb[size_t(pix) * ldj + c]), xv = __bfloat162float(xb[size_t(pix) * ldx + c]);
+    rb[size_t(pix) * ldr + c] = __float2bfloat16_rn(fmaf(a, jv, b * xv));
+  }
+  if (threadIdx.x == 0) norm_out[blockIdx.x] = ng;
+}
+// loss[0] += lambda inv_loss sum_b (norm_b - K)^2 (src/dra_gan.py:219); one block, fixed order
+__global__ void __launch_bounds__(kGpThreads) dra_loss_kernel(const float* __restrict__ norms, int B, float lambda, float K, float inv_loss,
+                                                              float* __restrict__ loss) {
+  griddep_sync();
+  __shared__ double sh[kGpThreads / 32];
+  double t = 0.0;
+  for (int b = threadIdx.x; b < B; b += kGpThreads) {
+    const double d = double(norms[b]) - double(K);
+    t += d * d;
+  }
+  t = block_sum<kGpThreads>(t, sh);
+  if (threadIdx.x == 0) loss[0] += float(double(lambda) * double(inv_loss) * t);
+}
+
 // im2col of the masked tensor x * LeakyReLU'(m) (m: the layer's activation, whose sign is the mask): the tangent
 // t_l = phi'_l(y_l) * u_l of the penalty's forward-mode pass, gathered straight into the column matrix that both the next
 // tangent GEMM and the penalty's weight-gradient GEMM read.  C % 8 == 0; the item mapping is im2col_k4s2_kernel<true>'s

@@ -14,7 +14,10 @@ README cites (Radford et al. 2015) with the reference's sigmoid outputs:
 
 variant="wgp" (WGAN-GP, src/w_gp_gan.py:177-239) trains D as a critic without BatchNorm — LeakyReLU on conv 1-4, output
 relu(s) (src/w_gp_gan.py:61) or s (d_out_act="none") — and adds the gradient penalty at x_hat = eps x + (1 - eps) G(z),
-whose double backward is closed form because the critic is piecewise linear (_d_grad_wgp, DESIGN.md §6b).
+whose double backward is closed form because the critic is piecewise linear (_d_grad_wgp, DESIGN.md §6b).  variant="dra"
+(DRAGAN, src/dra_gan.py:174-225) trains the same critic with a sigmoid output and the penalty at x_hat around the real data
+(dra_critic_grad); "ra" and "fisher" (src/ra_gan.py:204-205, src/fisher_gan.py:214-223) keep the batch-norm D and run
+their batch statistics in separate loss passes that stats_reduce can sum over data-parallel ranks.
 
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
@@ -122,8 +125,8 @@ class DcganEngine:
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls", "wgp") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*) and wgp")
+        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp and dra")
         if variant == "wgp":
             # WGAN-GP critic: no BatchNorm (one sample's input gradient must not depend on the batch, WGAN-GP paper §4),
             # output relu(s) as src/w_gp_gan.py:61 or the linear s
@@ -131,13 +134,18 @@ class DcganEngine:
             if d_out_act not in ("relu", "none"):
                 raise GmError("the WGAN-GP conv critic's output is relu or none")
         elif d_out_act not in (None, "sigmoid"):
-            raise GmError("the conv discriminator of the row-wise losses ends in a sigmoid")
+            raise GmError("the conv discriminator of the %s loss ends in a sigmoid" % variant)
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
         self.h = _lib.ctx(self.device.index)
         self.hd, self.z, self.ch, self.variant = hidden_dim, z_dim, channels, variant
         self.d_out_act = d_out_act or "sigmoid"
-        self.d_bn = variant != "wgp"                             # BatchNorm in D's layers 2-4
-        self.gp_lambda = 10.0                                    # LAMBDA of src/w_gp_gan.py:177
+        self.d_bn = variant not in ("wgp", "dra")                # BatchNorm in D's layers 2-4; the penalised critics have none
+        self.gp_lambda = 10.0                                    # LAMBDA of src/w_gp_gan.py:177, src/dra_gan.py:174
+        self.gp_k, self.dra_c = 1.0, 1.0                         # K, C of src/dra_gan.py:174
+        self.fisher = torch.tensor([0.0, 1e-6], device=self.device)   # Fisher's (LAMBDA, RHO), src/fisher_gan.py:117-118
+        # stats_reduce(buf): SUM a float64 statistic buffer over the data-parallel ranks in place (RaNS / Fisher loss
+        # moments, DRAGAN's image std); None on one process.  stat_batch (d_grad) is then the global batch.
+        self.stats_reduce = None
         self.zp = (z_dim + 1 + 7) // 8 * 8                       # noise rows: [z | 1 | pad], 16-byte rows
         hd = hidden_dim
         self.gc = [8 * hd, 4 * hd, 2 * hd, hd, channels]        # generator channels after each layer
@@ -158,7 +166,7 @@ class DcganEngine:
         self.run_D = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4) if self.d_bn}
         for r in list(self.run_G.values()) + list(self.run_D.values()):
             r[1].fill_(1.0)
-        self.loss_buf = torch.zeros(2, device=self.device)
+        self.loss_buf = torch.zeros(4, device=self.device)      # [D loss, G loss, loss-kernel scratch (sum ds, ..)]
         self._bufs = {}
         self.init_weights()
 
@@ -366,18 +374,61 @@ class DcganEngine:
         x = images.view(n, self.ch, 64, 64).permute(0, 2, 3, 1).to(torch.bfloat16).contiguous()
         return x.view(n * 4096, self.ch)
 
+    # the per-row loss each variant's rows share: WGAN-GP's are W's and DRAGAN's NS's (the penalty is separate); the G steps of
+    # RaNS and Fisher are NS's and W's -mean(D(G(z))) (src/ra_gan.py, src/fisher_gan.py train_G)
+    _ROW_LOSS = {"wgp": "w", "dra": "ns", "ra": "ns", "fisher": "w"}
+
     def _loss_rows(self, logits, n, g_step, inv, ds, loss):
-        variant = VARIANTS["w" if self.variant == "wgp" else self.variant]       # WGAN-GP's rows are W's; the penalty is separate
+        variant = VARIANTS[self._ROW_LOSS.get(self.variant, self.variant)]
         check(self.h, lib().gm_loss_rows(self.h, variant, OUT_ACTS[self.d_out_act], _ptr(logits), n, g_step, inv, _ptr(ds), None,
                                          loss, _stream()))
 
-    def d_grad(self, img_real, n, noise=None, inv_global_batch=None, seed=0, step=0, gp_lambda=None, eps=None):
-        """train_D + backward (src/ns_gan.py:172-194,138; src/w_gp_gan.py:177-220 for variant wgp): img_real NHWC rows of n
-        images (stage_images).  Writes the flat D gradient (self.D.grads) and loss_buf[0].  WGAN-GP only: gp_lambda (None =
-        self.gp_lambda) and eps [n] fp32 (None = on-device Philox keyed by (seed, step))."""
+    def _reduce_stats(self, buf):
+        if self.stats_reduce is not None:
+            self.stats_reduce(buf)
+
+    def fisher_state(self, lam=None, rho=None):
+        """Fisher GAN's multiplier and penalty weight (LAMBDA, RHO) on the device: set (both given) or read"""
+        if lam is not None:
+            self.fisher.copy_(torch.tensor([float(lam), float(rho)]))
+            return float(lam), float(rho)
+        lam, rho = self.fisher.tolist()
+        return lam, rho
+
+    def loss_stats(self, logits, n, stat_batch, stats):
+        """RaNS / Fisher statistics of the D-step logits [real n | fake n] into stats (float64 [8]): phase 0, the ranks'
+        sum, then (RaNS) phase 1 on the global phase-0 sums and its sum"""
+        v = VARIANTS[self.variant]
+        check(self.h, lib().gm_loss_stats(self.h, v, OUT_ACTS[self.d_out_act], _ptr(logits), n, stat_batch, 0, None, _ptr(stats), _stream()))
+        self._reduce_stats(stats[:4])
+        if self.variant == "ra":
+            check(self.h, lib().gm_loss_stats(self.h, v, OUT_ACTS[self.d_out_act], _ptr(logits), n, stat_batch, 1, _ptr(stats),
+                                              _ptr(stats[4:]), _stream()))
+            self._reduce_stats(stats[4:])
+
+    def loss_rows_stats(self, logits, n, stat_batch, stats, inv, ds, loss):
+        """pass 2 of the RaNS / Fisher D loss on global statistics: ds [2n], loss [4] ([0] the D loss, [2] Fisher's Omega);
+        Fisher's LAMBDA (self.fisher[0]) moves by -RHO Omega"""
+        check(self.h, lib().gm_loss_rows_stats(self.h, VARIANTS[self.variant], OUT_ACTS[self.d_out_act], _ptr(logits), n, inv, _ptr(stats),
+                                               stat_batch, _ptr(self.fisher), _ptr(ds), None, _ptr(loss), _stream()))
+
+    def d_grad(self, img_real, n, noise=None, inv_global_batch=None, seed=0, step=0, gp_lambda=None, eps=None, gp_k=None, dra_c=None,
+               delta=None, u=None, stat_batch=None):
+        """train_D + backward (src/ns_gan.py:172-194,138; src/w_gp_gan.py:177-220 for wgp, src/dra_gan.py:174-225 for dra,
+        src/ra_gan.py:186-207 for ra, src/fisher_gan.py:193-229 for fisher): img_real NHWC rows of n images (stage_images).
+        Writes the flat D gradient (self.D.grads) and loss_buf[0].  WGAN-GP and DRAGAN: gp_lambda (None = self.gp_lambda).
+        WGAN-GP: eps [n] fp32 (None = on-device Philox keyed by (seed, step)).  DRAGAN: gp_k, dra_c (None = self.gp_k,
+        self.dra_c), delta [n] and u [n, ch*64*64] (the reference's NCHW-flattened layout) or None for Philox.  RaNS, Fisher
+        and DRAGAN: stat_batch = the batch the statistics run over (None = n; the global batch under stats_reduce)."""
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
+        lam = self.gp_lambda if gp_lambda is None else float(gp_lambda)
+        stat_batch = n if stat_batch is None else int(stat_batch)
         if self.variant == "wgp":
-            return self._d_grad_wgp(img_real, n, noise, inv, seed, step, self.gp_lambda if gp_lambda is None else float(gp_lambda), eps)
+            return self._d_grad_wgp(img_real, n, noise, inv, seed, step, lam, eps)
+        if self.variant == "dra":
+            fake, _ = self.g_forward(n, noise, seed, 2 * step)
+            return self.dra_critic_grad(img_real, fake, n, inv, lam, self.gp_k if gp_k is None else float(gp_k),
+                                        self.dra_c if dra_c is None else float(dra_c), delta, u, seed, step, stat_batch)
         fake, gsv = self.g_forward(n, noise, seed, 2 * step)
         lr_, lf_ = self._buf("logits_r", 16, n, torch.float32), self._buf("logits_f", 16, n, torch.float32)
         sr = self.d_forward(img_real, n, lr_, "dr")
@@ -386,8 +437,16 @@ class DcganEngine:
         logits[:n].copy_(lr_[0])
         logits[n:].copy_(lf_[0])
         ds = self._buf("ds", 1, 2 * n, torch.float32)[0]
-        check(self.h, lib().gm_loss_rows(self.h, VARIANTS[self.variant], 0, _ptr(logits), n, 0, inv, _ptr(ds), None,
-                                         _ptr(self.loss_buf), _stream()))
+        if self.variant in ("ra", "fisher"):
+            stats = self._buf("loss_stats", 1, 8, torch.float64)[0]
+            lossv = self._buf("loss_stat_out", 1, 4, torch.float32)[0]
+            self.loss_stats(logits, n, stat_batch, stats)
+            self.loss_rows_stats(logits, n, stat_batch, stats, inv, ds, lossv)
+            self.loss_buf[0].copy_(lossv[0])
+            self.loss_stats_, self.fisher_omega_ = stats, lossv[2]
+        else:
+            check(self.h, lib().gm_loss_rows(self.h, VARIANTS[self.variant], 0, _ptr(logits), n, 0, inv, _ptr(ds), None,
+                                             _ptr(self.loss_buf), _stream()))
         g2 = self._buf("dgrad2", 1, self.D.total, torch.float32)[0]
         self.D.grads.zero_()
         g2.zero_()
@@ -406,33 +465,78 @@ class DcganEngine:
 
     def wgp_critic_grad(self, img_real, fake, n, inv, lam, eps=None, seed=0, step=0):
         """The critic half of _d_grad_wgp for given real and generated NHWC image rows (data-parallel splits, tests)."""
-        dc, D, ch = self.dc, self.D, self.ch
         R = n * 4096
-        x3 = self._buf("gp_x3", 3 * R, ch)                                  # NHWC rows [real | fake | x_hat]
+        x3 = self._buf("gp_x3", 3 * R, self.ch)                             # NHWC rows [real | fake | x_hat]
         x3[:R].copy_(img_real)
         x3[R:2 * R].copy_(fake)
         eps_used = self._buf("gp_eps", 1, n, torch.float32)[0]
         if eps is not None:
             eps = eps.reshape(n).float().contiguous()
-        check(self.h, lib().gm_gp_interp_rows(self.h, _ptr(x3), ch, _ptr(x3[R:]), ch, n, 4096, ch, _ptr(eps), _ptr(eps_used),
-                                              int(seed), int(2 * step), _ptr(x3[2 * R:]), ch, _stream()))
+        check(self.h, lib().gm_gp_interp_rows(self.h, _ptr(x3), self.ch, _ptr(x3[R:]), self.ch, n, 4096, self.ch, _ptr(eps), _ptr(eps_used),
+                                              int(seed), int(2 * step), _ptr(x3[2 * R:]), self.ch, _stream()))
+        self.gp_eps_ = eps_used
+        return self._penalised_critic_grad(x3, n, inv, lam)
+
+    def dra_std_sums(self, img_real, n, sums):
+        """this process's (sum x, sum x^2) of the real images (NHWC rows of n images) into sums (float64 [2])"""
+        cols = 4096 * self.ch
+        check(self.h, lib().gm_dra_std_sums(self.h, _ptr(img_real), n, cols, cols, _ptr(sums), _stream()))
+
+    def dra_critic_grad(self, img_real, fake, n, inv, lam, K=1.0, C=1.0, delta=None, u=None, seed=0, step=0, stat_batch=None):
+        """The critic half of the DRAGAN D step (src/dra_gan.py:174-225) for given real and generated NHWC image rows:
+        x_hat = delta x + (1 - delta)(x + C std(x) u) around the real data, std over the stat_batch images behind
+        stats_reduce, then the NS rows on real / fake and the penalty lam mean (||grad sigmoid(D(x_hat))|| - K)^2."""
+        R, cols = n * 4096, 4096 * self.ch
+        x3 = self._buf("gp_x3", 3 * R, self.ch)                             # NHWC rows [real | fake | x_hat]
+        x3[:R].copy_(img_real)
+        x3[R:2 * R].copy_(fake)
+        sums = self._buf("dra_sums", 1, 2, torch.float64)[0]
+        self.dra_std_sums(x3[:R], n, sums)
+        self._reduce_stats(sums)
+        rnd = None
+        if delta is not None or u is not None:
+            if delta is None or u is None:
+                raise GmError("DRAGAN's delta and u are given together or not at all")
+            u = u.reshape(n, self.ch, 64, 64).permute(0, 2, 3, 1).reshape(-1)       # NCHW-flattened -> the NHWC rows' order
+            rnd = torch.cat([delta.reshape(n).float(), u.float()]).to(self.device).contiguous()
+        count = float(n if stat_batch is None else stat_batch) * cols
+        check(self.h, lib().gm_dra_xhat_rows(self.h, _ptr(x3), n, cols, cols, _ptr(sums), count, float(C), _ptr(rnd), int(seed), int(2 * step),
+                                             _ptr(x3[2 * R:]), cols, _stream()))
+        self.dra_sums_ = sums
+        return self._penalised_critic_grad(x3, n, inv, lam, K)
+
+    def _penalised_critic_grad(self, x3, n, inv, lam, K=1.0):
+        """The D gradient of a batch-norm-free critic with a gradient penalty at x_hat (DESIGN.md §6b) from the stacked NHWC
+        rows x3 = [real | fake | x_hat] of n images each.  WGAN-GP: W rows, relu / linear output, penalty on ||grad D||;
+        DRAGAN: NS rows on the sigmoid output, penalty on ||grad sigmoid(s)|| = sigma' ||grad s|| with target K."""
+        dc, D, ch = self.dc, self.D, self.ch
+        R = n * 4096
+        dra = self.variant == "dra"
         # 1. primal forward of the 3n images; the LeakyReLU outputs y_l carry the masks
         logits = self._buf("gp_logits", 16, 3 * n, torch.float32)
         sv = self.d_forward(x3, 3 * n, logits, "dw")
-        # 2. upstream dL/dlogit: the W rows for real / fake (loss_buf[0] = mean(DG) - mean(DX)), and the penalty's seed
-        #    1[s > 0] (relu output) or 1 for x_hat: the loss kernel's train_G row (-d, gradient -act'(s) * inv) with inv = -1
+        # 2. upstream dL/dlogit: the loss rows for real / fake (loss_buf[0]), and the x_hat rows' seed - WGAN-GP: 1[s > 0]
+        #    (relu output) or 1, the loss kernel's train_G row (-d, gradient -act'(s) * inv) with inv = -1; DRAGAN: 1, so
+        #    that the chain below is J = ds/dx_hat and the sigmoid enters through the penalty kernel
         ds = self._buf("gp_ds", 1, 3 * n, torch.float32)[0]
         self._loss_rows(logits[0], n, 0, inv, ds, _ptr(self.loss_buf))
-        self._loss_rows(logits[0, 2 * n:], n, 1, -1.0, ds[2 * n:], _ptr(self._buf("gp_seed_loss", 1, 4, torch.float32)))
+        if dra:
+            ds[2 * n:].fill_(1.0)
+        else:
+            self._loss_rows(logits[0, 2 * n:], n, 1, -1.0, ds[2 * n:], _ptr(self._buf("gp_seed_loss", 1, 4, torch.float32)))
         dy5 = self._buf("dwdy5", 3 * n, 16)
         check(self.h, lib().gm_pack_col0(self.h, _ptr(ds), 3 * n, _ptr(dy5), 16, _stream()))
         betas = self._betas(sv, dy5, "dw")
-        # 2b. image gradient g at x_hat and 3. the penalty: loss_buf[0] += lam mean (||g|| - 1)^2, tangent seed r = dP/dg
+        # 2b. image gradient g at x_hat and 3. the penalty: loss_buf[0] += lam mean (||g|| - K)^2, tangent seed r
         g = self._dimg(sv, betas[0][2 * n * 1024:], "gp", C2I_NONE)
         r = self._buf("gp_r", R, ch)
         norms = self._buf("gp_norm", 1, n, torch.float32)[0]
-        check(self.h, lib().gm_gp_penalty(self.h, _ptr(g), ch, n, 4096, ch, lam, inv, 1.0 / n, _ptr(r), ch, _ptr(norms),
-                                          _ptr(self.loss_buf), _stream()))
+        if dra:
+            check(self.h, lib().gm_dra_penalty(self.h, _ptr(g), ch, _ptr(x3[2 * R:]), ch, _ptr(logits[0, 2 * n:]), n, 4096, ch, lam, K, inv,
+                                               1.0 / n, _ptr(r), ch, _ptr(norms), _ptr(self.loss_buf), _stream()))
+        else:
+            check(self.h, lib().gm_gp_penalty(self.h, _ptr(g), ch, n, 4096, ch, lam, inv, 1.0 / n, _ptr(r), ch, _ptr(norms),
+                                              _ptr(self.loss_buf), _stream()))
         # 4. tangent pass t_0 = r, t_l = LReLU'(y_l) * conv_l(t_{l-1}) under x_hat's masks.  im2col(t_{l-1}) overwrites
         #    x_hat's rows of the saved column matrices (and t_4 x_hat's rows of y_4 = the last layer's input), so that
         # 5. each layer's weight gradient is ONE GEMM over the 3n images: W part (activations) + penalty (tangents).
@@ -453,7 +557,7 @@ class DcganEngine:
         for i in range(4):
             gemm_bf16(betas[i], sv["col%d" % i], D.view("l%d.weight" % (i + 1), D.grads), "tn")
         self.scores_ = logits[0, :2 * n]
-        self.gp_norms_, self.gp_eps_ = norms, eps_used                      # per-image ||g|| and eps of this step
+        self.gp_norms_, self.gp_logits_, self.gp_r_ = norms, logits[0, 2 * n:], r   # per-image ||g||, x_hat logits, tangent seed
         return self.loss_buf[0]
 
     def g_grad(self, n, noise=None, inv_global_batch=None, seed=0, step=0):

@@ -341,6 +341,31 @@ int gm_im2col_k4s2_lrelu_mask(gm_ctx* ctx, const void* x_dev, int B, int H, int 
 /* out = x * LeakyReLU'(m) over rows [rows, C]; C a multiple of 8; out may alias x or m */
 int gm_lrelu_mask_rows(gm_ctx* ctx, const void* x_dev, int ldx, const void* m_dev, int ldm, long long rows, int C, float slope,
                        void* out_dev, int ldo, gm_stream stream);
+/* Batch-statistic D losses (RaNS src/ra_gan.py:204-205, Fisher src/fisher_gan.py:214-223) on a logit vector [real B | fake B],
+ * split so that data-parallel ranks can SUM the statistics between the calls.  bstat = the global batch the statistics run
+ * over (B x ranks).  stats: 8 doubles, [0..3] = phase 0 (sum d real, sum d fake, sum d^2 real, sum d^2 fake), [4] = phase 1
+ * (RaNS: sum over the real rows of q(1-q)/(q+1e-8), q = sigmoid(d - mean d_fake), given the global phase-0 sums in
+ * stats_in_dev).  gm_loss_rows_stats then writes ds_dev[2B] = dL/dlogit (scaled by inv_global_batch), d_out_dev (nullable),
+ * loss_dev[0] = loss (local means, global statistics), [1] = sum ds, [2] = Fisher's Omega, and for Fisher updates
+ * fisher_state_dev[0] (lambda) by -rho Omega with fisher_state_dev[1] = rho (src/fisher_gan.py:155). */
+int gm_loss_stats(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, long long bstat, int phase,
+                  const double* stats_in_dev, double* stats_out_dev, gm_stream stream);
+int gm_loss_rows_stats(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, float inv_global_batch,
+                       const double* stats_dev, long long bstat, float* fisher_state_dev, float* ds_dev, float* d_out_dev,
+                       float* loss_dev, gm_stream stream);
+/* DRAGAN (src/dra_gan.py:200-219) on contiguous image rows [rows, cols] (cols a multiple of 8, 16-byte aligned).
+ * gm_dra_std_sums: sums_dev[2] = (sum x, sum x^2) of this process's rows.  gm_dra_xhat_rows: with the global sums and their
+ * element count, x_hat = delta x + (1 - delta)(x + C std(x) u) (std unbiased); rnd_dev = [delta (rows) | u (rows x cols, the
+ * rows' own element order)] or NULL for Philox keyed by (seed, stream_id).  gm_dra_penalty: per x_hat image b with logit
+ * s_b and J_b = d s_b / d image: norm_dev[b] = ||g_b|| = sigma'(s_b) ||J_b||, the tangent seed
+ * r_b = k sigma' [J_b/||J_b|| + (1 - 2 sigma) ||J_b|| x_hat_b], k = 2 lambda inv_grad (||g_b|| - K) (0 when ||J_b|| = 0), and
+ * loss_dev[0] += lambda inv_loss sum_b (||g_b|| - K)^2 (loss_dev nullable). */
+int gm_dra_std_sums(gm_ctx* ctx, const void* x_dev, int rows, int cols, int ld, double* sums_dev, gm_stream stream);
+int gm_dra_xhat_rows(gm_ctx* ctx, const void* x_dev, int rows, int cols, int ld, const double* sums_dev, double count, float dra_c,
+                     const float* rnd_dev, uint64_t seed, uint64_t stream_id, void* out_dev, int ldo, gm_stream stream);
+int gm_dra_penalty(gm_ctx* ctx, const void* J_dev, int ldj, const void* xhat_dev, int ldx, const float* logits_dev, int B, int HW, int C,
+                   float lambda, float K, float inv_grad, float inv_loss, void* r_dev, int ldr, float* norm_dev, float* loss_dev,
+                   gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);

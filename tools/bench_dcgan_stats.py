@@ -1,0 +1,82 @@
+"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP and DRAGAN steps (D_steps = 1) on one GPU, in one process.
+
+    python tools/bench_dcgan_stats.py [--batch 1024] [--steps 20] [--warmup 5]
+
+Every engine runs the DCGAN of bench.py's dcgan workload (64x64x3, hidden 64, z 100) on device-resident synthetic images.
+The steps alternate (rounds of one step per variant, each timed with its own CUDA events after the warm-up), so clock or
+thermal drift hits all alike.  Prints one JSON line: device name and power limit (read in the same run), and per variant
+the median step time, images/s, library launches per step and the ratio to NSGAN.  Writes nothing but stdout.
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "generative-models_b200"), os.path.join(ROOT, "tools")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+from bench_dcgan_wgp import power_limit  # noqa: E402
+
+VARIANTS = ("ns", "ra", "fisher", "wgp", "dra")
+LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4}     # the reference's defaults per variant
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=1024)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    a = ap.parse_args()
+    import torch
+    import gm_b200
+    dev = torch.cuda.current_device()
+    B = a.batch
+    g = torch.Generator(device="cuda").manual_seed(77)
+    pool = torch.rand(2 * B * 4096, 3, device="cuda", generator=g).to(torch.bfloat16)
+    engines = {v: gm_b200.DcganEngine(64, 100, 3, variant=v) for v in VARIANTS}
+    hps = {v: gm_b200.AdamHP.make(LR[v]) for v in VARIANTS}
+
+    def step(name, s):
+        eng, hp = engines[name], hps[name]
+        x = pool[(s % 2) * B * 4096:(s % 2 + 1) * B * 4096]
+        eng.d_grad(x, B, seed=1000, step=s)
+        eng.apply(1, hp)
+        eng.g_grad(B, seed=1000, step=s)
+        eng.apply(0, hp)
+
+    launches = {}
+    for name in VARIANTS:
+        step(name, 0)
+        torch.cuda.synchronize()
+        gm_b200.launch_count(reset=True)
+        step(name, 1)
+        torch.cuda.synchronize()
+        launches[name] = gm_b200.launch_count(reset=True)
+    for s in range(a.warmup):
+        for name in VARIANTS:
+            step(name, 2 + s)
+    torch.cuda.synchronize()
+    ms = {name: [] for name in VARIANTS}
+    for s in range(a.steps):
+        for name in VARIANTS:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            step(name, 100 + s)
+            e1.record()
+            e1.synchronize()
+            ms[name].append(e0.elapsed_time(e1))
+    out = {"device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit(dev), "batch": B, "steps": a.steps,
+           "warmup": a.warmup}
+    for name in VARIANTS:
+        med = sorted(ms[name])[len(ms[name]) // 2]
+        out[name] = {"median_ms": round(med, 3), "min_ms": round(min(ms[name]), 3), "images_per_s": round(B / med * 1e3, 1),
+                     "launches_per_step": launches[name], "last_d_loss": float(engines[name].loss_buf[0])}
+    for name in VARIANTS[1:]:
+        out[name]["over_ns_images_per_s"] = round(out[name]["images_per_s"] / out["ns"]["images_per_s"], 3)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
