@@ -20,37 +20,22 @@ import torch.nn as nn  # noqa: F401
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
 from gm_b200.gan_api import to_cuda
-from dc_gan import Generator, DCGANTrainer
+from dc_gan import Generator, DCGAN, DCGANTrainer  # noqa: F401
 from dc_w_gp_gan import Discriminator as _Critic
 
 
 class Discriminator(_Critic):
     """ 64x64 -> 32x32 -> 16x16 -> 8x8 -> 4x4 -> 1 (convolutions + LeakyReLU(0.2), no BatchNorm, sigmoid output): the
     WGAN-GP critic's layers with src/dra_gan.py:59's sigmoid """
+    out_acts = ("sigmoid",)
 
     def __init__(self, image_size, hidden_dim, output_dim=1, channels=3):
-        super().__init__(image_size, hidden_dim, output_dim, channels, out_act="none")
-        self.out_act = "sigmoid"
+        super().__init__(image_size, hidden_dim, output_dim, channels, out_act="sigmoid")
 
 
-class DCDRAGAN(nn.Module):
+class DCDRAGAN(DCGAN):
     """ Super class to contain both Discriminator (D) and Generator (G) (as src/dra_gan.py:63-74) """
-
-    def __init__(self, image_size=64 * 64 * 3, hidden_dim=64, z_dim=100, output_dim=1, channels=3):
-        super().__init__()
-        if image_size != 64 * 64 * channels:
-            raise GmError("the conv path is built for 64x64 images (image_size = 64*64*channels)")
-        self.__dict__.update(dict(image_size=image_size, hidden_dim=hidden_dim, z_dim=z_dim, output_dim=output_dim,
-                                  channels=channels))
-        self.G = Generator(image_size, hidden_dim, z_dim, channels)
-        self.D = Discriminator(image_size, hidden_dim, output_dim, channels)
-        for m in self.modules():                                # DCGAN initialisation (Radford et al. 2015)
-            if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
-                nn.init.normal_(m.weight, 0.0, 0.02)
-            elif isinstance(m, nn.BatchNorm2d):
-                nn.init.normal_(m.weight, 1.0, 0.02)
-                nn.init.zeros_(m.bias)
-        self.shape = 64
+    _D = Discriminator
 
 
 class DCDRAGANTrainer(DCGANTrainer):

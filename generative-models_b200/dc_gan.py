@@ -47,39 +47,47 @@ class Generator(nn.Module):
 
 
 class Discriminator(nn.Module):
-    """ 64x64 -> 32x32 -> 16x16 -> 8x8 -> 4x4 -> 1 (convolutions, BatchNorm + LeakyReLU(0.2), sigmoid output) """
+    """ 64x64 -> 32x32 -> 16x16 -> 8x8 -> 4x4 -> 1 (convolutions + LeakyReLU(0.2), BatchNorm on layers 2-4 unless
+    batch_norm=False, output activation out_act: one of the class's out_acts) """
+    out_acts = ("sigmoid",)
 
-    def __init__(self, image_size, hidden_dim, output_dim=1, channels=3):
+    def __init__(self, image_size, hidden_dim, output_dim=1, channels=3, batch_norm=True, out_act="sigmoid"):
         super().__init__()
         if output_dim != 1:
             raise GmError("only output_dim=1 discriminators are built")
+        if out_act not in self.out_acts:
+            raise GmError("the output activation of %s is one of %s" % (type(self).__name__, ", ".join(self.out_acts)))
         c = [hidden_dim, 2 * hidden_dim, 4 * hidden_dim, 8 * hidden_dim]
         self.l1 = nn.Conv2d(channels, c[0], 4, 2, 1, bias=False)
         self.l2 = nn.Conv2d(c[0], c[1], 4, 2, 1, bias=False)
         self.l3 = nn.Conv2d(c[1], c[2], 4, 2, 1, bias=False)
         self.l4 = nn.Conv2d(c[2], c[3], 4, 2, 1, bias=False)
         self.l5 = nn.Conv2d(c[3], 1, 4, 1, 0, bias=False)
-        self.bn2, self.bn3, self.bn4 = (nn.BatchNorm2d(k) for k in c[1:])
+        if batch_norm:
+            self.bn2, self.bn3, self.bn4 = (nn.BatchNorm2d(k) for k in c[1:])
+        self.out_act = out_act
         self._owner = None
 
     def forward(self, x):
         tr = self._owner
         if tr is None:
-            raise GmError("Discriminator is not attached to a CUDA engine yet: construct the DCGANTrainer first")
+            raise GmError("Discriminator is not attached to a CUDA engine yet: construct its trainer first")
         return tr._engine_synced().discriminate(to_cuda(x).float().reshape(x.shape[0], -1))
 
 
 class DCGAN(nn.Module):
-    """ Super class to contain both Discriminator (D) and Generator (G) (as src/ns_gan.py:63-74) """
+    """ Super class to contain both Discriminator (D) and Generator (G) (as src/ns_gan.py:63-74).  A subclass names its
+    discriminator class in _D; d_options are that class's keyword options (e.g. the WGAN-GP critic's out_act). """
+    _D = Discriminator
 
-    def __init__(self, image_size=64 * 64 * 3, hidden_dim=64, z_dim=100, output_dim=1, channels=3):
+    def __init__(self, image_size=64 * 64 * 3, hidden_dim=64, z_dim=100, output_dim=1, channels=3, **d_options):
         super().__init__()
         if image_size != 64 * 64 * channels:
             raise GmError("the conv path is built for 64x64 images (image_size = 64*64*channels)")
         self.__dict__.update(dict(image_size=image_size, hidden_dim=hidden_dim, z_dim=z_dim, output_dim=output_dim,
                                   channels=channels))
         self.G = Generator(image_size, hidden_dim, z_dim, channels)
-        self.D = Discriminator(image_size, hidden_dim, output_dim, channels)
+        self.D = self._D(image_size, hidden_dim, output_dim, channels, **d_options)
         for m in self.modules():                                # DCGAN initialisation (Radford et al. 2015)
             if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
                 nn.init.normal_(m.weight, 0.0, 0.02)
@@ -115,14 +123,10 @@ class DCGANTrainer:
                 out["%s.%s" % (tag, k)] = v.detach()
         return out
 
-    def _engine_kwargs(self):
-        """extra DcganEngine arguments of a subclass (e.g. the critic's output activation)"""
-        return {}
-
     def _engine_synced(self):
         m = self.model
         if self._engine is None:
-            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, **self._engine_kwargs())
+            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, d_out_act=m.D.out_act)
             self._dirty = True
         if self._dirty:
             self._engine.load_torch_weights(self._sd())
@@ -190,19 +194,10 @@ class DCGANTrainer:
 
     def _loss(self, net, loss_val):
         eng = self._engine
-        mod = self.model.G if net == 0 else self.model.D
-        enet = eng.G if net == 0 else eng.D
-        grads = []
-        for k, p in mod.named_parameters():                         # engine layout -> torch layout, per tensor
-            g = enet.view(k, enet.grads).detach()
-            if k.startswith("l"):
-                if net == 0:
-                    g = g.view(4, 4, p.shape[1], p.shape[0]).permute(3, 2, 0, 1)
-                else:
-                    g = g[: p.shape[0]].view(p.shape[0], 4, 4, -1).permute(0, 3, 1, 2)
-            grads.append(g.reshape(-1).to(p.device))
+        tag, mod = ("G", self.model.G) if net == 0 else ("D", self.model.D)
+        tg = eng.torch_grads()
         params = [p for _, p in mod.named_parameters()]
-        flat = torch.cat(grads)
+        flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for k, p in mod.named_parameters()])
         self._dirty = True                                            # the caller's optimizer will change the module parameters
         return _FusedLoss.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat, params)
 

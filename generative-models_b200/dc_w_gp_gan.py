@@ -14,65 +14,33 @@ out_act="none" in the identity.  Its gradient penalty runs as a closed-form doub
 gm_b200.DcganEngine(variant="wgp") (DESIGN.md §6b).  Under torchrun the trainer is data-parallel like DCGANTrainer.
 """
 import torch
-import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
 from gm_b200.gan_api import to_cuda
-from dc_gan import Generator, DCGANTrainer
+import dc_gan
+from dc_gan import Generator, DCGAN, DCGANTrainer  # noqa: F401
 
 
-class Discriminator(nn.Module):
+class Discriminator(dc_gan.Discriminator):
     """ Critic: 64x64 -> 32x32 -> 16x16 -> 8x8 -> 4x4 -> 1 (convolutions + LeakyReLU(0.2), no BatchNorm, relu / linear output) """
+    out_acts = ("relu", "none")
 
     def __init__(self, image_size, hidden_dim, output_dim=1, channels=3, out_act="relu"):
-        super().__init__()
-        if output_dim != 1:
-            raise GmError("only output_dim=1 critics are built")
-        if out_act not in ("relu", "none"):
-            raise GmError("the critic's output activation is relu (src/w_gp_gan.py:61) or none")
-        c = [hidden_dim, 2 * hidden_dim, 4 * hidden_dim, 8 * hidden_dim]
-        self.l1 = nn.Conv2d(channels, c[0], 4, 2, 1, bias=False)
-        self.l2 = nn.Conv2d(c[0], c[1], 4, 2, 1, bias=False)
-        self.l3 = nn.Conv2d(c[1], c[2], 4, 2, 1, bias=False)
-        self.l4 = nn.Conv2d(c[2], c[3], 4, 2, 1, bias=False)
-        self.l5 = nn.Conv2d(c[3], 1, 4, 1, 0, bias=False)
-        self.out_act = out_act
-        self._owner = None
-
-    def forward(self, x):
-        tr = self._owner
-        if tr is None:
-            raise GmError("Discriminator is not attached to a CUDA engine yet: construct the DCWGPGANTrainer first")
-        return tr._engine_synced().discriminate(to_cuda(x).float().reshape(x.shape[0], -1))
+        super().__init__(image_size, hidden_dim, output_dim, channels, batch_norm=False, out_act=out_act)
 
 
-class DCWGPGAN(nn.Module):
+class DCWGPGAN(DCGAN):
     """ Super class to contain both Discriminator (D) and Generator (G) (as src/w_gp_gan.py:65-76) """
+    _D = Discriminator
 
     def __init__(self, image_size=64 * 64 * 3, hidden_dim=64, z_dim=100, output_dim=1, channels=3, out_act="relu"):
-        super().__init__()
-        if image_size != 64 * 64 * channels:
-            raise GmError("the conv path is built for 64x64 images (image_size = 64*64*channels)")
-        self.__dict__.update(dict(image_size=image_size, hidden_dim=hidden_dim, z_dim=z_dim, output_dim=output_dim,
-                                  channels=channels))
-        self.G = Generator(image_size, hidden_dim, z_dim, channels)
-        self.D = Discriminator(image_size, hidden_dim, output_dim, channels, out_act)
-        for m in self.modules():                                # DCGAN initialisation (Radford et al. 2015)
-            if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
-                nn.init.normal_(m.weight, 0.0, 0.02)
-            elif isinstance(m, nn.BatchNorm2d):
-                nn.init.normal_(m.weight, 1.0, 0.02)
-                nn.init.zeros_(m.bias)
-        self.shape = 64
+        super().__init__(image_size, hidden_dim, z_dim, output_dim, channels, out_act=out_act)
 
 
 class DCWGPGANTrainer(DCGANTrainer):
     """ Object to hold data iterators, train the conv WGAN-GP (surface of src/w_gp_gan.py:79-315) """
     variant = "wgp"
-
-    def _engine_kwargs(self):
-        return dict(d_out_act=self.model.D.out_act)
 
     def train(self, num_epochs, G_lr=1e-4, D_lr=1e-4, D_steps=5):
         """ Trainer.train (src/w_gp_gan.py:96-175) with LAMBDA = 10 and eps drawn on the device per rank """

@@ -14,7 +14,7 @@ README cites (Radford et al. 2015) with the reference's sigmoid outputs:
 
 variant="wgp" (WGAN-GP, src/w_gp_gan.py:177-239) trains D as a critic without BatchNorm — LeakyReLU on conv 1-4, output
 relu(s) (src/w_gp_gan.py:61) or s (d_out_act="none") — and adds the gradient penalty at x_hat = eps x + (1 - eps) G(z),
-whose double backward is closed form because the critic is piecewise linear (_d_grad_wgp, DESIGN.md §6b).  variant="dra"
+whose double backward is closed form because the critic is piecewise linear (wgp_critic_grad, DESIGN.md §6b).  variant="dra"
 (DRAGAN, src/dra_gan.py:174-225) trains the same critic with a sigmoid output and the penalty at x_hat around the real data
 (dra_critic_grad); "ra" and "fisher" (src/ra_gan.py:204-205, src/fisher_gan.py:214-223) keep the batch-norm D and run
 their batch statistics in separate loss passes that stats_reduce can sum over data-parallel ranks.
@@ -24,7 +24,7 @@ GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNo
 same matrices, the loss is the MLP path's loss kernel on the conv D's logits (gm_loss_rows), Adam is gm_adam_step.
 This module only sequences those C-ABI calls and owns the buffers (host language of the reference: Python).
 Weights are kept in GEMM layout — conv [Cout, (kh, kw, ci)], transposed conv [(kh, kw, co), Cin] — and converted to /
-from torch's Conv2d / ConvTranspose2d layouts at the state_dict boundary (torch_weights / load_torch_weights).
+from torch's Conv2d / ConvTranspose2d layouts at the state_dict boundary (torch_weights / load_torch_weights / torch_grads).
 """
 import ctypes as C
 
@@ -187,36 +187,33 @@ class DcganEngine:
         self.G.refresh()
         self.D.refresh()
 
-    def torch_weights(self):
-        """{torch-style name: tensor in torch's Conv2d / ConvTranspose2d layout} (CPU fp32)."""
+    def _torch_views(self, which):
+        """{torch-style name: view of the G / D tensor in torch's layout} over the flat params (which="params") or grads.
+        Conv weights are [Cout, (kh, kw, ci)] here and [Cout, Cin, kh, kw] in torch (D.l5: output channel 0 of the 16 padded
+        rows); transposed-conv weights are [(kh, kw, co), Cin] here and [Cin, Cout, kh, kw] in torch; BatchNorm vectors match."""
         out = {}
-        for i in range(5):
-            w = self.G.view("l%d.weight" % (i + 1)).detach().cpu()
-            cout, cin = w.shape[0] // 16, w.shape[1]
-            out["G.l%d.weight" % (i + 1)] = w.view(4, 4, cout, cin).permute(3, 2, 0, 1).contiguous()    # [Cin, Cout, kh, kw]
-        for i in range(5):
-            w = self.D.view("l%d.weight" % (i + 1)).detach().cpu()
-            if i == 4:
-                w = w[:1]
-            cout, cin = w.shape[0], w.shape[1] // 16
-            out["D.l%d.weight" % (i + 1)] = w.view(cout, 4, 4, cin).permute(0, 3, 1, 2).contiguous()    # [Cout, Cin, kh, kw]
-        for net, tag in ((self.G, "G"), (self.D, "D")):
+        for tag, net in (("G", self.G), ("D", self.D)):
             for n in net.names:
-                if n.startswith("bn"):
-                    out["%s.%s" % (tag, n)] = net.view(n).detach().cpu().clone()
+                w = net.view(n, getattr(net, which))
+                if n.startswith("l") and tag == "G":
+                    w = w.view(4, 4, w.shape[0] // 16, w.shape[1]).permute(3, 2, 0, 1)
+                elif n.startswith("l"):
+                    w = w[:1] if n == "l5.weight" else w
+                    w = w.view(w.shape[0], 4, 4, w.shape[1] // 16).permute(0, 3, 1, 2)
+                out["%s.%s" % (tag, n)] = w
         return out
 
+    def torch_weights(self):
+        """{torch-style name: tensor in torch's Conv2d / ConvTranspose2d / BatchNorm2d layout} (CPU fp32)."""
+        return {k: v.detach().cpu().contiguous() for k, v in self._torch_views("params").items()}
+
+    def torch_grads(self):
+        """{torch-style name: the current G / D gradient in torch's layout} (views of the device gradients)."""
+        return self._torch_views("grads")
+
     def load_torch_weights(self, sd):
-        for i in range(5):
-            w = sd["G.l%d.weight" % (i + 1)].float()
-            self.G.view("l%d.weight" % (i + 1)).copy_(w.permute(2, 3, 1, 0).reshape(-1, w.shape[0]))
-            w = sd["D.l%d.weight" % (i + 1)].float()
-            v = self.D.view("l%d.weight" % (i + 1))
-            v[: w.shape[0]].copy_(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1))
-        for net, tag in ((self.G, "G"), (self.D, "D")):
-            for n in net.names:
-                if n.startswith("bn"):
-                    net.view(n).copy_(sd["%s.%s" % (tag, n)].float())
+        for k, v in self._torch_views("params").items():
+            v.copy_(sd[k].float())
         self.G.refresh()
         self.D.refresh()
 
@@ -423,13 +420,12 @@ class DcganEngine:
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         lam = self.gp_lambda if gp_lambda is None else float(gp_lambda)
         stat_batch = n if stat_batch is None else int(stat_batch)
+        fake, _ = self.g_forward(n, noise, seed, 2 * step)
         if self.variant == "wgp":
-            return self._d_grad_wgp(img_real, n, noise, inv, seed, step, lam, eps)
+            return self.wgp_critic_grad(img_real, fake, n, inv, lam, eps, seed, step)
         if self.variant == "dra":
-            fake, _ = self.g_forward(n, noise, seed, 2 * step)
             return self.dra_critic_grad(img_real, fake, n, inv, lam, self.gp_k if gp_k is None else float(gp_k),
                                         self.dra_c if dra_c is None else float(dra_c), delta, u, seed, step, stat_batch)
-        fake, gsv = self.g_forward(n, noise, seed, 2 * step)
         lr_, lf_ = self._buf("logits_r", 16, n, torch.float32), self._buf("logits_f", 16, n, torch.float32)
         sr = self.d_forward(img_real, n, lr_, "dr")
         sf = self.d_forward(fake, n, lf_, "df")
@@ -445,8 +441,7 @@ class DcganEngine:
             self.loss_buf[0].copy_(lossv[0])
             self.loss_stats_, self.fisher_omega_ = stats, lossv[2]
         else:
-            check(self.h, lib().gm_loss_rows(self.h, VARIANTS[self.variant], 0, _ptr(logits), n, 0, inv, _ptr(ds), None,
-                                             _ptr(self.loss_buf), _stream()))
+            self._loss_rows(logits, n, 0, inv, ds, _ptr(self.loss_buf))
         g2 = self._buf("dgrad2", 1, self.D.total, torch.float32)[0]
         self.D.grads.zero_()
         g2.zero_()
@@ -456,19 +451,20 @@ class DcganEngine:
         self.scores_ = logits
         return self.loss_buf[0]
 
-    def _d_grad_wgp(self, img_real, n, noise, inv, seed, step, lam, eps):
-        """D_loss = mean(D(G(z))) - mean(D(x)) + lam mean_b (||grad D(x_hat_b)|| - 1)^2 and its D gradient (src/w_gp_gan.py:
-        186-218), the penalty's double backward in closed form (DESIGN.md §6b).  The critic has no BatchNorm, so real, fake
-        and x_hat images go through ONE forward and ONE input-gradient chain as 3n stacked images."""
-        fake, _ = self.g_forward(n, noise, seed, 2 * step)
-        return self.wgp_critic_grad(img_real, fake, n, inv, lam, eps, seed, step)
-
-    def wgp_critic_grad(self, img_real, fake, n, inv, lam, eps=None, seed=0, step=0):
-        """The critic half of _d_grad_wgp for given real and generated NHWC image rows (data-parallel splits, tests)."""
+    def _stack_x3(self, img_real, fake, n):
+        """NHWC rows [real | fake | x_hat] of n images each for the penalised critics; the caller writes x_hat's rows"""
         R = n * 4096
-        x3 = self._buf("gp_x3", 3 * R, self.ch)                             # NHWC rows [real | fake | x_hat]
+        x3 = self._buf("gp_x3", 3 * R, self.ch)
         x3[:R].copy_(img_real)
         x3[R:2 * R].copy_(fake)
+        return x3
+
+    def wgp_critic_grad(self, img_real, fake, n, inv, lam, eps=None, seed=0, step=0):
+        """The critic half of the WGAN-GP D step for given real and generated NHWC image rows: D_loss = mean(D(G(z))) -
+        mean(D(x)) + lam mean_b (||grad D(x_hat_b)|| - 1)^2 at x_hat = eps x + (1 - eps) G(z) (src/w_gp_gan.py:186-218),
+        the penalty's double backward in closed form (DESIGN.md §6b)."""
+        R = n * 4096
+        x3 = self._stack_x3(img_real, fake, n)
         eps_used = self._buf("gp_eps", 1, n, torch.float32)[0]
         if eps is not None:
             eps = eps.reshape(n).float().contiguous()
@@ -487,9 +483,7 @@ class DcganEngine:
         x_hat = delta x + (1 - delta)(x + C std(x) u) around the real data, std over the stat_batch images behind
         stats_reduce, then the NS rows on real / fake and the penalty lam mean (||grad sigmoid(D(x_hat))|| - K)^2."""
         R, cols = n * 4096, 4096 * self.ch
-        x3 = self._buf("gp_x3", 3 * R, self.ch)                             # NHWC rows [real | fake | x_hat]
-        x3[:R].copy_(img_real)
-        x3[R:2 * R].copy_(fake)
+        x3 = self._stack_x3(img_real, fake, n)
         sums = self._buf("dra_sums", 1, 2, torch.float64)[0]
         self.dra_std_sums(x3[:R], n, sums)
         self._reduce_stats(sums)

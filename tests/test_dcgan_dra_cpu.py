@@ -1,17 +1,17 @@
 """DRAGAN, RaNSGAN and Fisher GAN on the DCGAN conv path, CPU side: the closed-form DRAGAN D gradient (tangent seed r,
-shared weight-gradient step; tests/dcgan_dra_oracle.py) against autograd's double backward in float64, and the surface of
+shared weight-gradient step; oracle/dcgan_torch.py) against autograd's double backward in float64, and the surface of
 the dc_dra_gan, dc_ra_gan and dc_fisher_gan drop-ins.  No GPU needed."""
 import inspect
 
 import pytest
 import torch
 
-import dcgan_dra_oracle as O
+from oracle import dcgan_torch as O
 
 
 def _critic(hd=8, seed=0, wstd=0.05):
     torch.manual_seed(seed)
-    D = O.SigmoidCritic(hd, 3).double()
+    D = O.Critic(hd, 3, "sigmoid").double()
     with torch.no_grad():
         for l in D.layers():
             l.weight.normal_(0.0, wstd)

@@ -3,31 +3,15 @@ x_hat, the sigmoid / K penalty, the split batch-statistic loss passes), one D an
 autograd at the CUDA path's bf16 storage points, global statistics from two half batches, DRAGAN's penalty descent,
 Fisher's multiplier update and the drop-ins on the reference's driver lines.  With GM_PARITY_DIR set, the measured errors
 are written to $GM_PARITY_DIR/parity_dcgan_stats.json."""
-import json
-import os
-
-import numpy as np
 import pytest
 import torch
 
-import dcgan_dra_oracle as R
+import dcgan_harness as H
+from dcgan_harness import nrel
+from oracle import dcgan_torch as O
 
 pytestmark = pytest.mark.gpu
-_REPORT = {}
-
-
-def _nrel(a, b):
-    a, b = a.detach().double().reshape(-1).cpu(), b.detach().double().reshape(-1).cpu()
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
-
-
-def _dump():
-    out = os.environ.get("GM_PARITY_DIR")
-    if not out:
-        return
-    os.makedirs(out, exist_ok=True)
-    with open(os.path.join(out, "parity_dcgan_stats.json"), "w") as f:
-        json.dump(_REPORT, f, indent=1, sort_keys=True)
+_REPORT = H.Report("dcgan_stats")
 
 
 def _L():
@@ -56,8 +40,7 @@ def test_std_sums_and_dragan_xhat_rows_match_torch():
     sd = float(xd.std())
     ref = delta.view(n, 1) * xf + (1 - delta.view(n, 1)) * (xf + C * sd * u)
     err = (out.float() - ref).abs() / ref.abs().clamp_min(1e-3)
-    _REPORT["xhat_rows"] = {"max_rel": float(err.max()), "std": sd}
-    _dump()
+    _REPORT.add("xhat_rows", {"max_rel": float(err.max()), "std": sd})
     assert float(err.max()) <= 2 ** -8 * 1.01, float(err.max())                 # one bf16 rounding of the fp32 value
     # Philox: keyed by (seed, stream), delta per row and u per element in [0, 1]
     draws = []
@@ -93,9 +76,8 @@ def test_dragan_penalty_kernel_seed_norm_and_loss():
     rref = torch.where((nJ > 0).view(n, 1), k.view(n, 1) * (Jd / nJ.clamp_min(1e-300).view(n, 1) + ((1 - 2 * sg) * nJ).view(n, 1) * xd),
                        torch.zeros_like(Jd))
     lref = 0.25 + lam * float(((ng - K) ** 2).mean())
-    rep = {"norm": _nrel(norms, ng), "r": _nrel(r.view(n, -1), rref), "loss": abs(float(loss[0]) - lref) / lref}
-    _REPORT["penalty_kernel"] = rep
-    _dump()
+    rep = {"norm": nrel(norms, ng), "r": nrel(r.view(n, -1), rref), "loss": abs(float(loss[0]) - lref) / lref}
+    _REPORT.add("penalty_kernel", rep)
     assert float(norms[4]) == 0.0 and bool((r[4 * 4096:5 * 4096] == 0).all())
     assert float(norms[5]) < 1e-15 and float(r[5 * 4096:].float().abs().max()) < 1e-12
     assert rep["norm"] < 1e-6 and rep["loss"] < 1e-6 and rep["r"] < 4e-3, rep            # r: bf16 rounding of the stored seed
@@ -141,12 +123,11 @@ def test_batch_statistic_loss_passes_match_torch(variant):
     eng.fisher_state(lam, rho)
     _, ds, loss = _stat_call(eng, logits, n, n, 1.0 / n)
     lref, dsref, omega = _stat_loss_torch(variant, logits, n, lam, rho)
-    rep = {"loss": abs(float(loss[0]) - lref) / abs(lref), "ds": _nrel(ds, dsref)}
+    rep = {"loss": abs(float(loss[0]) - lref) / abs(lref), "ds": nrel(ds, dsref)}
     if variant == "fisher":
         rep["omega"] = abs(float(loss[2]) - omega)
         rep["lambda"] = abs(eng.fisher_state()[0] - (lam - rho * omega))
-    _REPORT["loss_pass_" + variant] = rep
-    _dump()
+    _REPORT.add("loss_pass_" + variant, rep)
     assert rep["loss"] < 1e-5 and rep["ds"] < 1e-5, rep
     if variant == "fisher":
         assert rep["omega"] < 1e-6 and rep["lambda"] < 1e-6, rep
@@ -188,39 +169,20 @@ def test_batch_statistics_of_two_halves_equal_the_full_batch(variant):
         out.append((ds, loss))
     ds_split = torch.cat([out[0][0][:n], out[1][0][:n], out[0][0][n:], out[1][0][n:]])
     loss_split = 0.5 * (float(out[0][1][0]) + float(out[1][1][0]))
-    rep = {"ds": _nrel(ds_split, ds_full), "loss": abs(loss_split - float(loss_full[0])) / abs(float(loss_full[0]))}
+    rep = {"ds": nrel(ds_split, ds_full), "loss": abs(loss_split - float(loss_full[0])) / abs(float(loss_full[0]))}
     if variant == "fisher":
         rep["lambda"] = [abs(e.fisher_state()[0] - lam_full) for e in engs]
-    _REPORT["split_stats_" + variant] = rep
-    _dump()
+    _REPORT.add("split_stats_" + variant, rep)
     assert rep["ds"] < 1e-6 and rep["loss"] < 1e-5, rep
     if variant == "fisher":
         assert max(rep["lambda"]) < 1e-7, rep
 
 
 # ------------------------------------------------------------------ one D step and one G step (hidden 16, batch 8)
-def _bn_setup(variant, hd=16, z=100, wstd=0.05):
-    import gm_b200
-    from oracle import dcgan_torch as O
-    eng = gm_b200.DcganEngine(hidden_dim=hd, z_dim=z, variant=variant)
-    g = torch.Generator().manual_seed(11)
-    for net in (eng.G, eng.D):
-        for name in net.names:
-            if name.startswith("l"):
-                net.view(name).copy_(wstd * torch.randn(net.view(name).shape, generator=g))
-    eng.D.view("l5.weight")[1:].zero_()
-    eng.G.refresh(); eng.D.refresh()
-    G, D = O.Generator(hd, z), O.Discriminator(hd)
-    O.load_from_engine_weights(G, D, eng.torch_weights())
-    G.train(); D.train()
-    G.q = D.q = staticmethod(O.bf16_points)
-    return eng, G, D
-
-
 @pytest.mark.parametrize("variant", ["ra", "fisher"])
 def test_ra_fisher_d_and_g_step_match_the_oracle(variant):
     n, z = 8, 100
-    eng, G, D = _bn_setup(variant)
+    eng, G, D, _ = H.setup(variant)
     lam, rho = 0.4, 0.3
     eng.fisher_state(lam, rho)
     g = torch.Generator().manual_seed(5)
@@ -235,11 +197,9 @@ def test_ra_fisher_d_and_g_step_match_the_oracle(variant):
         Ld_ref = -((DX.mean() - DG.mean()) + lam * omega - (rho / 2) * omega ** 2)
     gd = torch.autograd.grad(Ld_ref, list(D.parameters()))
     rep = {"D_loss": abs(Ld - Ld_ref.item()) / abs(Ld_ref.item())}
+    tg = eng.torch_grads()
     for (name, p), gref in zip(D.named_parameters(), gd):
-        got = eng.D.view(name, eng.D.grads).detach().cpu()
-        if name.startswith("l"):
-            got = got[: p.shape[0]].view(p.shape[0], 4, 4, -1).permute(0, 3, 1, 2)
-        rep["gradD_" + name] = _nrel(got, gref)
+        rep["gradD_" + name] = nrel(tg["D." + name], gref)
     if variant == "fisher":
         rep["lambda"] = abs(eng.fisher_state()[0] - (lam - rho * float(omega)))
     # G step: NS for RaNS (as the conv NSGAN), -mean(D(G(z))) for Fisher
@@ -248,13 +208,10 @@ def test_ra_fisher_d_and_g_step_match_the_oracle(variant):
     Lg_ref = -torch.mean(torch.log(dg + 1e-8)) if variant == "ra" else -dg.mean()
     gg = torch.autograd.grad(Lg_ref, list(G.parameters()))
     rep["G_loss"] = abs(Lg - Lg_ref.item()) / abs(Lg_ref.item())
+    tg = eng.torch_grads()
     for (name, p), gref in zip(G.named_parameters(), gg):
-        got = eng.G.view(name, eng.G.grads).detach().cpu()
-        if name.startswith("l"):
-            got = got.view(4, 4, p.shape[1], p.shape[0]).permute(3, 2, 0, 1)
-        rep["gradG_" + name] = _nrel(got, gref)
-    _REPORT["step_" + variant] = rep
-    _dump()
+        rep["gradG_" + name] = nrel(tg["G." + name], gref)
+    _REPORT.add("step_" + variant, rep)
     assert rep["D_loss"] < 5e-3 and rep["G_loss"] < 1e-2, rep
     if variant == "fisher":
         assert rep["lambda"] < 5e-3 * rho * abs(float(omega)), rep        # Omega of the device's scores vs the oracle's
@@ -264,75 +221,38 @@ def test_ra_fisher_d_and_g_step_match_the_oracle(variant):
             assert v < 0.12, (k, v, rep)
 
 
-def _dra_setup(hd=16, z=100, n=8, wstd=0.05, seed=11):
-    import gm_b200
-    from oracle import dcgan_torch as O
-    eng = gm_b200.DcganEngine(hidden_dim=hd, z_dim=z, variant="dra")
-    g = torch.Generator().manual_seed(seed)
-    for net in (eng.G, eng.D):
-        for name in net.names:
-            if name.startswith("l"):
-                net.view(name).copy_(wstd * torch.randn(net.view(name).shape, generator=g))
-    eng.D.view("l5.weight")[1:].zero_()
-    eng.G.refresh(); eng.D.refresh()
-    G = O.Generator(hd, z)
-    D = R.SigmoidCritic(hd, 3)
-    sd = eng.torch_weights()
-    assert not any(k.startswith("D.bn") for k in sd)
-    with torch.no_grad():
-        for name, p in G.named_parameters():
-            p.copy_(sd["G." + name])
-    R.W.load_engine_weights(D, sd)
-    G.train()
-    imgs = torch.rand(n, 3 * 64 * 64, generator=g)
-    zz = torch.randn(n, z, generator=g)
-    delta = torch.rand(n, generator=g)
-    u = torch.rand(n, 3 * 64 * 64, generator=g)
-    return eng, G, D, imgs, zz, delta, u
-
-
-def _dgrads(eng, D):
-    out = []
-    for i in range(5):
-        w = eng.D.view("l%d.weight" % (i + 1), eng.D.grads).detach().cpu()
-        p = D.layers()[i].weight
-        out.append(w[: p.shape[0]].view(p.shape[0], 4, 4, -1).permute(0, 3, 1, 2))
-    return out
-
-
 def test_dra_d_step_matches_autograd_and_the_closed_form_oracle():
-    from oracle import dcgan_torch as O
     n, lam, K, Cc = 8, 10.0, 1.0, 1.0
-    eng, G, D, imgs, z, delta, u = _dra_setup(n=n)
+    eng, G, D, imgs, z, (delta, u) = H.critic_setup("dra", n=n)
     Ld = eng.d_grad(eng.stage_images(imgs.cuda()), n, noise=z.cuda(), gp_lambda=lam, gp_k=K, dra_c=Cc, delta=delta.cuda(),
                     u=u.cuda()).item()
     norms = eng.gp_norms_.cpu().double()
     gp = lam * float(((norms - K) ** 2).mean())
-    got = _dgrads(eng, D)
+    tg = eng.torch_grads()
+    got = [tg["D.l%d.weight" % (i + 1)].cpu() for i in range(5)]
     with torch.no_grad():
         fake = G(z)
-    xh = R.make_xhat(imgs, delta, u, Cc)
-    ex = R.autograd_d_step(D, imgs, fake, xh, lam, K)
+    xh = O.make_xhat(imgs, delta, u, Cc)
+    ex = O.autograd_d_step(D, imgs, fake, xh, lam, K)
     Gq = O.Generator(D.l1.weight.shape[0], z.shape[1])
     Gq.load_state_dict(G.state_dict())
     Gq.q = staticmethod(O.bf16_points)
     Gq.train()
     with torch.no_grad():
         fake_q = Gq(z)
-    rq = R.bf16_points(imgs)
-    xh_q = R.bf16_points(R.make_xhat(rq, delta, u, Cc))
-    cf = R.closed_form_d_step(D, rq, fake_q, xh_q, lam, K, q=R.bf16_points)
+    rq = O.bf16_points(imgs)
+    xh_q = O.bf16_points(O.make_xhat(rq, delta, u, Cc))
+    cf = O.closed_form_d_step(D, rq, fake_q, xh_q, lam, K, q=O.bf16_points)
     rep = {"D_loss": abs(Ld - float(ex["loss"])) / abs(float(ex["loss"])), "GP": abs(gp - float(ex["gp"])) / abs(float(ex["gp"])),
-           "NS_part": abs((Ld - gp) - float(ex["ns"])) / abs(float(ex["ns"])), "norms_vs_exact": _nrel(norms, ex["norms"]),
-           "norms_vs_bf16_oracle": _nrel(norms, cf["norms"]), "xhat_logits_vs_bf16_oracle": _nrel(eng.gp_logits_, cf["s"])}
+           "NS_part": abs((Ld - gp) - float(ex["rows"])) / abs(float(ex["rows"])), "norms_vs_exact": nrel(norms, ex["norms"]),
+           "norms_vs_bf16_oracle": nrel(norms, cf["norms"]), "xhat_logits_vs_bf16_oracle": nrel(eng.gp_logits_, cf["s"])}
     for i in range(5):
-        rep["gradD_l%d_vs_bf16_oracle" % (i + 1)] = _nrel(got[i], cf["grads"][i])
-        rep["gradD_l%d_vs_exact" % (i + 1)] = _nrel(got[i], ex["grads"][i])
+        rep["gradD_l%d_vs_bf16_oracle" % (i + 1)] = nrel(got[i], cf["grads"][i])
+        rep["gradD_l%d_vs_exact" % (i + 1)] = nrel(got[i], ex["grads"][i])
         scale = sum(float(cf["parts"][k][i].norm()) for k in ("real", "fake", "penalty"))
         rep["gradD_l%d_cancellation" % (i + 1)] = scale / float(cf["grads"][i].norm())
         rep["gradD_l%d_vs_bf16_oracle_of_parts" % (i + 1)] = float((got[i].double() - cf["grads"][i].double()).norm()) / scale
-    _REPORT["d_step_dra"] = rep
-    _dump()
+    _REPORT.add("d_step_dra", rep)
     assert rep["D_loss"] < 5e-3 and rep["GP"] < 5e-3, rep
     # the WGAN-GP critic bounds of test_dcgan_wgp_gpu
     for i in range(5):
@@ -341,22 +261,18 @@ def test_dra_d_step_matches_autograd_and_the_closed_form_oracle():
 
 
 def test_dra_g_step_matches_the_oracle():
-    from oracle import dcgan_torch as O
     n = 8
-    eng, G, D, imgs, z, delta, u = _dra_setup(n=n)
+    eng, G, D, imgs, z, _ = H.critic_setup("dra", n=n)
     Lg = eng.g_grad(n, noise=z.cuda()).item()
     G.q = staticmethod(O.bf16_points)
-    s, _ = D.trace(G(z), R.bf16_points)
+    s, _ = D.trace(G(z), O.bf16_points)
     loss = -torch.mean(torch.log(torch.sigmoid(s) + 1e-8))               # src/dra_gan.py:245
     gg = torch.autograd.grad(loss, list(G.parameters()))
     rep = {"G_loss": abs(Lg - loss.item()) / abs(loss.item())}
+    tg = eng.torch_grads()
     for (name, p), gref in zip(G.named_parameters(), gg):
-        got = eng.G.view(name, eng.G.grads).detach().cpu()
-        if name.startswith("l"):
-            got = got.view(4, 4, p.shape[1], p.shape[0]).permute(3, 2, 0, 1)
-        rep["gradG_" + name] = _nrel(got, gref)
-    _REPORT["g_step_dra"] = rep
-    _dump()
+        rep["gradG_" + name] = nrel(tg["G." + name], gref)
+    _REPORT.add("g_step_dra", rep)
     assert rep["G_loss"] < 5e-3, rep
     for k, v in rep.items():
         if k.startswith("grad"):
@@ -366,57 +282,18 @@ def test_dra_g_step_matches_the_oracle():
 def test_dra_split_batch_sums_to_the_full_batch():
     """data-parallel contract on one GPU: with std(x) summed over both halves through stats_reduce, the D gradient of 2n
     images equals the SUM of the two n-image gradients at inv_global_batch = 1/(2n)"""
-    n = 4
-    eng, G, D, imgs, z, delta, u = _dra_setup(n=2 * n)
-    fake, _ = eng.g_forward(2 * n, z.cuda())
-    fake = fake.clone()
-    real = eng.stage_images(imgs.cuda())
-    inv = 1.0 / (2 * n)
-    dc, uc = delta.cuda(), u.cuda()
-    loc = []
-    for k in range(2):
-        s = torch.zeros(2, device="cuda", dtype=torch.float64)
-        eng.dra_std_sums(real[k * n * 4096:(k + 1) * n * 4096].clone(), n, s)
-        loc.append(s)
-    total = loc[0] + loc[1]
-    eng.stats_reduce = lambda buf: buf.copy_(total)
-    L = eng.dra_critic_grad(real, fake, 2 * n, inv, 10.0, 1.0, 1.0, dc, uc, stat_batch=2 * n).item()
-    full = eng.D.grads.clone()
-    parts, losses = [], []
-    for k in range(2):
-        rows = slice(k * n * 4096, (k + 1) * n * 4096)
-        losses.append(eng.dra_critic_grad(real[rows].clone(), fake[rows].clone(), n, inv, 10.0, 1.0, 1.0, dc[k * n:(k + 1) * n].clone(),
-                                          uc[k * n:(k + 1) * n].clone(), stat_batch=2 * n).item())
-        parts.append(eng.D.grads.clone())
-    eng.stats_reduce = None
-    rel = _nrel(parts[0] + parts[1], full)
-    _REPORT["dra_split_batch"] = {"grad_nrel": rel, "loss_abs": abs(L - 0.5 * (losses[0] + losses[1]))}
-    _dump()
-    assert rel <= 1e-5, rel
-    assert abs(L - 0.5 * (losses[0] + losses[1])) <= 1e-5 * max(1.0, abs(L)), (L, losses)
+    H.split_batch_sums_to_the_full_batch("dra", _REPORT, "dra_split_batch")
 
 
 # ------------------------------------------------------------------ behaviour
 def test_dra_penalty_pulls_gradient_norms_to_k():
-    import gm_b200
-    n = 16
-    eng, G, D, imgs, z, delta, u = _dra_setup(n=n)
-    x, zc, dc, uc = eng.stage_images(imgs.cuda()), z.cuda(), delta.cuda(), u.cuda()
-    hp = gm_b200.AdamHP.make(1e-4)
-    dev = []
-    for _ in range(30):
-        eng.d_grad(x, n, noise=zc, delta=dc, u=uc)
-        dev.append(float((eng.gp_norms_ - 1.0).abs().mean()))
-        eng.apply(1, hp)
-    _REPORT["dra_penalty_descent"] = {"first": dev[0], "last": dev[-1]}
-    _dump()
-    assert all(np.isfinite(dev)) and dev[-1] < dev[0], dev
+    H.penalty_pulls_gradient_norms_to_one("dra", None, _REPORT, "dra_penalty_descent")
 
 
 def test_fisher_lambda_follows_rho_omega_step_by_step():
     import gm_b200
     n = 8
-    eng, G, D = _bn_setup("fisher")
+    eng, G, D, _ = H.setup("fisher")
     g = torch.Generator().manual_seed(6)
     x = eng.stage_images(torch.rand(n, 3 * 64 * 64, generator=g).cuda())
     rho = 0.05
@@ -431,62 +308,11 @@ def test_fisher_lambda_follows_rho_omega_step_by_step():
         errs.append(abs(new - (lam - rho * omega)))
         lam = new
         eng.apply(1, hp)
-    _REPORT["fisher_lambda"] = {"max_err": max(errs), "lambda": lam}
-    _dump()
+    _REPORT.add("fisher_lambda", {"max_err": max(errs), "lambda": lam})
     assert max(errs) < 1e-7 and lam != 0.0, errs
 
 
 # ------------------------------------------------------------------ the drop-ins on the reference's driver lines
 @pytest.mark.parametrize("which", ["ra", "fisher", "dra"])
 def test_dropins_run_the_reference_driver_code(which):
-    import tempfile
-    import importlib
-    mod = importlib.import_module({"ra": "dc_ra_gan", "fisher": "dc_fisher_gan", "dra": "dc_dra_gan"}[which])
-    Model, Trainer = {"ra": (mod.__dict__.get("DCRaNSGAN"), mod.__dict__.get("DCRaNSGANTrainer")),
-                      "fisher": (mod.__dict__.get("DCFisherGAN"), mod.__dict__.get("DCFisherGANTrainer")),
-                      "dra": (mod.__dict__.get("DCDRAGAN"), mod.__dict__.get("DCDRAGANTrainer"))}[which]
-    g = torch.Generator().manual_seed(0)
-    imgs = torch.rand(64, 3, 64, 64, generator=g)
-    loader = torch.utils.data.DataLoader(torch.utils.data.TensorDataset(imgs, torch.zeros(64)), batch_size=16, shuffle=True)
-    torch.manual_seed(3)
-    model = Model(image_size=64 * 64 * 3, hidden_dim=16, z_dim=100)
-    before = {k: v.clone() for k, v in model.state_dict().items()}
-    trainer = Trainer(model=model, train_iter=loader, val_iter=loader, test_iter=loader, viz=False)
-    if which == "ra":
-        trainer.train(num_epochs=2, G_lr=2e-4, D_lr=2e-4, D_steps=1)                  # src/ra_gan.py __main__
-    elif which == "fisher":
-        trainer.train(num_epochs=2, G_lr=1e-4, D_lr=1e-4, D_steps=1, RHO=1e-6)        # src/fisher_gan.py __main__
-        assert trainer.LAMBDA.shape == (1,) and float(trainer.LAMBDA) != 0.0 and float(trainer.RHO) == pytest.approx(1e-6)
-    else:
-        trainer.train(num_epochs=2, G_lr=1e-4, D_lr=1e-4, D_steps=1)                  # src/dra_gan.py __main__
-    assert len(trainer.Dlosses) == 8 and len(trainer.Glosses) == 8
-    assert all(np.isfinite(trainer.Dlosses)) and all(np.isfinite(trainer.Glosses))
-    after = model.state_dict()
-    assert all(not torch.equal(before[k], after[k]) for k in before if k.startswith("D.l") and k.endswith("weight"))
-    assert any(not torch.equal(before[k], after[k]) for k in before if k.startswith("G.") and k.endswith("weight"))
-    assert trainer.generate_images(0, num_outputs=4).shape == (4, 3, 64, 64)
-    d = model.D(imgs[:8])
-    assert d.shape == (8, 1) and float(d.min()) > 0 and float(d.max()) < 1                 # sigmoid output
-    with tempfile.TemporaryDirectory() as tmp:
-        path = os.path.join(tmp, "model.ckpt")
-        trainer.save_model(path)
-        model2 = Model(image_size=64 * 64 * 3, hidden_dim=16, z_dim=100)
-        tr2 = Trainer(model2, loader, loader, loader)
-        tr2.load_model(path)
-        assert list(model2.state_dict()) == list(model.state_dict())
-        zz = torch.randn(4, 100)
-        assert _nrel(model2.G(zz), model.G(zz)) < 1e-6
-    # the reference's loop body: D_loss.backward() delivers torch-layout gradients
-    model.D.zero_grad()
-    if which == "fisher":
-        loss, ipm = trainer.train_D(imgs[:16].reshape(16, -1))
-        assert isinstance(ipm, float)
-    elif which == "dra":
-        loss = trainer.train_D(imgs[:16].reshape(16, -1), LAMBDA=10, K=1, C=1)
-    else:
-        loss = trainer.train_D(imgs[:16].reshape(16, -1))
-    loss.backward()
-    assert model.D.l4.weight.grad is not None and float(model.D.l4.weight.grad.abs().sum()) > 0
-    gl = trainer.train_G(imgs[:16])
-    gl.backward()
-    assert np.isfinite(float(gl))
+    H.run_reference_driver_lines(which)

@@ -1,12 +1,12 @@
 """WGAN-GP on the DCGAN conv path, CPU side: the closed-form double backward of the batch-norm-free critic
-(tests/dcgan_wgp_oracle.py, the five steps the CUDA path runs) against autograd's double backward in float64, and the
+(oracle/dcgan_torch.py, the five steps the CUDA path runs) against autograd's double backward in float64, and the
 surface of the dc_w_gp_gan drop-in.  No GPU needed."""
 import inspect
 
 import pytest
 import torch
 
-import dcgan_wgp_oracle as O
+from oracle import dcgan_torch as O
 
 
 def _critic(out_act, sign, hd=8, seed=0):
@@ -29,9 +29,7 @@ def _batch(n=5, seed=1):
 
 def _rows_with_live_and_dead(D, real, fake, eps):
     """x_hat rows whose logit is positive (live) and negative (dead): a relu critic must be tested on both"""
-    n = real.shape[0]
-    xh = eps.view(n, 1) * real + (1 - eps.view(n, 1)) * fake
-    return O.Critic.trace(D, xh)[0]
+    return O.Critic.trace(D, O.interpolate(real, fake, eps))[0]
 
 
 def _mixed_case(out_act):
@@ -55,8 +53,9 @@ def _mixed_case(out_act):
 def test_closed_form_penalty_gradient_equals_autograd_double_backward(out_act):
     D, real, fake, eps, s = _mixed_case(out_act)
     assert bool((s > 0).any()) and bool((s < 0).any()), s          # live and dead rows in the same batch
-    cf = O.closed_form_d_step(D, real, fake, eps, lam=10.0)
-    ag = O.autograd_d_step(D, real, fake, eps, lam=10.0)
+    xh = O.interpolate(real, fake, eps)
+    cf = O.closed_form_d_step(D, real, fake, xh, lam=10.0)
+    ag = O.autograd_d_step(D, real, fake, xh, lam=10.0)
     assert abs(float(cf["loss"] - ag["loss"])) <= 1e-9 * max(1.0, abs(float(ag["loss"])))
     assert abs(float(cf["gp"] - ag["gp"])) <= 1e-9 * abs(float(ag["gp"]))
     for l, (a, b) in enumerate(zip(cf["grads"], ag["grads"])):
@@ -76,8 +75,9 @@ def test_dead_relu_batch_has_penalty_lambda_and_only_the_w_gradient():
     real, fake, eps = _batch()
     s = _rows_with_live_and_dead(D, real, fake, eps)
     assert bool((s < 0).all())
-    cf = O.closed_form_d_step(D, real, fake, eps, lam=10.0)
-    no_gp = O.closed_form_d_step(D, real, fake, eps, lam=0.0)
+    xh = O.interpolate(real, fake, eps)
+    cf = O.closed_form_d_step(D, real, fake, xh, lam=10.0)
+    no_gp = O.closed_form_d_step(D, real, fake, xh, lam=0.0)
     assert float(cf["gp"]) == 10.0
     for a, b in zip(cf["grads"], no_gp["grads"]):
         assert torch.equal(a, b)
@@ -88,9 +88,10 @@ def test_split_batch_sums_to_the_full_batch():
     D, real, fake, eps, _ = _mixed_case("relu")
     real, fake, eps = torch.cat([real, real.flip(0)]), torch.cat([fake, fake.flip(0)]), torch.cat([eps, eps.flip(0) * 0.5])
     n = real.shape[0] // 2
-    full = O.closed_form_d_step(D, real, fake, eps)
-    a = O.closed_form_d_step(D, real[:n], fake[:n], eps[:n], inv=1.0 / (2 * n))
-    b = O.closed_form_d_step(D, real[n:], fake[n:], eps[n:], inv=1.0 / (2 * n))
+    xh = O.interpolate(real, fake, eps)
+    full = O.closed_form_d_step(D, real, fake, xh)
+    a = O.closed_form_d_step(D, real[:n], fake[:n], xh[:n], inv=1.0 / (2 * n))
+    b = O.closed_form_d_step(D, real[n:], fake[n:], xh[n:], inv=1.0 / (2 * n))
     for f, x, y in zip(full["grads"], a["grads"], b["grads"]):
         assert float((f - (x + y)).norm() / f.norm()) < 1e-12
 
