@@ -126,7 +126,8 @@ class DCGANTrainer:
     def _engine_synced(self):
         m = self.model
         if self._engine is None:
-            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, d_out_act=m.D.out_act)
+            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, d_out_act=m.D.out_act,
+                                       embed_dim=getattr(m.D, "embed_dim", None))
             self._dirty = True
         if self._dirty:
             self._engine.load_torch_weights(self._sd())
@@ -181,13 +182,20 @@ class DCGANTrainer:
                 ring[D_steps, i] = eng.g_grad(n, inv_global_batch=inv, seed=seed, step=self._step)
                 par.sum_gradients(eng.G.grads)
                 eng.apply(0, hpG)
+                self._after_g_step(eng)
                 self._step += 1
             G_losses, D_losses = ring[D_steps].tolist(), ring[:D_steps].mean(dim=0).tolist()
             self.Glosses.extend(G_losses)
             self.Dlosses.extend(D_losses)
-            print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
+            print(self._epoch_line(eng, epoch, num_epochs, G_losses, D_losses))
             self.num_epochs += 1
         self._pull()
+
+    def _epoch_line(self, eng, epoch, num_epochs, G_losses, D_losses):
+        return "Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses))
+
+    def _after_g_step(self, eng):
+        """per-step device work of a subclass after each G update (e.g. BEGAN's K control); enqueued, never synchronising"""
 
     def _pre_train(self, eng):
         """per-train() state of a subclass (e.g. Fisher GAN's multiplier), after the optimizers are reset"""

@@ -81,6 +81,7 @@ def lib():
     L.gm_prof_collect.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_longlong)]
     L.gm_gemm_bf16.argtypes = [vp, C.POINTER(GemmDesc), vp]
     L.gm_adam_step.argtypes = [vp, vp, vp, vp, vp, i, C.POINTER(AdamHP), i, vp]
+    L.gm_adam_step_lr.argtypes = [vp, vp, vp, vp, vp, i, C.POINTER(AdamHP), vp, i, vp]
     L.gm_gan_create.argtypes = [vp, C.POINTER(GanDesc), C.POINTER(vp)]
     L.gm_gan_destroy.argtypes = [vp]
     L.gm_gan_param_count.argtypes = [vp, i]
@@ -144,6 +145,10 @@ def lib():
     L.gm_dra_std_sums.argtypes = [vp, vp, i, i, i, vp, vp]
     L.gm_dra_xhat_rows.argtypes = [vp, vp, i, i, i, vp, C.c_double, f, vp, u64, u64, vp, i, vp]
     L.gm_dra_penalty.argtypes = [vp, vp, i, vp, i, vp, i, i, i, f, f, f, f, vp, i, vp, vp, vp]
+    L.gm_l1_rows.argtypes = [vp, vp, vp, i, i, f, vp, vp, vp, vp]
+    L.gm_began_loss_final.argtypes = [vp, vp, vp, i, i, vp, vp, vp]
+    L.gm_began_control.argtypes = [vp, vp, f, f, f, vp]
+    L.gm_began_dfake_rows.argtypes = [vp, vp, vp, vp, vp, i, i, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]
@@ -264,6 +269,7 @@ def gemm_bf16(A, B, out, mode="nt", N=None, K=None, M=None, bias=None, act=0, au
     check(h, lib().gm_gemm_bf16(h, C.byref(d), _stream()))
 
 
-def adam_step(p, g, m, v, hp, step):
+def adam_step(p, g, m, v, hp, step, lr_scale=None):
+    """One Adam update; lr_scale: None or a device fp32 scalar tensor multiplying hp.lr when the kernel runs"""
     h = ctx()
-    check(h, lib().gm_adam_step(h, _ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), C.byref(hp), int(step), _stream()))
+    check(h, lib().gm_adam_step_lr(h, _ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), C.byref(hp), _ptr(lr_scale), int(step), _stream()))

@@ -572,6 +572,60 @@ __global__ void __launch_bounds__(256) moments_sum_kernel(const double* __restri
   if (threadIdx.x == 0) { out[0] = s1; out[1] = s2; }
 }
 
+// ---- BEGAN's L1 reconstruction loss (src/be_gan.py:225,233,256) on the autoencoder D of the conv path
+// r, x: `groups` 16-byte groups of bf16 (NHWC image rows back to back).  grad = sign(r - x) * inv * (coef ? coef[0] : 1) as
+// bf16 (sign(0) = 0, torch's abs backward; coef is a device scalar so that K never crosses to the host), and the block's
+// partial of sum |r - x| in double (r - x of two bf16 values is exact in double).  Each of r and x is read once.
+constexpr int kL1Unroll = 2;
+__global__ void __launch_bounds__(256) l1_rows_kernel(const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ x,
+                                                      uint32_t groups, float inv, const float* __restrict__ coef,
+                                                      __nv_bfloat16* __restrict__ grad, double* __restrict__ part) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  const float k = coef ? inv * coef[0] : inv;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  double acc = 0.0;
+  for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < groups; i0 += stride * kL1Unroll) {
+    uint4 rv[kL1Unroll], xv[kL1Unroll];
+#pragma unroll
+    for (int u = 0; u < kL1Unroll; ++u) {
+      const uint32_t i = i0 + u * stride;
+      rv[u] = xv[u] = make_uint4(0, 0, 0, 0);
+      if (i < groups && i >= i0) {
+        rv[u] = __ldg(reinterpret_cast<const uint4*>(r) + i);
+        xv[u] = __ldg(reinterpret_cast<const uint4*>(x) + i);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kL1Unroll; ++u) {
+      const uint32_t i = i0 + u * stride;
+      if (i >= groups || i < i0) continue;
+      const uint32_t a[4] = {rv[u].x, rv[u].y, rv[u].z, rv[u].w}, b[4] = {xv[u].x, xv[u].y, xv[u].z, xv[u].w};
+      float o[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float rr = (q & 1) ? bf16_hi(a[q >> 1]) : bf16_lo(a[q >> 1]);
+        const float xx = (q & 1) ? bf16_hi(b[q >> 1]) : bf16_lo(b[q >> 1]);
+        const double d = double(rr) - double(xx);
+        acc += fabs(d);
+        o[q] = d > 0.0 ? k : (d < 0.0 ? -k : 0.f);
+      }
+      store_bf16x8(grad + size_t(i) * 8, o, 0);
+    }
+  }
+  acc = block_sum<256>(acc, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = acc;
+}
+// sum of the per-block partials of l1_rows_kernel -> out[0] (one block, fixed order)
+__global__ void __launch_bounds__(256) l1_sum_kernel(const double* __restrict__ part, int nblk, double* __restrict__ out) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  double s = 0;
+  for (int i = threadIdx.x; i < nblk; i += 256) s += part[i];
+  s = block_sum<256>(s, sh);
+  if (threadIdx.x == 0) out[0] = s;
+}
+
 // One block per x_hat image b.  J [HW*C] = image gradient of the logit s_b (the beta chain seeded with 1), xh the image.
 // sigma = sigmoid(s_b), sigma' = sigma (1 - sigma), ||g|| = sigma' ||J|| (the gradient of D's sigmoid output),
 // k = 2 lambda inv_grad (||g|| - K); the tangent seed of the penalty's double backward is

@@ -524,17 +524,23 @@ static void fill_adam(AdamParams& a, const gm_adam_hp* hp, int step) {
   a.update = 1;
 }
 
-extern "C" int gm_adam_step(gm_ctx* c, float* p, const float* g, float* m, float* v, int n, const gm_adam_hp* hp,
-                            int step, gm_stream stream) {
+extern "C" int gm_adam_step_lr(gm_ctx* c, float* p, const float* g, float* m, float* v, int n, const gm_adam_hp* hp,
+                               const float* lr_scale_dev, int step, gm_stream stream) {
   if (!c || !p || !g || !m || !v || !hp || n <= 0 || step <= 0) return fail(c, GM_ERR_ARG, "gm_adam_step: bad argument");
   AdamParams a;
   memset(&a, 0, sizeof a);
   a.p = p; a.g = g; a.m = m; a.v = v; a.total = n; a.nseg = 0;
   fill_adam(a, hp, step);
+  a.lr_scale = lr_scale_dev;
   launch_pdl("adam_kernel", adam_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
   c->launches++;
   CU_OK(c, cudaGetLastError());
   return GM_OK;
+}
+
+extern "C" int gm_adam_step(gm_ctx* c, float* p, const float* g, float* m, float* v, int n, const gm_adam_hp* hp,
+                            int step, gm_stream stream) {
+  return gm_adam_step_lr(c, p, g, m, v, n, hp, nullptr, step, stream);
 }
 
 // ------------------------------------------------------------------ bf16 arena

@@ -17,7 +17,10 @@ relu(s) (src/w_gp_gan.py:61) or s (d_out_act="none") — and adds the gradient p
 whose double backward is closed form because the critic is piecewise linear (wgp_critic_grad, DESIGN.md §6b).  variant="dra"
 (DRAGAN, src/dra_gan.py:174-225) trains the same critic with a sigmoid output and the penalty at x_hat around the real data
 (dra_critic_grad); "ra" and "fisher" (src/ra_gan.py:204-205, src/fisher_gan.py:214-223) keep the batch-norm D and run
-their batch statistics in separate loss passes that stats_reduce can sum over data-parallel ranks.
+their batch statistics in separate loss passes that stats_reduce can sum over data-parallel ranks.  variant="be" (BEGAN,
+src/be_gan.py:212-258) makes D an autoencoder: the D trunk above with a linear embed_dim-wide conv 5 as the encoder, the
+generator stack with a linear output as the decoder, L1 reconstruction losses (gm_l1_rows) and K and the plateau scheduler
+as device state (be_state, gm_began_control).
 
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
@@ -111,23 +114,30 @@ class _Net:
             check(h, lib().gm_cast_bf16(h, _ptr(w), w.shape[0], w.shape[1], _ptr(self.bf[n]), self.bf[n].stride(0),
                                         _ptr(self.bf_t[n]), self.bf_t[n].stride(0), _stream()))
 
-    def adam(self, hp):
+    def adam(self, hp, lr_scale=None):
         self.step += 1
-        adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, hp, self.step)
+        adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, hp, self.step, lr_scale)
         self.refresh()
 
 
 class DcganEngine:
     """One DCGAN (64x64xchannels images) on one GPU; see the module docstring."""
 
-    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None, d_out_act=None):
+    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None, d_out_act=None, embed_dim=None):
         if not torch.cuda.is_available():
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp and dra")
-        if variant == "wgp":
+        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra and be")
+        if embed_dim is not None and (variant != "be" or embed_dim <= 0):
+            raise GmError("embed_dim is the positive embedding width of BEGAN's autoencoder D (variant='be')")
+        if variant == "be":
+            # BEGAN's D is an autoencoder whose reconstruction is linear (src/be_gan.py:73-76)
+            if d_out_act not in (None, "none"):
+                raise GmError("the BEGAN autoencoder's output is linear (d_out_act='none')")
+            d_out_act = "none"
+        elif variant == "wgp":
             # WGAN-GP critic: no BatchNorm (one sample's input gradient must not depend on the batch, WGAN-GP paper §4),
             # output relu(s) as src/w_gp_gan.py:61 or the linear s
             d_out_act = "relu" if d_out_act is None else d_out_act
@@ -144,29 +154,51 @@ class DcganEngine:
         self.gp_k, self.dra_c = 1.0, 1.0                         # K, C of src/dra_gan.py:174
         self.fisher = torch.tensor([0.0, 1e-6], device=self.device)   # Fisher's (LAMBDA, RHO), src/fisher_gan.py:117-118
         # stats_reduce(buf): SUM a float64 statistic buffer over the data-parallel ranks in place (RaNS / Fisher loss
-        # moments, DRAGAN's image std); None on one process.  stat_batch (d_grad) is then the global batch.
+        # moments, DRAGAN's image std, BEGAN's L1 sums); None on one process.  stat_batch (d_grad) is then the global batch.
         self.stats_reduce = None
         self.zp = (z_dim + 1 + 7) // 8 * 8                       # noise rows: [z | 1 | pad], 16-byte rows
         hd = hidden_dim
         self.gc = [8 * hd, 4 * hd, 2 * hd, hd, channels]        # generator channels after each layer
         self.dc = [hd, 2 * hd, 4 * hd, 8 * hd]                  # discriminator channels after conv 1..4
-        g_shapes = [("l1.weight", (16 * self.gc[0], z_dim))]
-        for i in range(1, 5):
-            g_shapes.append(("l%d.weight" % (i + 1), (16 * self.gc[i], self.gc[i - 1])))
-        for i in range(4):
-            g_shapes += [("bn%d.weight" % (i + 1), (self.gc[i],)), ("bn%d.bias" % (i + 1), (self.gc[i],))]
-        d_shapes = [("l1.weight", (self.dc[0], 16 * channels))]
-        for i in range(1, 4):
-            d_shapes.append(("l%d.weight" % (i + 1), (self.dc[i], 16 * self.dc[i - 1])))
-        d_shapes.append(("l5.weight", (16, 16 * self.dc[3])))   # 1 real output channel (row 0), padded to the MMA's N = 16
-        for i in range(1, 4) if self.d_bn else ():
-            d_shapes += [("bn%d.weight" % (i + 1), (self.dc[i],)), ("bn%d.bias" % (i + 1), (self.dc[i],))]
-        self.G, self.D = _Net(g_shapes, self.device), _Net(d_shapes, self.device)
+        def g_stack(pfx, zin):                                   # the generator's transposed-conv stack on zin input columns
+            out = [(pfx + "l1.weight", (16 * self.gc[0], zin))]
+            for i in range(1, 5):
+                out.append((pfx + "l%d.weight" % (i + 1), (16 * self.gc[i], self.gc[i - 1])))
+            for i in range(4):
+                out += [(pfx + "bn%d.weight" % (i + 1), (self.gc[i],)), (pfx + "bn%d.bias" % (i + 1), (self.gc[i],))]
+            return out
+
+        def d_stack(pfx, nout):                                  # the discriminator's conv stack with nout output rows
+            out = [(pfx + "l1.weight", (self.dc[0], 16 * channels))]
+            for i in range(1, 4):
+                out.append((pfx + "l%d.weight" % (i + 1), (self.dc[i], 16 * self.dc[i - 1])))
+            out.append((pfx + "l5.weight", (nout, 16 * self.dc[3])))
+            for i in range(1, 4) if self.d_bn else ():
+                out += [(pfx + "bn%d.weight" % (i + 1), (self.dc[i],)), (pfx + "bn%d.bias" % (i + 1), (self.dc[i],))]
+            return out
+
+        self.e = z_dim if embed_dim is None else int(embed_dim)  # BEGAN's embedding width (N_h = N_z in the BEGAN paper)
+        self.ep = (self.e + 15) // 16 * 16                       # embedding rows: [e | 0 pad], N of a bf16-output GEMM
+        if variant == "be":
+            # D = encoder (the DCGAN D trunk, l5: e outputs, zero-padded to ep rows) + decoder (the generator stack with e
+            # in place of z, l1's input columns zero-padded to ep); the torch views trim the padding (_TRIM)
+            self._trim = {"D.encoder.l5.weight": self.e, "D.decoder.l1.weight": self.e}
+            d_shapes = d_stack("encoder.", self.ep) + g_stack("decoder.", self.ep)
+        else:
+            self._trim = {"D.l5.weight": 1}
+            d_shapes = d_stack("", 16)                           # 1 real output channel (row 0), padded to the MMA's N = 16
+        self.G, self.D = _Net(g_stack("", z_dim), self.device), _Net(d_shapes, self.device)
         self.run_G = {i: torch.zeros(2, self.gc[i], device=self.device) for i in range(4)}
         self.run_D = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4) if self.d_bn}
-        for r in list(self.run_G.values()) + list(self.run_D.values()):
+        self.run_dec = {i: torch.zeros(2, self.gc[i], device=self.device) for i in range(4)} if variant == "be" else {}
+        for r in list(self.run_G.values()) + list(self.run_D.values()) + list(self.run_dec.values()):
             r[1].fill_(1.0)
         self.loss_buf = torch.zeros(4, device=self.device)      # [D loss, G loss, loss-kernel scratch (sum ds, ..)]
+        # BEGAN's device state, the layout of gm_gan_began_state: [K, inv_b, -K inv_b, DX, DG, plateau best, plateau bad
+        # count, lr scale, inv_b, inv_b, convergence]; the conv path passes its gradient scales per call ([1], [2], [8], [9] unused)
+        self.be_state = torch.zeros(11, device=self.device)
+        if variant == "be":
+            self.began_init(0.0, 1)
         self._bufs = {}
         self.init_weights()
 
@@ -179,28 +211,41 @@ class DcganEngine:
                 v = net.view(n)
                 if n.endswith("bias"):
                     v.zero_()
-                elif n.startswith("bn"):
+                elif n.split(".")[-2].startswith("bn"):
                     v.copy_(1.0 + 0.02 * torch.randn(v.shape, generator=g))
                 else:
                     v.copy_(0.02 * torch.randn(v.shape, generator=g))
-        self.D.view("l5.weight")[1:].zero_()                     # padding rows of the 1-channel output layer
+        self.zero_padding()
         self.G.refresh()
         self.D.refresh()
 
+    def zero_padding(self):
+        """zero the padding of D's padded weights (the 1-channel output layer's rows 1..15; BEGAN's embedding rows / columns
+        beyond e): their gradients are then zero, so they stay zero and the padded GEMM columns read zeros"""
+        if self.variant == "be":
+            self.D.view("encoder.l5.weight")[self.e:].zero_()
+            self.D.view("decoder.l1.weight")[:, self.e:].zero_()
+        else:
+            self.D.view("l5.weight")[1:].zero_()
+
     def _torch_views(self, which):
         """{torch-style name: view of the G / D tensor in torch's layout} over the flat params (which="params") or grads.
-        Conv weights are [Cout, (kh, kw, ci)] here and [Cout, Cin, kh, kw] in torch (D.l5: output channel 0 of the 16 padded
-        rows); transposed-conv weights are [(kh, kw, co), Cin] here and [Cin, Cout, kh, kw] in torch; BatchNorm vectors match."""
+        Conv weights are [Cout, (kh, kw, ci)] here and [Cout, Cin, kh, kw] in torch; transposed-conv weights (G, BEGAN's
+        decoder) are [(kh, kw, co), Cin] here and [Cin, Cout, kh, kw] in torch; BatchNorm vectors match.  Padded weights are
+        trimmed on torch's dim 0 (_trim: D.l5 keeps output channel 0 of its 16 rows, BEGAN's encoder l5 / decoder l1 the e
+        embedding channels)."""
         out = {}
         for tag, net in (("G", self.G), ("D", self.D)):
             for n in net.names:
                 w = net.view(n, getattr(net, which))
-                if n.startswith("l") and tag == "G":
-                    w = w.view(4, 4, w.shape[0] // 16, w.shape[1]).permute(3, 2, 0, 1)
-                elif n.startswith("l"):
-                    w = w[:1] if n == "l5.weight" else w
-                    w = w.view(w.shape[0], 4, 4, w.shape[1] // 16).permute(0, 3, 1, 2)
-                out["%s.%s" % (tag, n)] = w
+                key = "%s.%s" % (tag, n)
+                if n.split(".")[-2].startswith("l"):
+                    if tag == "G" or n.startswith("decoder."):
+                        w = w.view(4, 4, w.shape[0] // 16, w.shape[1]).permute(3, 2, 0, 1)
+                    else:
+                        w = w.view(w.shape[0], 4, 4, w.shape[1] // 16).permute(0, 3, 1, 2)
+                    w = w[:self._trim[key]] if key in self._trim else w
+                out[key] = w
         return out
 
     def torch_weights(self):
@@ -225,54 +270,74 @@ class DcganEngine:
         return t[:rows]
 
     # ------------------------------------------------------------------ generator
-    def g_forward(self, n, noise=None, seed=0, stream_id=0, tag="g"):
-        """G(z) for n samples -> (images [n*4096, ch] NHWC bf16, saved activations)."""
-        zb = self._buf(tag + "z", n, self.zp)
-        check(self.h, lib().gm_noise_rows(self.h, _ptr(noise), _ptr(zb), n, self.z, self.zp, int(seed), int(stream_id), _stream()))
-        sv = {"z": zb, "n": n}
+    def g_forward(self, n, noise=None, seed=0, stream_id=0, tag="g", net=None, pfx="", x_rows=None, out_mode=C2I_SIGMOID, run=None):
+        """G(z) for n samples -> (images [n*4096, ch] NHWC bf16, saved activations).  The same transposed-conv stack runs
+        BEGAN's decoder: net / pfx name its weights (default G), x_rows [n, >= K] bf16 are its input rows instead of the
+        noise rows, out_mode is the final col2im's (C2I_NONE: linear output) and run its BatchNorm running statistics."""
+        net = self.G if net is None else net
+        run = self.run_G if run is None else run
+        K = net.shapes[pfx + "l1.weight"][1]
+        if x_rows is None:
+            x_rows = self._buf(tag + "z", n, self.zp)
+            check(self.h, lib().gm_noise_rows(self.h, _ptr(noise), _ptr(x_rows), n, self.z, self.zp, int(seed), int(stream_id), _stream()))
+        sv = {"z": x_rows, "n": n}
         gc = self.gc
         c = self._buf(tag + "c0", n, 16 * gc[0])
-        gemm_bf16(zb, self.G.bf["l1.weight"], c, "nt", K=self.z)                           # [n, (kh,kw,co)] = NHWC [n*16, 8h]
+        gemm_bf16(x_rows, net.bf[pfx + "l1.weight"], c, "nt", K=K)                          # [n, (kh,kw,co)] = NHWC [n*16, 8h]
         x = c.view(n * 16, gc[0])
         hw = 4
         for i in range(4):
             a = self._buf(tag + "a%d" % i, x.shape[0], gc[i])
             st = self._buf(tag + "st%d" % i, 2, gc[i], torch.float32)
-            _bn_fwd(x, self.G.view("bn%d.weight" % (i + 1)), self.G.view("bn%d.bias" % (i + 1)), ACT_RELU, a, st, self.run_G[i])
+            _bn_fwd(x, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_RELU, a, st, run[i])
             sv["c%d" % i], sv["a%d" % i], sv["st%d" % i] = x, a, st
             col = self._buf(tag + "col%d" % i, a.shape[0], 16 * gc[i + 1])
-            gemm_bf16(a, self.G.bf["l%d.weight" % (i + 2)], col, "nt")
+            gemm_bf16(a, net.bf[pfx + "l%d.weight" % (i + 2)], col, "nt")
             y = self._buf(tag + "c%d" % (i + 1), n * 4 * hw * hw, gc[i + 1])
-            _col2im(col, n, hw, hw, gc[i + 1], y, C2I_SIGMOID if i == 3 else C2I_NONE)
+            _col2im(col, n, hw, hw, gc[i + 1], y, out_mode if i == 3 else C2I_NONE)
             x, hw = y, 2 * hw
         sv["img"] = x
         return x, sv
 
-    def g_backward(self, sv, dpre):
-        """dpre [n*4096, ch] = dL/d(pre-sigmoid output) -> flat G gradient (self.G.grads)."""
-        n, gc, G = sv["n"], self.gc, self.G
-        G.grads.zero_()
+    def g_backward(self, sv, dpre, net=None, pfx="", grads=None, need_wgrad=True, need_dx=False, tag="g"):
+        """dpre [n*4096, ch] = dL/d(pre-sigmoid output) -> flat G gradient (self.G.grads, zeroed first).  For BEGAN's decoder
+        (net / pfx, see g_forward) dpre is dL/d(linear output) and the weight gradients go to the flat D-layout `grads` when
+        need_wgrad; need_dx returns dL/d(input rows) [n, ep] bf16 instead (one more GEMM, with l1's transposed copy)."""
+        n, gc = sv["n"], self.gc
+        net = self.G if net is None else net
+        if grads is None and need_wgrad:
+            grads = net.grads
+            grads.zero_()
         d, hw = dpre, 64
         for i in range(3, -1, -1):
             hw //= 2                                                                      # input grid of transposed conv i+2
             a, c, st = sv["a%d" % i], sv["c%d" % i], sv["st%d" % i]
             dcol = self._buf("gdcol%d" % i, a.shape[0], 16 * gc[i + 1])
             _im2col(d, n, 2 * hw, 2 * hw, gc[i + 1], dcol)                                # gradient of col2im
-            gemm_bf16(dcol, a, G.view("l%d.weight" % (i + 2), G.grads), "tn")             # [16 Cout, Cin] = dcol^T a
+            if need_wgrad:
+                gemm_bf16(dcol, a, net.view(pfx + "l%d.weight" % (i + 2), grads), "tn")   # [16 Cout, Cin] = dcol^T a
             da = self._buf("gda%d" % i, a.shape[0], gc[i])
-            gemm_bf16(dcol, G.bf_t["l%d.weight" % (i + 2)], da, "nt")                     # da = dcol Wm
+            gemm_bf16(dcol, net.bf_t[pfx + "l%d.weight" % (i + 2)], da, "nt")             # da = dcol Wm
             dc = self._buf("gdc%d" % i, a.shape[0], gc[i])
             dgb = self._buf("gdgb%d" % i, 2, gc[i], torch.float32)
-            _bn_bwd(da, c, st, G.view("bn%d.weight" % (i + 1)), G.view("bn%d.bias" % (i + 1)), ACT_RELU, dc, dgb)
-            G.view("bn%d.bias" % (i + 1), G.grads).copy_(dgb[0])
-            G.view("bn%d.weight" % (i + 1), G.grads).copy_(dgb[1])
+            _bn_bwd(da, c, st, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_RELU, dc, dgb)
+            if need_wgrad:
+                net.view(pfx + "bn%d.bias" % (i + 1), grads).copy_(dgb[0])
+                net.view(pfx + "bn%d.weight" % (i + 1), grads).copy_(dgb[1])
             d = dc
-        gemm_bf16(d.view(n, 16 * gc[0]), sv["z"], G.view("l1.weight", G.grads), "tn", N=self.z)   # [(kh,kw,co), z]
-        return G.grads
+        w1 = pfx + "l1.weight"
+        if need_wgrad:
+            gemm_bf16(d.view(n, 16 * gc[0]), sv["z"], net.view(w1, grads), "tn", N=net.shapes[w1][1])   # [(kh,kw,co), z]
+        if not need_dx:
+            return grads
+        dx = self._buf(tag + "dx", n, net.shapes[w1][1])
+        gemm_bf16(d.view(n, 16 * gc[0]), net.bf_t[w1], dx, "nt")                             # [n, ep] = d Wm
+        return dx
 
     # ------------------------------------------------------------------ discriminator
-    def d_forward(self, img, n, logits, tag):
-        """D(img) for n NHWC images; logits: fp32 view [16, ld] (row 0 receives the n logits).  Returns saved activations."""
+    def d_forward(self, img, n, logits, tag, pfx=""):
+        """D(img) for n NHWC images; logits: fp32 view [16, ld] (row 0 receives the n logits), or a bf16 [n, ep] buffer that
+        receives BEGAN's linear embedding (pfx "encoder.").  Returns saved activations."""
         dc = self.dc
         sv = {"n": n, "img": img}
         x, hw, cin = img, 64, self.ch
@@ -283,29 +348,35 @@ class DcganEngine:
             c = self._buf(tag + "c%d" % i, n * hw * hw, dc[i])
             sv["col%d" % i] = col
             if i == 0 or not self.d_bn:
-                gemm_bf16(col, self.D.bf["l%d.weight" % (i + 1)], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU epilogue
+                gemm_bf16(col, self.D.bf[pfx + "l%d.weight" % (i + 1)], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU epilogue
                 y = c
             else:
-                gemm_bf16(col, self.D.bf["l%d.weight" % (i + 1)], c, "nt")
+                gemm_bf16(col, self.D.bf[pfx + "l%d.weight" % (i + 1)], c, "nt")
                 y = self._buf(tag + "y%d" % i, c.shape[0], dc[i])
                 st = self._buf(tag + "st%d" % i, 2, dc[i], torch.float32)
-                _bn_fwd(c, self.D.view("bn%d.weight" % (i + 1)), self.D.view("bn%d.bias" % (i + 1)), ACT_LRELU, y, st, self.run_D[i])
+                _bn_fwd(c, self.D.view(pfx + "bn%d.weight" % (i + 1)), self.D.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, st,
+                        self.run_D[i])
                 sv["c%d" % i], sv["st%d" % i] = c, st
             sv["y%d" % i] = y
             x, cin = y, dc[i]
         flat = x.view(n, 16 * dc[3])
         sv["flat"] = flat
-        gemm_bf16(flat, self.D.bf["l5.weight"], logits, "nt", transpose=True)             # fp32 [16, ld]: row 0 = logits
+        # fp32 [16, ld] with row 0 = logits, or the bf16 embedding rows [n, ep]
+        gemm_bf16(flat, self.D.bf[pfx + "l5.weight"], logits, "nt", transpose=logits.dtype == torch.float32)
         return sv
 
-    def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d"):
-        """ds [n] fp32 = dL/dlogit.  Accumulates nothing: writes this pass's D gradient into `grads` (flat, D layout) when
-        need_wgrad; returns dL/d(pre-sigmoid generator output) when need_dimg (img must then be a generator output)."""
+    def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d", pfx="", dimg_mode=C2I_SIGMOID_GRAD):
+        """ds [n] fp32 = dL/dlogit, or a bf16 [n, ep] upstream gradient of BEGAN's embedding (pfx "encoder.").  Accumulates
+        nothing: writes this pass's D gradient into `grads` (flat, D layout) when need_wgrad; returns dL/d(pre-sigmoid
+        generator output) (dimg_mode C2I_SIGMOID_GRAD) or dL/d(image) (C2I_NONE) when need_dimg."""
         n, dc, D = sv["n"], self.dc, self.D
-        dy5 = self._buf(tag + "dy5", n, 16)
-        check(self.h, lib().gm_pack_col0(self.h, _ptr(ds), n, _ptr(dy5), 16, _stream()))
+        if ds.dtype == torch.bfloat16:
+            dy5 = ds
+        else:
+            dy5 = self._buf(tag + "dy5", n, 16)
+            check(self.h, lib().gm_pack_col0(self.h, _ptr(ds), n, _ptr(dy5), 16, _stream()))
         if need_wgrad:
-            gemm_bf16(dy5, sv["flat"], D.view("l5.weight", grads), "tn")                  # [16, 128h]
+            gemm_bf16(dy5, sv["flat"], D.view(pfx + "l5.weight", grads), "tn")            # [16 (ep), 128h]
         if not self.d_bn:
             betas = self._betas(sv, dy5, tag)
             if need_wgrad:
@@ -313,34 +384,34 @@ class DcganEngine:
                     gemm_bf16(betas[i], sv["col%d" % i], D.view("l%d.weight" % (i + 1), grads), "tn")
             return self._dimg(sv, betas[0], tag) if need_dimg else None
         dflat = self._buf(tag + "dflat", n, 16 * dc[3])
-        gemm_bf16(dy5, D.bf_t["l5.weight"], dflat, "nt", K=16)
+        gemm_bf16(dy5, D.bf_t[pfx + "l5.weight"], dflat, "nt", K=dy5.shape[1])
         d, hw = dflat.view(n * 16, dc[3]), 4
         for i in range(3, 0, -1):
             c, st, col = sv["c%d" % i], sv["st%d" % i], sv["col%d" % i]
             dcv = self._buf(tag + "dc%d" % i, c.shape[0], dc[i])
             dgb = self._buf(tag + "dgb%d" % i, 2, dc[i], torch.float32)
-            _bn_bwd(d, c, st, D.view("bn%d.weight" % (i + 1)), D.view("bn%d.bias" % (i + 1)), ACT_LRELU, dcv, dgb)
+            _bn_bwd(d, c, st, D.view(pfx + "bn%d.weight" % (i + 1)), D.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, dcv, dgb)
             if need_wgrad:
-                D.view("bn%d.bias" % (i + 1), grads).copy_(dgb[0])
-                D.view("bn%d.weight" % (i + 1), grads).copy_(dgb[1])
-                gemm_bf16(dcv, col, D.view("l%d.weight" % (i + 1), grads), "tn")          # [Cout, 16 Cin]
+                D.view(pfx + "bn%d.bias" % (i + 1), grads).copy_(dgb[0])
+                D.view(pfx + "bn%d.weight" % (i + 1), grads).copy_(dgb[1])
+                gemm_bf16(dcv, col, D.view(pfx + "l%d.weight" % (i + 1), grads), "tn")    # [Cout, 16 Cin]
             dcol = self._buf(tag + "dcol%d" % i, col.shape[0], col.shape[1])
-            gemm_bf16(dcv, D.bf_t["l%d.weight" % (i + 1)], dcol, "nt")
+            gemm_bf16(dcv, D.bf_t[pfx + "l%d.weight" % (i + 1)], dcol, "nt")
             dprev = self._buf(tag + "dprev%d" % i, n * 4 * hw * hw, dc[i - 1])
             # layer i's input is y_{i-1}: a BN layer's output (its backward applies LeakyReLU') or, for i == 1, lrelu(c_0)
             _col2im(dcol, n, hw, hw, dc[i - 1], dprev, C2I_LRELU_GRAD if i == 1 else C2I_NONE, sv["y0"] if i == 1 else None)
             d, hw = dprev, 2 * hw
         if need_wgrad:
-            gemm_bf16(d, sv["col0"], D.view("l1.weight", grads), "tn")                    # [h, 16 ch]
+            gemm_bf16(d, sv["col0"], D.view(pfx + "l1.weight", grads), "tn")              # [h, 16 ch]
         if not need_dimg:
             return None
-        return self._dimg(sv, d, tag)
+        return self._dimg(sv, d, tag, dimg_mode, pfx)
 
-    def _dimg(self, sv, d, tag, mode=C2I_SIGMOID_GRAD):
+    def _dimg(self, sv, d, tag, mode=C2I_SIGMOID_GRAD, pfx=""):
         """d = dL/d(conv 1 output) -> dL/d(image) (mode C2I_NONE) or dL/d(pre-sigmoid generator output) (C2I_SIGMOID_GRAD)"""
         n = d.shape[0] // 1024
         dcol = self._buf(tag + "dcol0", d.shape[0], 16 * self.ch)
-        gemm_bf16(d, self.D.bf_t["l1.weight"], dcol, "nt")
+        gemm_bf16(d, self.D.bf_t[pfx + "l1.weight"], dcol, "nt")
         dpre = self._buf(tag + ("dpre" if mode == C2I_SIGMOID_GRAD else "dimg"), n * 4096, self.ch)
         _col2im(dcol, n, 32, 32, self.ch, dpre, mode, sv["img"] if mode == C2I_SIGMOID_GRAD else None)
         return dpre
@@ -421,6 +492,8 @@ class DcganEngine:
         lam = self.gp_lambda if gp_lambda is None else float(gp_lambda)
         stat_batch = n if stat_batch is None else int(stat_batch)
         fake, _ = self.g_forward(n, noise, seed, 2 * step)
+        if self.variant == "be":
+            return self._began_d_grad(img_real, fake, n, inv, stat_batch)
         if self.variant == "wgp":
             return self.wgp_critic_grad(img_real, fake, n, inv, lam, eps, seed, step)
         if self.variant == "dra":
@@ -558,6 +631,8 @@ class DcganEngine:
         """train_G + backward (src/ns_gan.py:196-216,155): G gradients only."""
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         fake, gsv = self.g_forward(n, noise, seed, 2 * step + 1)
+        if self.variant == "be":
+            return self._began_g_grad(fake, gsv, n, inv)
         logits = self._buf("logits_g", 16, n, torch.float32)
         sf = self.d_forward(fake, n, logits, "df")
         ds = self._buf("ds_g", 1, n, torch.float32)[0]
@@ -567,7 +642,98 @@ class DcganEngine:
         return self.loss_buf[1]
 
     def apply(self, net, hp):
-        (self.G if net == 0 else self.D).adam(hp)
+        # BEGAN: both learning rates carry the plateau scale be_state[7]; the reference's two schedulers see the same
+        # measure with the same settings (src/be_gan.py:133-136,194-195), so one scale is exact
+        (self.G if net == 0 else self.D).adam(hp, self.be_state[7:8] if self.variant == "be" else None)
+
+    # ------------------------------------------------------------------ BEGAN (src/be_gan.py:212-258)
+    def began_state(self, values=None):
+        """BEGAN device state (11 floats, the layout of gm_gan_began_state): set (values given) or read"""
+        if values is not None:
+            self.be_state.copy_(torch.tensor([float(v) for v in values]))
+            return list(values)
+        return self.be_state.tolist()
+
+    def began_init(self, K, batch):
+        """K, a fresh plateau scheduler (best = inf, lr scale 1) and the MLP layout's scale fields for `batch` images"""
+        inv = 1.0 / batch
+        return self.began_state([K, inv, -K * inv, 0.0, 0.0, float("inf"), 0.0, 1.0, inv, inv, 0.0])
+
+    def began_control(self, gamma, lam, patience):
+        """K <- clip(K + lam (gamma DX - DG), 0, 1), the convergence measure and the ReduceLROnPlateau pair on the device
+        (src/be_gan.py:186-195), from the DX, DG of the last D step"""
+        check(self.h, lib().gm_began_control(self.h, _ptr(self.be_state), float(gamma), float(lam), float(patience), _stream()))
+
+    def l1_rows(self, r, x, n, inv, coef, grad, total):
+        """BEGAN's L1 term on n NHWC images: grad = sign(r - x) inv (coef[0] if coef is given) as bf16, total[0] = sum |r - x|"""
+        check(self.h, lib().gm_l1_rows(self.h, _ptr(r), _ptr(x), n, 4096 * self.ch, float(inv), _ptr(coef), _ptr(grad), _ptr(total),
+                                       _stream()))
+
+    def began_loss_final(self, sums, batch, g_step, loss):
+        """sums (float64 [2]: this process's sum |D(x) - x|, sum |D(G(z)) - G(z)|) -> loss[0]: D step (summed over the ranks
+        by stats_reduce first; batch = the global batch) DX - K DG with be_state[3], [4] = DX, DG; G step DG"""
+        if not g_step:
+            self._reduce_stats(sums)
+        check(self.h, lib().gm_began_loss_final(self.h, _ptr(sums[0:1]), _ptr(sums[1:2]), int(batch), int(g_step), _ptr(self.be_state),
+                                                _ptr(loss), _stream()))
+
+    def autoencode(self, x, n, tag="be"):
+        """D(x) = decoder(encoder(x)) for n NHWC images -> (reconstruction [n*4096, ch] bf16, encoder and decoder saved
+        activations).  Each call takes its own BatchNorm batch statistics."""
+        emb = self._buf(tag + "emb", n, self.ep)
+        sve = self.d_forward(x, n, emb, tag + "e", "encoder.")
+        rec, svd = self.g_forward(n, tag=tag + "d", net=self.D, pfx="decoder.", x_rows=emb, out_mode=C2I_NONE, run=self.run_dec)
+        return rec, sve, svd
+
+    def _autoencoder_backward(self, sve, svd, dr, grads, tag="be"):
+        """dr = dL/d(reconstruction) -> the autoencoder's weight gradients into `grads` (flat D layout)"""
+        demb = self.g_backward(svd, dr, self.D, "decoder.", grads, need_dx=True, tag=tag + "d")
+        self.d_backward(sve, demb, grads, tag=tag + "e", pfx="encoder.")
+
+    def _began_d_grad(self, img_real, fake, n, inv, stat_batch):
+        """train_D + backward (src/be_gan.py:212-238): D_loss = DX - K DG.  The real and the generated half each run the
+        autoencoder, the L1 kernel and the backward in turn (sharing buffers); the fake half's gradient carries -K inv with K
+        read on the device.  The two sums then meet the ranks' (stats_reduce) in the loss finalisation."""
+        sums = self._buf("be_sums", 1, 2, torch.float64)[0]
+        g2 = self._buf("dgrad2", 1, self.D.total, torch.float32)[0]
+        self.D.grads.zero_()
+        g2.zero_()
+        drs = []
+        for k, (x, grads) in enumerate(((img_real, self.D.grads), (fake, g2))):
+            rec, sve, svd = self.autoencode(x, n)
+            dr = self._buf("be_dr%d" % k, n * 4096, self.ch)
+            self.l1_rows(rec, x, n, inv if k == 0 else -inv, None if k == 0 else self.be_state[0:1], dr, sums[k:k + 1])
+            self._autoencoder_backward(sve, svd, dr, grads)
+            drs.append(dr)
+        self.D.grads.add_(g2)
+        self.began_loss_final(sums, stat_batch, 0, self.loss_buf[0:1])
+        self.be_sums_, self.be_dr_ = sums, drs                       # this process's L1 sums (before stats_reduce), dL/dr
+        return self.loss_buf[0]
+
+    def _began_g_grad(self, fake, gsv, n, inv):
+        """train_G + backward (src/be_gan.py:240-258): G_loss = mean_i sum |D(G(z)) - G(z)|, whose gradient reaches G(z) through
+        D (T, the autoencoder's input-gradient chain without weight gradients) and directly through the target (-dr).  The
+        gradients carry inv (1 / the global batch); the reported G loss is this process's mean, like every G loss of the conv
+        path (only the D step's DX and DG are global: K and the lr scale must agree on every rank)."""
+        sums = self._buf("be_sums_g", 1, 2, torch.float64)[0]
+        rec, sve, svd = self.autoencode(fake, n)
+        dr = self._buf("be_drg", n * 4096, self.ch)
+        self.l1_rows(rec, fake, n, inv, None, dr, sums[1:2])
+        self.began_loss_final(sums, n, 1, self.loss_buf[1:2])
+        demb = self.g_backward(svd, dr, self.D, "decoder.", need_wgrad=False, need_dx=True, tag="bed")
+        T = self.d_backward(sve, demb, None, need_wgrad=False, need_dimg=True, tag="bee", pfx="encoder.", dimg_mode=C2I_NONE)
+        dpre = self._buf("be_dpre", n * 4096, self.ch)
+        check(self.h, lib().gm_began_dfake_rows(self.h, _ptr(T), _ptr(dr), _ptr(fake), _ptr(dpre), n, 4096 * self.ch, _stream()))
+        self.g_backward(gsv, dpre)
+        # the step's stored tensors: dL/dr, the autoencoder's saved activations, the embedding gradient, T, dpre, G's activations
+        self.be_drg_, self.be_g_saved_ = dr, dict(sve=sve, svd=svd, demb=demb, T=T, dpre=dpre, gsv=gsv, fake=fake)
+        return self.loss_buf[1]
+
+    def reconstruct(self, images):
+        """BEGAN's D(images): flat [n, ch*64*64] (NCHW flattened) -> the reconstructions in the same layout (fp32)"""
+        n = images.shape[0]
+        rec, _, _ = self.autoencode(self.stage_images(images), n, "ber")
+        return rec.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
 
     def generate(self, noise):
         n = noise.shape[0]

@@ -102,6 +102,10 @@ int gm_gemm_bf16(gm_ctx* ctx, const gm_gemm_desc* d, gm_stream stream);
  * step count (bias correction).  Replaces optim.Adam.step (src/ns_gan.py:139,156). */
 int gm_adam_step(gm_ctx* ctx, float* p_dev, const float* g_dev, float* m_dev, float* v_dev, int n,
                  const gm_adam_hp* hp, int step, gm_stream stream);
+/* gm_adam_step with the learning rate hp->lr * lr_scale_dev[0] (a device scalar, e.g. BEGAN's plateau scheduler, read at
+ * run time); lr_scale_dev NULL is gm_adam_step. */
+int gm_adam_step_lr(gm_ctx* ctx, float* p_dev, const float* g_dev, float* m_dev, float* v_dev, int n,
+                    const gm_adam_hp* hp, const float* lr_scale_dev, int step, gm_stream stream);
 
 /* ---- GAN train-step engine --------------------------------------------------
  * MLP generator z -> hidden -> image (sigmoid) and discriminator image -> hidden
@@ -366,6 +370,20 @@ int gm_dra_xhat_rows(gm_ctx* ctx, const void* x_dev, int rows, int cols, int ld,
 int gm_dra_penalty(gm_ctx* ctx, const void* J_dev, int ldj, const void* xhat_dev, int ldx, const float* logits_dev, int B, int HW, int C,
                    float lambda, float K, float inv_grad, float inv_loss, void* r_dev, int ldr, float* norm_dev, float* loss_dev,
                    gm_stream stream);
+/* BEGAN (src/be_gan.py:212-258) on the conv autoencoder D; images are contiguous rows [rows, cols] (cols a multiple of 8,
+ * 16-byte aligned).  gm_l1_rows: grad_dev = sign(r - x) inv (coef_dev ? coef_dev[0] : 1) as bf16 (sign(0) = 0) and
+ * sum_dev[0] = sum |r - x| (one double, a fixed-order reduction, for data-parallel ranks to SUM).  gm_began_loss_final: from
+ * the summed doubles over `batch` (the global batch) images, D step: loss_dev[0] = DX - K DG, state [3], [4] = DX, DG; G step
+ * (g_step != 0, sum_x_dev unused): loss_dev[0] = DG.  gm_began_control: K and the ReduceLROnPlateau pair on a caller-owned
+ * state_dev[11] (the layout of gm_gan_began_state).  gm_began_dfake_rows: out = (T - dr) f (1 - f), the G step's
+ * dL/d(pre-sigmoid G output) from T = D's input gradient at f = G(z) and dr = gm_l1_rows' grad. */
+int gm_l1_rows(gm_ctx* ctx, const void* r_dev, const void* x_dev, int rows, int cols, float inv, const float* coef_dev, void* grad_dev,
+               double* sum_dev, gm_stream stream);
+int gm_began_loss_final(gm_ctx* ctx, const double* sum_x_dev, const double* sum_g_dev, int batch, int g_step, float* state_dev,
+                        float* loss_dev, gm_stream stream);
+int gm_began_control(gm_ctx* ctx, float* state_dev, float gamma, float lambda, float patience, gm_stream stream);
+int gm_began_dfake_rows(gm_ctx* ctx, const void* T_dev, const void* dr_dev, const void* fake_dev, void* out_dev, int rows, int cols,
+                        gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);

@@ -1,4 +1,4 @@
-"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP and DRAGAN train steps (D_steps = 1) on one GPU, in one process.
+"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP, DRAGAN and BEGAN train steps (D_steps = 1) on one GPU, in one process.
 
     python tools/bench_dcgan.py [--batch 1024] [--steps 20] [--warmup 5]
 
@@ -8,7 +8,9 @@ device-resident binarised synthetic images (each value 1 with probability 0.3), 
 all alike.  Prints one JSON line: device name and power limit (read in the same run), and per variant the median step
 time, images/s, library launches per step, the ratio to NSGAN and achieved TFLOP/s from FLOPs counted from the shapes
 (bench.py's _dcgan_flop_per_img; the penalised critics of WGAN-GP and DRAGAN add one critic forward, one input-gradient
-chain to the image, one tangent forward and one weight-gradient pass = 4 critic forwards).  Writes nothing but stdout.
+chain to the image, one tangent forward and one weight-gradient pass = 4 critic forwards; BEGAN's from its autoencoder's
+shapes, began_flop_per_img).  BEGAN's step includes began_control, as its trainer runs it after every G update.  Writes
+nothing but stdout.
 """
 import argparse
 import json
@@ -21,14 +23,30 @@ for p in (ROOT, os.path.join(ROOT, "generative-models_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-VARIANTS = ("ns", "ra", "fisher", "wgp", "dra")
-LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4}     # the reference's defaults per variant
+VARIANTS = ("ns", "ra", "fisher", "wgp", "dra", "be")
+LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4, "be": 1e-4}     # the reference's defaults per variant
 
 
 def critic_flop_per_img(hd=64, ch=3):
     dc = [hd, 2 * hd, 4 * hd, 8 * hd]
     d_l = [1024 * dc[0] * 16 * ch, 256 * dc[1] * 16 * dc[0], 64 * dc[2] * 16 * dc[1], 16 * dc[3] * 16 * dc[2], 16 * dc[3]]
     return 2.0 * sum(d_l)
+
+
+def began_flop_per_img(hd=64, z=100, e=100, ch=3):
+    """algorithmic FLOPs of one BEGAN step, counted like bench.py's _dcgan_flop_per_img: D step = G fwd + 2 autoencoder fwd +
+    2 autoencoder bwd (weight grads everywhere, input grads down to the encoder's first layer); G step = G fwd + autoencoder
+    fwd + its input-gradient chain down to the image + G bwd"""
+    gc, dc = [8 * hd, 4 * hd, 2 * hd, hd, ch], [hd, 2 * hd, 4 * hd, 8 * hd]
+    enc = [1024 * dc[0] * 16 * ch, 256 * dc[1] * 16 * dc[0], 64 * dc[2] * 16 * dc[1], 16 * dc[3] * 16 * dc[2], 16 * dc[3] * e]
+    g_l = [z * 16 * gc[0], 16 * gc[0] * 16 * gc[1], 64 * gc[1] * 16 * gc[2], 256 * gc[2] * 16 * gc[3], 1024 * gc[3] * 16 * gc[4]]
+    dec = [e * 16 * gc[0]] + g_l[1:]
+    ae = sum(enc) + sum(dec)
+    Gf, AEf = 2.0 * sum(g_l), 2.0 * ae
+    ae_bwd = 2.0 * (2 * ae - enc[0])                 # wgrad everywhere + dgrad except into the image
+    ae_dgrad = 2.0 * ae                              # G step: input-gradient chain only, down to the image
+    g_bwd = 2.0 * (2 * sum(g_l) - g_l[0])
+    return (Gf + 2 * AEf + 2 * ae_bwd) + (Gf + AEf + ae_dgrad + g_bwd)
 
 
 def power_limit(index):
@@ -63,6 +81,8 @@ def main():
         eng.apply(1, hp)
         eng.g_grad(B, seed=1000, step=s)
         eng.apply(0, hp)
+        if name == "be":
+            eng.began_control(0.5, 1e-3, 5 * 4)                 # GAMMA, LAMBDA, patience 5 len(train_iter) of src/be_gan.py
 
     launches = {}
     for name in VARIANTS:
@@ -89,7 +109,10 @@ def main():
            "warmup": a.warmup}
     for name in VARIANTS:
         med = sorted(ms[name])[len(ms[name]) // 2]
-        flop = _dcgan_flop_per_img() + (4 * critic_flop_per_img() if name in ("wgp", "dra") else 0.0)
+        if name == "be":
+            flop = began_flop_per_img()
+        else:
+            flop = _dcgan_flop_per_img() + (4 * critic_flop_per_img() if name in ("wgp", "dra") else 0.0)
         out[name] = {"median_ms": round(med, 3), "min_ms": round(min(ms[name]), 3), "images_per_s": round(B / med * 1e3, 1),
                      "launches_per_step": launches[name], "gflop_per_image": round(flop / 1e9, 3),
                      "tflops": round(flop * B / med / 1e9, 1), "last_losses": [float(v) for v in engines[name].loss_buf.tolist()]}
