@@ -100,7 +100,7 @@ enum PlanKind { PK_NT_208 = 0, PK_NT_64, PK_TN_256, PK_TN_64 };
 struct GemmPlan {
   CUtensorMap tmA, tmB;
   CUtensorMap tmA2, tmB2;   // residual (lo) planes of the operands in split mode, else copies of tmA / tmB
-  // output map of the K-major bf16 kernels (32 x 32 box, 64-byte swizzle), encoded at the first
+  // output map of the K-major bf16 kernels (16-row x 32-column box, 64-byte swizzle), encoded at the first
   // launch because the epilogue (output pointer / leading dimension) is set after plan_gemm
   mutable CUtensorMap tmC;
   mutable int tmc_state;   // 0: not encoded yet, 1: in use, 2: output not eligible (STG path)
@@ -223,7 +223,7 @@ static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
     const bool plain = p.aux_mode == AUX_NONE && p.dot_w == nullptr && p.dot_sq == 0;
     if (g_tma_store && nt && plain && p.nparts == 1 && p.epi == EPI_BF16 && p.out != nullptr && !(reinterpret_cast<uintptr_t>(p.out) & 15) &&
         (p.ldo * 2) % 16 == 0 && p.out_cols > 0) {
-      int rc = make_tmap(c, &pl.tmC, p.out, uint64_t(p.out_cols), uint64_t(p.M), uint64_t(p.ldo), kEpiCols, 32, CU_TENSOR_MAP_SWIZZLE_64B);
+      int rc = make_tmap(c, &pl.tmC, p.out, uint64_t(p.out_cols), uint64_t(p.M), uint64_t(p.ldo), kEpiCols, kEpiRows, CU_TENSOR_MAP_SWIZZLE_64B);
       if (rc) return rc;
       pl.tmc_state = 1;
     }

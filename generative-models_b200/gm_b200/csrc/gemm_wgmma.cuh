@@ -9,14 +9,15 @@
 //                                                   -> dW GEMMs (A^T * B)
 // Tiles: 128 x BN x 64, 128-byte TMA / wgmma swizzle, one m64nBNk16 wgmma per warpgroup and k-step.
 //
-// Warp roles (288 threads): warps 0..7 = two consumer warpgroups, warp 8 = TMA producer.
-// Consumer warpgroup g accumulates rows [64 g, 64 g + 64) of the tile in registers; at the end
-// of the tile both warpgroups write their accumulators to one fp32 tile in shared memory (row
-// r = thread r of a warp quarter, as the epilogue reads it) and the same 8 warps run the fused
-// epilogue from there: warp w serves rows 32 (w & 3) .. + 31 and every other 32-column block
-// (parity w >> 2).  Meanwhile the producer keeps filling the smem ring with the next tile's
-// operands.  Pipelines: smem ring full/empty mbarriers (TMA <-> wgmma), named barriers around
-// the shared accumulator tile, static round-robin tile scheduler (grid = #SMs).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected lane of warp 0 issues; the
+// warpgroup gives its registers away with setmaxnreg), warpgroups 1..2 = consumers.
+// Consumer warpgroup g accumulates rows [64 g, 64 g + 64) of the tile in registers and runs the
+// fused epilogue straight from them: each consumer warp owns the 16 rows its fragments hold and
+// walks the tile in 64-column steps.  Per step the warp writes its fragments to a private 4 KB
+// fp32 scratch tile, and lane L takes row L & 15 and the 32-column block of parity L >> 4 through
+// the per-row epilogue; the scratch is then reused as the bf16 staging of the store.  Meanwhile
+// the producer keeps filling the smem ring with the next tile's operands.  Pipelines: smem ring
+// full/empty mbarriers (TMA <-> wgmma), static round-robin tile scheduler (grid = #SMs).
 #pragma once
 #include "ptx.cuh"
 
@@ -25,9 +26,15 @@ namespace gm {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int kMmaK = 16;
-constexpr int kConsumerWarps = 8;                        // two warpgroups: wgmma, then the epilogue
-constexpr int kGemmThreads = (kConsumerWarps + 1) * 32;  // + the TMA producer warp
-constexpr int kSmemBudget = 227 * 1024;                  // H100: opt-in dynamic shared memory per block
+constexpr int kProducerThreads = 128;                               // warpgroup 0: TMA producer
+constexpr int kConsumerWarps = 8;                                   // warpgroups 1..2: wgmma, then the epilogue
+constexpr int kGemmThreads = kProducerThreads + kConsumerWarps * 32;
+// setmaxnreg budget: 384 threads launch with 168 registers each; the producer drops to 40 so the consumers can hold a
+// 128 x 208 (or 256) fp32 accumulator next to the epilogue's registers
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(kProducerThreads * kProducerRegs + kConsumerWarps * 32 * kConsumerRegs <= 65536, "register file");
+constexpr int kSmemBudget = 227 * 1024;                             // H100: opt-in dynamic shared memory per block
 
 enum : int { EPI_BF16 = 0, EPI_F32 = 1 };
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2, ACT_LRELU = 3 };   // LeakyReLU(act_slope): universal epilogue only
@@ -87,14 +94,19 @@ struct GemmParams {
   float act_slope;      // ACT_LRELU
 };
 
-// per-epilogue-warp staging tile for one 32-column block: 32 rows x (64 B data + 16 B pad):
-// conflict-free row-wise writes (thread = row), row-contiguous reads (4 lanes = 64 B of a row)
-constexpr int kEpiCols = 32;
-constexpr int kEpiPitch = 80;
-constexpr int kEpiStageBytes = 32 * kEpiPitch;
-constexpr int kEpiVecBlocks = 8;                       // column blocks per warp the bias/dot staging holds
+// Epilogue of one consumer warp: 16 rows (its fragments) x 64-column steps, one 32-column block per lane and step.
+// Its scratch tile holds a step's fp32 fragments (16-byte chunks of row r XOR-swizzled by frag_swz(r): conflict-free
+// 8-byte fragment stores and 16-byte row reads), then the step's bf16 staging: 16 rows x (128 B data + 16 B pad) for
+// LDS + STG, or two 16 x 32 TMA-store boxes (64-byte rows, 64B swizzle) at 0 and 1 KB.
+constexpr int kEpiRows = 16;
+constexpr int kEpiStep = 64;
+constexpr int kEpiCols = 32;                           // columns of one lane's block (the TMA-store box width)
+constexpr int kEpiScratchBytes = kEpiRows * kEpiStep * 4;
+constexpr int kEpiPitch = 144;
+constexpr int kEpiVecBlocks = 8;                       // 32-column blocks of a tile the bias/dot staging holds
 constexpr int kEpiVecBytes = kEpiVecBlocks * kEpiCols * 4 * 2;   // bias + row-dot weights
-constexpr int kParts = 2;                              // column-block parities of a tile (warp >> 2)
+static_assert(kEpiRows * kEpiPitch <= kEpiScratchBytes && 2 * kEpiRows * kEpiCols * 2 <= kEpiScratchBytes, "staging");
+__device__ __forceinline__ uint32_t frag_swz(int r) { return uint32_t(((r & 3) << 1) | ((r >> 2) & 1)); }
 
 // Phase timing (tools/time_phases.py) is compiled in only with -DGM_PHASE_TIMING.
 #ifdef GM_PHASE_TIMING
@@ -108,41 +120,27 @@ constexpr bool kPhaseTiming = false;
 template <int BN_, bool STAGED_EPI = true>
 struct GemmCfg {
   static constexpr int BN = BN_;
-  // fp32 accumulator tile [BM][BN] in shared memory; the 16-byte chunks of row r are XOR-swizzled by r & ACC_SWZ
-  // so that the row-per-lane reads of the epilogue hit 2 (BN = 208) or 1 (BN % 32 == 0) bank wavefronts per phase
-  static constexpr int ACC_SWZ = (BN / 4) % 8 == 0 ? 7 : 3;
-  static constexpr int ACC_BYTES = BM * BN * 4;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // per-warp staging tile + per-warp copies of its blocks' bias / row-dot weight slices
-  static constexpr int EPI_BYTES = STAGED_EPI ? kConsumerWarps * (kEpiStageBytes + kEpiVecBytes) : 0;
+  // per-warp scratch / staging tile (+ per-warp copies of the tile's bias / row-dot weights in the K-major kernels)
+  static constexpr int EPI_BYTES = kConsumerWarps * (kEpiScratchBytes + (STAGED_EPI ? kEpiVecBytes : 0));
   static_assert(!STAGED_EPI || (BN + kEpiCols - 1) / kEpiCols <= kEpiVecBlocks, "bias/dot staging too small");
-  static constexpr int FIXED_BYTES = 1024 + 512 + ACC_BYTES + EPI_BYTES;   // 1024: alignment slack; 512: barriers
+  static constexpr int FIXED_BYTES = 1024 + 512 + EPI_BYTES;   // 1024: alignment slack; 512: barriers
   static constexpr int STAGES_RAW = (kSmemBudget - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;   // staging tiles stay 512-B aligned (TMA 64B swizzle)
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;   // scratch tiles stay 512-B aligned (TMA 64B swizzle)
   static constexpr int BOXN = BN;   // K-major B: one box of BN rows
   static_assert(BN % 16 == 0 && BN <= 256, "wgmma N constraint (and 16-column epilogue chunks)");
   static_assert(STAGES >= 2, "need a pipeline");
+  static_assert(BN < 208 || STAGES >= 4, "the 208- and 256-wide kernels need a 4-stage ring to hide TMA latency");
 };
-
-// 16 consecutive fp32 accumulator columns of one row of the shared accumulator tile
-template <int BN, int SWZ>
-__device__ __forceinline__ void acc_ld16(uint32_t acc_s, int row, int col, uint32_t (&r)[16]) {
-  const uint32_t rb = acc_s + uint32_t(row) * (BN * 4);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint4 v = lds128(rb + ((uint32_t((col >> 2) + i) ^ uint32_t(row & SWZ)) << 4));
-    r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
-  }
-}
 
 // Epilogue specialisation: ACT_T / AUX_T / BIAS_T / DOT_T >= 0 fix the fused epilogue at
 // compile time (small code: the whole kernel must stay inside the instruction cache);
 // -1 selects the universal variant that reads the choice from GemmParams at run time.
 template <int BN, bool A_MN, bool B_MN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false>
-// 9 warps: one of the four SM sub-partitions holds 3 of them, so a warp may use at most 16 K / 3 / 32 -> 168 registers
+// 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA2,
@@ -150,7 +148,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   static_assert(!SPLIT || ACT_T < 0, "split operands: universal epilogue only");
   using Cfg = GemmCfg<BN, !A_MN>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int SWZ = Cfg::ACC_SWZ;
   static_assert(!B_MN || BN % 64 == 0, "MN-major B needs 64-wide atoms");
 
   extern __shared__ uint8_t smem_raw[];
@@ -158,14 +155,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t acc_s = bar_base + 512u;                        // fp32 accumulator tile
-  const uint32_t epi_base = acc_s + Cfg::ACC_BYTES;              // per-warp staging tiles, then bias / row-dot slices
+  const uint32_t epi_base = bar_base + 512u;   // per-warp scratch tiles, then bias / row-dot slices
 
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0);   // provably warp-uniform (wgmma issue)
   const int lane = threadIdx.x & 31;
 
   griddep_launch();   // the next grid may start its prologue as soon as SMs free up
-  if (warp == kConsumerWarps && lane == 0) {
+  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if constexpr (SPLIT) { tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB2); }
@@ -182,57 +178,62 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int tiles = p.m_tiles * p.n_tiles;   // work items walk (split, m-tile, n-tile)
   const int total = tiles * p.splits;
 
-  if (warp == kConsumerWarps) {
+  if (warp < kProducerThreads / 32) {
     // =========================== TMA producer ===========================
-    // The whole warp walks the loop (warp-uniform control flow and addresses keep the TMA
-    // operands in uniform registers); one elected lane issues.
-    int stage = 0;
-    uint32_t phase = 0;
-    const bool leader = elect_one();
-    for (int item = blockIdx.x; item < total; item += gridDim.x) {
-      const int split = item / tiles;
-      const int rem = item - split * tiles;
-      const int m0 = (rem / p.n_tiles) * BM;
-      const int n0 = (rem % p.n_tiles) * BN;
-      const int kb0 = split * p.kb_per_split;
-      const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        if (leader) {
-          const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t b_dst = a_dst + Cfg::A_BYTES;
-          int kk = kb, opart = 0;
-          if constexpr (SPLIT) { opart = kb / p.kb_part; kk = kb - opart * p.kb_part; }
-          const CUtensorMap* const ta = (SPLIT && opart == 2) ? &tmA2 : &tmA;   // (hi,hi), (hi,lo), (lo,hi)
-          const CUtensorMap* const tb = (SPLIT && opart == 1) ? &tmB2 : &tmB;
-          const int k0 = kk * BK;
-          mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-          if constexpr (!A_MN) {
-            tma_load_2d(a_dst, ta, full_bar(stage), k0, m0);
-          } else {
+    // Warp 0 walks the loop (warp-uniform control flow and addresses keep the TMA operands in
+    // uniform registers); one elected lane issues.  Warps 1..3 only release their registers.
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const bool leader = elect_one();
+      for (int item = blockIdx.x; item < total; item += gridDim.x) {
+        const int split = item / tiles;
+        const int rem = item - split * tiles;
+        const int m0 = (rem / p.n_tiles) * BM;
+        const int n0 = (rem % p.n_tiles) * BN;
+        const int kb0 = split * p.kb_per_split;
+        const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1u);
+          if (leader) {
+            const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
+            const uint32_t b_dst = a_dst + Cfg::A_BYTES;
+            int kk = kb, opart = 0;
+            if constexpr (SPLIT) { opart = kb / p.kb_part; kk = kb - opart * p.kb_part; }
+            const CUtensorMap* const ta = (SPLIT && opart == 2) ? &tmA2 : &tmA;   // (hi,hi), (hi,lo), (lo,hi)
+            const CUtensorMap* const tb = (SPLIT && opart == 1) ? &tmB2 : &tmB;
+            const int k0 = kk * BK;
+            mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+            if constexpr (!A_MN) {
+              tma_load_2d(a_dst, ta, full_bar(stage), k0, m0);
+            } else {
 #pragma unroll
-            for (int a = 0; a < BM / 64; ++a)
-              tma_load_2d(a_dst + a * (BK * 128), ta, full_bar(stage), m0 + a * 64, k0);
-          }
-          if constexpr (!B_MN) {
-            tma_load_2d(b_dst, tb, full_bar(stage), k0, n0);
-          } else {
+              for (int a = 0; a < BM / 64; ++a)
+                tma_load_2d(a_dst + a * (BK * 128), ta, full_bar(stage), m0 + a * 64, k0);
+            }
+            if constexpr (!B_MN) {
+              tma_load_2d(b_dst, tb, full_bar(stage), k0, n0);
+            } else {
 #pragma unroll
-            for (int b = 0; b < BN / 64; ++b)
-              tma_load_2d(b_dst + b * (BK * 128), tb, full_bar(stage), n0 + b * 64, k0);
+              for (int b = 0; b < BN / 64; ++b)
+                tma_load_2d(b_dst + b * (BK * 128), tb, full_bar(stage), n0 + b * 64, k0);
+            }
           }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
     }
   } else {
     // ====================== consumers: wgmma, then the epilogue ======================
-    const int wg = warp >> 2;        // warpgroup: rows [64 wg, 64 wg + 64) in the mainloop; column parity in the epilogue
-    const int quarter = warp & 3;    // epilogue: rows [32 quarter, 32 quarter + 32) of the tile
-    const int part = A_MN ? 0 : wg;  // epilogue: which interleaved set of 32-column blocks (K-major kernels)
-    const uint32_t stage_s = epi_base + uint32_t(warp) * kEpiStageBytes;  // staging tile (NT kernels)
-    const uint32_t vec_s = epi_base + kConsumerWarps * kEpiStageBytes + uint32_t(warp) * kEpiVecBytes;
+    setmaxnreg_inc<kConsumerRegs>();
+    const int cw = warp - kProducerThreads / 32;   // consumer warp 0..7
+    const int wg = cw >> 2;                        // warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int er = lane & 15;                      // epilogue: this lane's row of the warp's 16
+    const int par = lane >> 4;                     // epilogue: parity of this lane's 32-column block in a 64-column step
+    const uint32_t scratch_s = epi_base + uint32_t(cw) * kEpiScratchBytes;
+    const uint32_t vec_s = epi_base + kConsumerWarps * kEpiScratchBytes + uint32_t(cw) * kEpiVecBytes;   // K-major kernels
     const int act = ACT_T >= 0 ? ACT_T : p.act;
     const int aux_mode = AUX_T >= 0 ? AUX_T : p.aux_mode;
     const bool has_bias = BIAS_T >= 0 ? (BIAS_T != 0) : (p.bias != nullptr);
@@ -242,11 +243,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const bool mask_all = DOT_T >= 0 ? (DOT_T == 3) : (p.dot_mask == 1);
     const bool mask_rows = DOT_T >= 0 ? (DOT_T == 4) : (p.dot_mask == 2);
     const bool has_sq = DOT_T >= 0 ? (DOT_T == 2) : (p.dot_sq != 0);
-    const bool tma_st = !A_MN && p.tma_store != 0;
-    bool st_pending = false;   // a bulk store may still be reading this warp's staging tile
+    // The bulk store serves the plain-activation epilogues only (launch_plan), so it is compiled out of the aux / row-dot
+    // instances, and out of the universal 208-wide one, which those plain epilogues never reach.  Where the store path is
+    // compiled in, ptxas keeps the consumers at the launch register count (168) despite setmaxnreg: those instances spill
+    // 300-370 bytes with it and none without it.
+    constexpr bool kTmaStore = !A_MN && !SPLIT && AUX_T <= 0 && DOT_T <= 0 && !(BN == 208 && ACT_T < 0);
+    const bool tma_st = kTmaStore && p.tma_store != 0;
+    bool st_pending = false;   // a bulk store may still be reading this warp's scratch tile
     auto stage_acquire = [&]() {
       if (st_pending) {
-        if (lane == 0) bulk_wait_read();
+        if (er == 0) bulk_wait_read();   // lanes 0 and 16 issue the stores
         __syncwarp();
         st_pending = false;
       }
@@ -257,7 +263,37 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t B_LBO = B_MN ? BK * 128 : 16, B_KADV = B_MN ? kMmaK * 128 : kMmaK * 2;
     constexpr uint32_t A_WG_OFF = A_MN ? BK * 128 : 64 * 128;   // this warpgroup's 64 rows of the A tile
     constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 30);      // SBO, 128B swizzle
+    constexpr int kSteps = (BN + kEpiStep - 1) / kEpiStep;
     float acc[BN / 2];
+    // step s's fragments (columns [64 s, 64 s + 64), rows (lane >> 2) + {0, 8}) -> the scratch tile.  The acc index must
+    // be a compile-time constant, so every step has its own unrolled copy of the stores and s selects one of them.
+    auto frag_to_scratch = [&](int s) {
+#pragma unroll
+      for (int t = 0; t < kSteps; ++t) {
+        if (t == s) {
+#pragma unroll
+          for (int jj = 0; jj < kEpiStep / 8; ++jj) {
+            const int j = t * (kEpiStep / 8) + jj;
+            if (j < BN / 8) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int r = (lane >> 2) + 8 * h, c = 8 * jj + 2 * (lane & 3);
+                const uint32_t a = scratch_s + uint32_t(r) * (kEpiStep * 4) + ((uint32_t(c >> 2) ^ frag_swz(r)) << 4) + uint32_t(c & 3) * 4;
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1]) : "memory");
+              }
+            }
+          }
+        }
+      }
+    };
+    // 16 fp32 columns [c, c + 16) of this lane's row of the scratch tile
+    auto scratch_ld16 = [&](int c, uint32_t (&r)[16]) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint4 v = lds128(scratch_s + uint32_t(er) * (kEpiStep * 4) + ((uint32_t((c >> 2) + i) ^ frag_swz(er)) << 4));
+        r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
+      }
+    };
     int stage = 0;
     uint32_t phase = 0;
     int acc_iter = 0;
@@ -309,64 +345,41 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (lane == 0) mbar_arrive(empty_bar(prev));
       }
       const long long tm1 = phase_clock();
-      // ---------------- accumulator registers -> shared tile (after every warp has read the previous one)
-      named_bar_sync(1, kConsumerWarps * 32);
-      {
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int c0 = 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 8 * h, c = 8 * j + c0;
-            const uint32_t a = acc_s + uint32_t(r) * (BN * 4) + ((uint32_t(c >> 2) ^ uint32_t(r & SWZ)) << 4) + uint32_t(c & 3) * 4;
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1]) : "memory");
-          }
-        }
-      }
-      // the next tile's first wgmma overwrites the accumulator (scale_d = 0); redefining it here ends the registers'
-      // liveness, so they are free for the epilogue instead of being carried (or spilled) across it
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      named_bar_sync(1, kConsumerWarps * 32);
-      const long long te0 = tm1, te1 = phase_clock();   // accumulator hand-off: barrier + shared-tile store
-      if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && acc_iter < 16 && threadIdx.x == 0) {
+      if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && acc_iter < 16 && threadIdx.x == kProducerThreads) {
         long long* d = p.dbg + acc_iter * 4;   // [tile][0, mainloop, 0, start stamp]
         d[0] = 0; d[1] = tm1 - tm0; d[2] = 0; d[3] = tm0;
       }
-      const int wrow0 = m0 + quarter * 32;   // first row of this warp
-      const int row = wrow0 + lane;
-      const int arow = quarter * 32 + lane;  // this lane's row of the accumulator tile
+      long long t_frag = 0, t_ld = 0;   // phase timing: fragment stores to the scratch tile, row reads from it
+      const int wrow0 = m0 + wg * 64 + (cw & 3) * 16;   // first row of this warp
+      const int row = wrow0 + er;
       const bool row_ok = row < p.M;
       const bool mask_out = mask_all || (kRowMask && mask_rows && row >= p.mask_row0);
       constexpr bool kUniversal = ACT_T < 0;
       if (!A_MN && !(kUniversal && p.epi == EPI_F32)) {
         // ================= bf16 epilogue (K-major kernels) =================
-        // coalesced lane mapping for aux reads / output writes: 4 lanes x 16 B = one 64-byte
-        // row segment, 8 rows per pass, 4 passes
-        const int lr = lane >> 2, lc = lane & 3;
+        // coalesced lane mapping for aux reads / output writes: 8 lanes x 16 B = one 128-byte
+        // row segment (a whole step), 4 rows per pass, 4 passes
+        const int lr = lane >> 3, lc = lane & 7;
         constexpr int kBlocks = (BN + kEpiCols - 1) / kEpiCols;
-        // aux tile (32 rows x 32 columns of the warp's next block):
+        // aux tile (16 rows x 64 columns of the warp's next step):
         //  * kernels without bias / row-dot (dX, dHg, penalty T): cp.async straight into the
-        //    warp's (otherwise unused) bias staging area, 64-byte rows with the 16-byte chunks
-        //    XOR-swizzled by (row >> 1) & 3 so that the row-per-lane reads are conflict-free.
-        //    No registers held across the block, no STS;
-        //  * otherwise: coalesced LDG into registers, transposed through the staging tile.
-        //    With a bias (VAE decoder output, BEGAN decoder; 16 epilogue warps) the tile sits behind the warp's four bias
-        //    blocks in an enlarged staging area: the register path (16 registers held across the block) spilled there.
+        //    warp's (otherwise unused) bias staging area, 128-byte rows with the 16-byte chunks
+        //    XOR-swizzled by row & 7 so that the row-per-lane reads are conflict-free.
+        //    No registers held across the step, no STS;
+        //  * otherwise: coalesced LDG into registers, transposed through the scratch tile.
         constexpr bool kAuxAsync = (AUX_T > 0) && (DOT_T == 0) && (BIAS_T == 0);
-        const uint32_t auxt_s = vec_s;   // 32 rows x 64 B, chunks XOR-swizzled
+        const uint32_t auxt_s = vec_s;   // 16 rows x 128 B, chunks XOR-swizzled
         uint4 pre[kAuxAsync ? 1 : 4];
-        auto aux_fetch = [&](int c_first) {
-          const int c = c_first + lc * 8;
+        auto aux_fetch = [&](int cs) {   // columns [cs, cs + 64) of the tile
+          const int c = n0 + cs + lc * 8;
 #pragma unroll
           for (int it = 0; it < 4; ++it) {
-            const int rl = it * 8 + lr;
+            const int rl = it * 4 + lr;
             const int r = wrow0 + rl;
-            const bool ok = r < p.M && c < p.out_cols;
+            const bool ok = r < p.M && c < p.out_cols && cs + lc * 8 < BN;
             if constexpr (kAuxAsync) {
               const __nv_bfloat16* src = ok ? p.aux + size_t(r) * p.ld_aux + c : p.aux;
-              cp_async16_zfill(auxt_s + rl * 64 + ((lc ^ ((rl >> 1) & 3)) << 4), src, ok ? 16u : 0u);
+              cp_async16_zfill(auxt_s + rl * 128 + ((lc ^ (rl & 7)) << 4), src, ok ? 16u : 0u);
             } else {
               pre[it] = make_uint4(0, 0, 0, 0);
               if (ok) pre[it] = __ldg(reinterpret_cast<const uint4*>(p.aux + size_t(r) * p.ld_aux + c));
@@ -374,15 +387,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
           if constexpr (kAuxAsync) cp_async_commit();
         };
-        // bias / row-dot weights of this warp's column blocks -> smem and the first aux tile ->
-        // registers before the accumulator tile is read: no global-load latency after it
+        // bias / row-dot weights of the tile's column blocks -> smem and the first aux tile ->
+        // registers before the fragments are read: no global-load latency after them
         if (has_bias || has_dot) {
 #pragma unroll
           for (int pass = 0; pass < kEpiVecBlocks / 4; ++pass) {
             const int blk = pass * 4 + (lane >> 3), c4 = (lane & 7) * 4;   // 4 blocks x 8 float4 per pass
-            const int c = n0 + (part + blk * kParts) * kEpiCols + c4;
+            const int c = n0 + blk * kEpiCols + c4;
             uint4 bz = make_uint4(0, 0, 0, 0), wz = bz;
-            if (part + blk * kParts < kBlocks && c < p.N) {
+            if (blk < kBlocks && c < p.N) {
               if (has_bias) {
                 bz = __ldg(reinterpret_cast<const uint4*>(p.bias + c));
                 if (act == ACT_SIGMOID) {   // sigmoid(x + b) = 0.5 tanh(0.5 x + 0.5 b) + 0.5: stage 0.5 b, one FFMA later
@@ -392,80 +405,82 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               }
               if (has_dot) wz = __ldg(reinterpret_cast<const uint4*>(p.dot_w + c));
             }
-            if (blk < kEpiVecBlocks / kParts) {   // a warp owns at most 4 blocks
-              if (has_bias) sts128(vec_s + (blk * kEpiCols + c4) * 4, bz);
-              if (has_dot) sts128(vec_s + kEpiVecBytes / 2 + (blk * kEpiCols + c4) * 4, wz);
-            }
+            if (has_bias) sts128(vec_s + (blk * kEpiCols + c4) * 4, bz);
+            if (has_dot) sts128(vec_s + kEpiVecBytes / 2 + (blk * kEpiCols + c4) * 4, wz);
           }
           __syncwarp();
         }
         if (aux_mode != AUX_NONE) {
-          aux_fetch(n0 + part * kEpiCols);
-          // pull the aux tile of the NEXT tile this warp will process (same accumulator stage)
+          aux_fetch(0);
+          // pull the aux tile of the NEXT tile this warp will process (same rows of the tile)
           // into L2 now: its loads are otherwise HBM-latency-bound
           const int nitem = item + gridDim.x;
           if (nitem < total) {
             const int nrem = nitem - (nitem / tiles) * tiles;
-            const int nm0 = (nrem / p.n_tiles) * BM + quarter * 32;
+            const int nm0 = (nrem / p.n_tiles) * BM + wg * 64 + (cw & 3) * 16;
             const int nn0 = (nrem % p.n_tiles) * BN;
-            // 32 rows x 416 B: each of the kParts warps of this quarter takes every kParts-th row
-            for (int t = lane; t < (32 / kParts) * 4; t += 32) {
-              const int r = nm0 + (t >> 2) * kParts + part, c = nn0 + (t & 3) * 64;
+            // 16 rows x 416 B: four 128-byte lines per row
+            for (int t = lane; t < kEpiRows * 4; t += 32) {
+              const int r = nm0 + (t >> 2), c = nn0 + (t & 3) * 64;
               if (r < p.M && c < p.out_cols)
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(p.aux + size_t(r) * p.ld_aux + c));
             }
           }
         }
-        long long t_ld = 0;
         float dot = 0.f;
         float l1_scale = 0.f;
         if (aux_mode == AUX_L1) l1_scale = __ldg(p.row_scale + (row < p.row_split ? 0 : 1));
         if (aux_mode == AUX_SIGMOID_GRAD || aux_mode == AUX_RELU_MASK || aux_mode == AUX_NONZERO_MASK) l1_scale = (p.row_vec != nullptr && row_ok) ? __ldg(p.row_vec + row) : 1.f;
 #pragma unroll 1
-        for (int bi = 0; part + bi * kParts < kBlocks; ++bi) {
-          const int cb = (part + bi * kParts) * kEpiCols;
+        for (int s = 0; s < kSteps; ++s) {
+          const int cs = s * kEpiStep;
+          if (n0 + cs >= p.out_cols) break;
+          const int bi = 2 * s + par;            // this lane's 32-column block of the tile
+          const int cb = bi * kEpiCols;
           const int col0 = n0 + cb;
-          if (col0 >= p.out_cols) break;
-          const int nch = (BN - cb) >= kEpiCols ? 2 : (BN - cb) / 16;
-          const int cb_next = cb + kParts * kEpiCols;
-          const bool last_block = (cb_next >= BN) || (n0 + cb_next >= p.out_cols);
+          const int nch = (cb >= BN || col0 >= p.out_cols) ? 0 : (BN - cb) >= kEpiCols ? 2 : (BN - cb) / 16;
+          const bool last_step = (cs + kEpiStep >= BN) || (n0 + cs + kEpiStep >= p.out_cols);
+          // full 64-column step -> one bulk tensor store per 32-column block of the (64-byte rows, XOR-swizzled) staging
+          const bool step_tma = tma_st && BN - cs >= kEpiStep && wrow0 < p.M;
+          // accumulator fragments -> scratch -> this lane's row: both chunks in flight, one wait
+          stage_acquire();
+          const long long tf0 = phase_clock();
+          frag_to_scratch(s);
+          __syncwarp();
+          const long long tl0 = phase_clock();
+          uint32_t raw[2][16];
+#pragma unroll
+          for (int q = 0; q < 2; ++q)
+            if (q < nch && col0 + q * 16 < p.N) scratch_ld16(par * kEpiCols + q * 16, raw[q]);
+          __syncwarp();
+          t_frag += tl0 - tf0;
+          t_ld += phase_clock() - tl0;
           uint4 ax[4];
           if (aux_mode != AUX_NONE) {   // prefetched aux (coalesced mapping) -> smem -> own row
             if constexpr (kAuxAsync) {
               cp_async_wait_all();
               __syncwarp();
 #pragma unroll
-              for (int q = 0; q < 4; ++q) ax[q] = lds128(auxt_s + lane * 64 + ((q ^ ((lane >> 1) & 3)) << 4));
+              for (int q = 0; q < 4; ++q) ax[q] = lds128(auxt_s + er * 128 + (((4 * par + q) ^ (er & 7)) << 4));
             } else {
-              stage_acquire();
 #pragma unroll
-              for (int it = 0; it < 4; ++it) sts128(stage_s + (it * 8 + lr) * kEpiPitch + lc * 16, pre[it]);
+              for (int it = 0; it < 4; ++it) sts128(scratch_s + (it * 4 + lr) * kEpiPitch + lc * 16, pre[it]);
               __syncwarp();
 #pragma unroll
-              for (int q = 0; q < 4; ++q) ax[q] = lds128(stage_s + lane * kEpiPitch + q * 16);
+              for (int q = 0; q < 4; ++q) ax[q] = lds128(scratch_s + er * kEpiPitch + par * 64 + q * 16);
             }
             __syncwarp();
-            if (!last_block) aux_fetch(n0 + cb_next);   // overlaps with this block's math + stores
+            if (!last_step) aux_fetch(cs + kEpiStep);   // overlaps with this step's math + stores
           }
           uint4 axl[4] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
           if constexpr (SPLIT) {   // residual plane of the aux values of this lane's row (plain loads: the split kernels are not tuned)
             if (p.lo_off != 0 && aux_mode != AUX_NONE && aux_mode != AUX_RELU_MASK && aux_mode != AUX_NONZERO_MASK && row_ok) {
 #pragma unroll
               for (int q = 0; q < 4; ++q)
-                if (col0 + q * 8 < p.out_cols)
+                if (q < 2 * nch && col0 + q * 8 < p.out_cols)
                   axl[q] = __ldg(reinterpret_cast<const uint4*>(p.aux + p.lo_off + size_t(row) * p.ld_aux + col0 + q * 8));
             }
           }
-          // accumulator columns -> registers: both chunks in flight, one wait
-          uint32_t raw[2][16];
-          const long long tl0 = phase_clock();
-#pragma unroll
-          for (int q = 0; q < 2; ++q)
-            if (q < nch && col0 + q * 16 < p.N) acc_ld16<BN, SWZ>(acc_s, arow, cb + q * 16, raw[q]);
-          t_ld += phase_clock() - tl0;
-          // full 32-column block -> one bulk tensor store of the (64-byte rows, XOR-swizzled) tile
-          const bool blk_tma = tma_st && nch == 2 && wrow0 < p.M;
-          stage_acquire();
 #pragma unroll
           for (int q = 0; q < 2; ++q) {
             if (q < nch) {
@@ -578,88 +593,95 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                        pack_bf16x2_residual(v[12], v[13], hi.z), pack_bf16x2_residual(v[14], v[15], hi.w));
                   }
                 }
-                if (blk_tma) {
-                  const uint32_t sw = (lane >> 1) & 3, rowb = stage_s + lane * 64;
+                if (step_tma) {
+                  const uint32_t sw = (er >> 1) & 3, rowb = scratch_s + par * (kEpiRows * kEpiCols * 2) + er * 64;
                   sts128(rowb + (((2 * q) ^ sw) << 4), lo);
                   sts128(rowb + (((2 * q + 1) ^ sw) << 4), hi);
                 } else {
-                  sts128(stage_s + lane * kEpiPitch + q * 32, lo);
-                  sts128(stage_s + lane * kEpiPitch + q * 32 + 16, hi);
+                  sts128(scratch_s + er * kEpiPitch + par * 64 + q * 32, lo);
+                  sts128(scratch_s + er * kEpiPitch + par * 64 + q * 32 + 16, hi);
                 }
               }
             }
           }
-          if (blk_tma) {
+          if (step_tma) {
             fence_proxy_async_smem();
             __syncwarp();
-            if (lane == 0) {
-              tma_store_2d(&tmC, stage_s, col0, wrow0);
+            if (er == 0 && nch == 2) {
+              tma_store_2d(&tmC, scratch_s + par * (kEpiRows * kEpiCols * 2), col0, wrow0);
               bulk_commit();
             }
             st_pending = true;
-            continue;
-          }
-          __syncwarp();
-          // coalesced store: 4 lanes cover 64 contiguous bytes of one row, 8 rows per pass
-          if (p.out != nullptr && lc < nch * 2 && col0 + lc * 8 < p.out_cols) {
-            __nv_bfloat16* o = p.out + size_t(wrow0 + lr) * p.ldo + col0 + lc * 8;
-            const uint32_t sa = stage_s + lr * kEpiPitch + lc * 16;
+          } else {
+            __syncwarp();
+            // coalesced store: 8 lanes cover the step's 128 contiguous bytes of one row, 4 rows per pass
+            const int oc = n0 + cs + lc * 8;
+            if (p.out != nullptr && cs + lc * 8 < BN && oc < p.out_cols) {
+              __nv_bfloat16* o = p.out + size_t(wrow0 + lr) * p.ldo + oc;
+              const uint32_t sa = scratch_s + lr * kEpiPitch + lc * 16;
 #pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int rr = wrow0 + it * 8 + lr;
-              if (rr < p.M) {
-                __nv_bfloat16* dst = o + size_t(it * 8) * p.ldo;
-                if constexpr (kRowMask) {
-                  if (mask_rows && rr >= p.mask_row0) dst = p.out_alt + size_t(rr - p.mask_row0) * p.ldo + col0 + lc * 8;
+              for (int it = 0; it < 4; ++it) {
+                const int rr = wrow0 + it * 4 + lr;
+                if (rr < p.M) {
+                  __nv_bfloat16* dst = o + size_t(it * 4) * p.ldo;
+                  if constexpr (kRowMask) {
+                    if (mask_rows && rr >= p.mask_row0) dst = p.out_alt + size_t(rr - p.mask_row0) * p.ldo + oc;
+                  }
+                  *reinterpret_cast<uint4*>(dst) = lds128(sa + it * 4 * kEpiPitch);
                 }
-                *reinterpret_cast<uint4*>(dst) = lds128(sa + it * 8 * kEpiPitch);
+              }
+            }
+            __syncwarp();
+          }
+        }
+        if ((has_dot || has_sq || aux_mode == AUX_VAE_OUT || aux_mode == AUX_L1) && p.dot_out != nullptr && row_ok)
+          p.dot_out[size_t(n_tile * 2 + par) * p.dot_ld + row] = dot;
+        if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && lane == 0 && cw == 0 && acc_iter < 16) {
+          long long* d = p.dbg + 64 + acc_iter * 4;   // [tile][fragment stores, rest of the epilogue, of which scratch reads, start stamp]
+          d[0] = t_frag; d[1] = phase_clock() - tm1 - t_frag; d[2] = t_ld; d[3] = tm1;
+        }
+      } else {
+        // ====== fp32 epilogue: split-K partials (MN-major kernels) or biased fp32 output ======
+        float* base = p.part + size_t(split) * p.part_stride;
+#pragma unroll 1
+        for (int s = 0; s < kSteps; ++s) {
+          if (n0 + s * kEpiStep >= p.N) break;
+          frag_to_scratch(s);
+          __syncwarp();
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            const int c = s * kEpiStep + par * kEpiCols + q * 16;   // tile column of this lane's 16-column chunk
+            const int col0 = n0 + c;
+            if (c >= BN || col0 >= p.N) continue;
+            float v[16];
+            {
+              uint32_t raw[16];
+              scratch_ld16(par * kEpiCols + q * 16, raw);
+#pragma unroll
+              for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(raw[j]);
+            }
+            if (p.bias != nullptr) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j)
+                if (col0 + j < p.N) v[j] += __ldg(p.bias + col0 + j);
+            }
+            if (row_ok) {
+              if (p.transpose) {
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                  if (col0 + j < p.N) base[size_t(col0 + j) * p.ldp + row] = v[j];
+              } else if (col0 + 16 <= p.N) {
+                float4* o = reinterpret_cast<float4*>(base + size_t(row) * p.ldp + col0);
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4) o[k4] = make_float4(v[4 * k4], v[4 * k4 + 1], v[4 * k4 + 2], v[4 * k4 + 3]);
+              } else {
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                  if (col0 + j < p.N) base[size_t(row) * p.ldp + col0 + j] = v[j];
               }
             }
           }
           __syncwarp();
-        }
-        if ((has_dot || has_sq || aux_mode == AUX_VAE_OUT || aux_mode == AUX_L1) && p.dot_out != nullptr && row_ok)
-          p.dot_out[size_t(n_tile * 2 + (kParts == 2 ? part : 0)) * p.dot_ld + row] = dot;
-        if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && lane == 0 && quarter == 0 && part == 0 && acc_iter < 16) {
-          long long* d = p.dbg + 64 + acc_iter * 4;   // [tile][accumulator hand-off, epilogue work, of which acc-tile reads, start stamp]
-          d[0] = te1 - te0; d[1] = phase_clock() - te1; d[2] = t_ld; d[3] = te0;
-        }
-      } else {
-        // ====== fp32 epilogue: split-K partials (MN-major kernels) or biased fp32 output ======
-        const int c_first = wg;
-        const int c_step = kConsumerWarps / 4;
-        float* base = p.part + size_t(split) * p.part_stride;
-#pragma unroll 1
-        for (int c = c_first; c < BN / 16; c += c_step) {
-          const int col0 = n0 + c * 16;
-          if (col0 >= p.N) break;
-          float v[16];
-          {
-            uint32_t raw[16];
-            acc_ld16<BN, SWZ>(acc_s, arow, c * 16, raw);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(raw[j]);
-          }
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (col0 + j < p.N) v[j] += __ldg(p.bias + col0 + j);
-          }
-          if (row_ok) {
-            if (p.transpose) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (col0 + j < p.N) base[size_t(col0 + j) * p.ldp + row] = v[j];
-            } else if (col0 + 16 <= p.N) {
-              float4* o = reinterpret_cast<float4*>(base + size_t(row) * p.ldp + col0);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) o[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (col0 + j < p.N) base[size_t(row) * p.ldp + col0 + j] = v[j];
-            }
-          }
         }
       }
     }

@@ -132,10 +132,11 @@ __device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t da, ui
       : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
-// named barrier over the first `threads` threads of the block (warp-aligned)
-__device__ __forceinline__ void named_bar_sync(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
+// per-warpgroup register budget (all four warps of a warpgroup execute it): the producer hands registers to the consumers
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // 16-byte shared-memory accesses by 32-bit shared address
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {

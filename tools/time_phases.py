@@ -1,7 +1,9 @@
-"""Per-tile phase timing of the GEMM kernel (CTA 0): MMA issuer and one epilogue warp.
+"""Per-tile phase timing of the GEMM kernel (CTA 0): first consumer warp's mainloop and epilogue.
 
-The clock reads are compiled out of the shipped library (they cost registers in the 96-register
-epilogue): build an instrumented copy and point GM_B200_LIB at it, e.g.
+The epilogue record splits the tile's epilogue into the fragment stores to the warp's scratch
+tile (summed over its 64-column steps), the rest of the epilogue, and of that the row reads
+from the scratch tile.  The clock reads are compiled out of the shipped library (they cost
+registers next to the accumulators): build an instrumented copy and point GM_B200_LIB at it, e.g.
   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Xcompiler -fPIC -shared -I include \
        -DGM_PHASE_TIMING -o build_variants/lib_timing.so generative-models_b200/gm_b200/csrc/engine.cu
   GM_B200_LIB=$PWD/build_variants/lib_timing.so python tools/time_phases.py"""
@@ -39,7 +41,7 @@ def run(name, fn):
     t0 = int(d[0, 0, 3])
     for i in range(10):
         print("       %2d   %8d %8d %8d   @%d" % (i, d[0, i, 0], d[0, i, 1], d[0, i, 2], int(d[0, i, 3]) - t0))
-    print(" EPI  : tile | acc hand-off | work | of which acc-tile reads | start")
+    print(" EPI  : tile | fragment stores | rest of epilogue | of which scratch reads | start")
     for i in range(0, 10):
         print("       %2d   %8d %8d %8d   @%d" % (i, d[1, i, 0], d[1, i, 1], d[1, i, 2], int(d[1, i, 3]) - t0))
 
