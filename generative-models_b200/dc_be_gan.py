@@ -88,7 +88,7 @@ class DCBEGANTrainer(DCGANTrainer):
     def _pre_train(self, eng):
         eng.began_init(self._control[3], getattr(self.train_iter, "batch_size", None) or 1)   # fresh schedulers per train()
 
-    def _after_g_step(self, eng):
+    def _after_g_step(self, eng, n, inv, seed):
         eng.began_control(*self._control[:3])                                                # src/be_gan.py:186-195
 
     def _epoch_line(self, eng, epoch, num_epochs, G_losses, D_losses):

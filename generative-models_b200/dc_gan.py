@@ -88,13 +88,18 @@ class DCGAN(nn.Module):
                                   channels=channels))
         self.G = Generator(image_size, hidden_dim, z_dim, channels)
         self.D = self._D(image_size, hidden_dim, output_dim, channels, **d_options)
-        for m in self.modules():                                # DCGAN initialisation (Radford et al. 2015)
-            if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
-                nn.init.normal_(m.weight, 0.0, 0.02)
-            elif isinstance(m, nn.BatchNorm2d):
-                nn.init.normal_(m.weight, 1.0, 0.02)
-                nn.init.zeros_(m.bias)
+        dcgan_init(self)
         self.shape = 64
+
+
+def dcgan_init(module):
+    """DCGAN initialisation (Radford et al. 2015) of every conv / BatchNorm layer in module"""
+    for m in module.modules():
+        if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
+            nn.init.normal_(m.weight, 0.0, 0.02)
+        elif isinstance(m, nn.BatchNorm2d):
+            nn.init.normal_(m.weight, 1.0, 0.02)
+            nn.init.zeros_(m.bias)
 
 
 class DCGANTrainer:
@@ -116,9 +121,13 @@ class DCGANTrainer:
         object.__setattr__(model.D, "_owner", self)
 
     # ------------------------------------------------------------------ engine <-> module parameters
+    def _nets(self):
+        """(state_dict prefix, module) of every network the engine trains"""
+        return [("G", self.model.G), ("D", self.model.D)]
+
     def _sd(self):
         out = {}
-        for tag, mod in (("G", self.model.G), ("D", self.model.D)):
+        for tag, mod in self._nets():
             for k, v in mod.named_parameters():
                 out["%s.%s" % (tag, k)] = v.detach()
         return out
@@ -127,7 +136,8 @@ class DCGANTrainer:
         m = self.model
         if self._engine is None:
             self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=self.variant, d_out_act=m.D.out_act,
-                                       embed_dim=getattr(m.D, "embed_dim", None))
+                                       embed_dim=getattr(m.D, "embed_dim", None), disc_dim=getattr(m, "disc_dim", None),
+                                       cont_dim=getattr(m, "cont_dim", None))
             self._dirty = True
         if self._dirty:
             self._engine.load_torch_weights(self._sd())
@@ -138,13 +148,15 @@ class DCGANTrainer:
         """engine -> module parameters (after training; before state_dict / save_model)"""
         if self._engine is None:
             return
-        tw = self._engine.torch_weights()
+        eng = self._engine
+        tw = eng.torch_weights()
+        runs = {"G": eng.run_G, "D": eng.run_D, "Q": eng.run_Q}
         with torch.no_grad():
-            for tag, mod in (("G", self.model.G), ("D", self.model.D)):
+            for tag, mod in self._nets():
                 for k, v in mod.named_parameters():
                     v.copy_(tw["%s.%s" % (tag, k)].to(v.device))
                 for i, bn in ((i, getattr(mod, "bn%d" % i, None)) for i in range(1, 5)):       # a critic may have none
-                    run = (self._engine.run_G.get(i - 1) if tag == "G" else self._engine.run_D.get(i - 1))
+                    run = runs[tag].get(i - 1)
                     if bn is not None and run is not None:
                         bn.running_mean.copy_(run[0].cpu())
                         bn.running_var.copy_(run[1].cpu())
@@ -182,7 +194,7 @@ class DCGANTrainer:
                 ring[D_steps, i] = eng.g_grad(n, inv_global_batch=inv, seed=seed, step=self._step)
                 par.sum_gradients(eng.G.grads)
                 eng.apply(0, hpG)
-                self._after_g_step(eng)
+                self._after_g_step(eng, n, inv, seed)
                 self._step += 1
             G_losses, D_losses = ring[D_steps].tolist(), ring[:D_steps].mean(dim=0).tolist()
             self.Glosses.extend(G_losses)
@@ -194,18 +206,23 @@ class DCGANTrainer:
     def _epoch_line(self, eng, epoch, num_epochs, G_losses, D_losses):
         return "Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses))
 
-    def _after_g_step(self, eng):
-        """per-step device work of a subclass after each G update (e.g. BEGAN's K control); enqueued, never synchronising"""
+    def _after_g_step(self, eng, n, inv, seed):
+        """per-step device work of a subclass after each G update (e.g. BEGAN's K control, InfoGAN's MI step) for the step's
+        local batch n, gradient scale inv and Philox seed; enqueued, never synchronising"""
 
     def _pre_train(self, eng):
         """per-train() state of a subclass (e.g. Fisher GAN's multiplier), after the optimizers are reset"""
 
     def _loss(self, net, loss_val):
-        eng = self._engine
-        tag, mod = ("G", self.model.G) if net == 0 else ("D", self.model.D)
-        tg = eng.torch_grads()
-        params = [p for _, p in mod.named_parameters()]
-        flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for k, p in mod.named_parameters()])
+        return self._fused_loss([("G", self.model.G)] if net == 0 else [("D", self.model.D)], loss_val)
+
+    def _fused_loss(self, mods, loss_val):
+        """loss_val as a 0-dim loss whose backward() puts the engine's current gradients of the (tag, module) pairs `mods`
+        on those modules' parameters"""
+        tg = self._engine.torch_grads()
+        named = [(tag, k, p) for tag, mod in mods for k, p in mod.named_parameters()]
+        params = [p for _, _, p in named]
+        flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for tag, k, p in named])
         self._dirty = True                                            # the caller's optimizer will change the module parameters
         return _FusedLoss.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat, params)
 

@@ -149,6 +149,8 @@ def lib():
     L.gm_began_loss_final.argtypes = [vp, vp, vp, i, i, vp, vp, vp]
     L.gm_began_control.argtypes = [vp, vp, f, f, f, vp]
     L.gm_began_dfake_rows.argtypes = [vp, vp, vp, vp, vp, i, i, vp]
+    L.gm_info_noise_rows.argtypes = [vp, vp, i, vp, i, i, i, i, u64, u64, vp]
+    L.gm_info_loss_rows.argtypes = [vp, vp, i, vp, i, i, i, i, i, f, vp, i, vp, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]

@@ -626,6 +626,52 @@ __global__ void __launch_bounds__(256) l1_sum_kernel(const double* __restrict__ 
   if (threadIdx.x == 0) out[0] = s;
 }
 
+// ---- InfoGAN's structured generator input (compute_noise, src/info_gan.py:306-325) drawn on the device
+// Row r of the bf16 GEMM operand out [rows, ld] is [z (zd) | one-hot (nd) | continuous code (nc) | 1 | 0 ...], and codes
+// [rows, K = zd + nd + nc] fp32 holds the same K values (the MI loss's targets).  The N(0, 1) values are rounded to bf16
+// before both stores, so the two copies agree bit for bit.  One thread per (row, 8-column group holding draws or the ones
+// column), 16-byte stores; the thread also writes its share of the row's zero padding groups (stage_noise_kernel's mapping).
+// Philox is keyed by seed; the counter's high 64 bits are stream_id, the low 64 bits a block index unique within the
+// stream: row r owns blocks [r (2 gz + 1), (r + 1)(2 gz + 1)).  Its first block draws the category, (w nd) >> 32 of one
+// 32-bit word w (uniform over [0, nd) to 2^-32, never nd), so every thread of the row computes the same index; group g
+// draws its 8 normals from blocks 2g + 1 and 2g + 2.
+__global__ void __launch_bounds__(256) info_noise_kernel(__nv_bfloat16* __restrict__ out, int ld, float* __restrict__ codes, int rows,
+                                                         int zd, int nd, int nc, unsigned long long seed, unsigned long long stream_id) {
+  griddep_sync();
+  const int K = zd + nd + nc, groups = ld / 8, gz = (K + 8) / 8;
+  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (t >= (long long)rows * gz) return;
+  const int r = int(t / gz), g = int(t % gz), c0 = g * 8;
+  const unsigned long long blk0 = (unsigned long long)r * (2 * gz + 1);
+  float v[8];
+  if (c0 < K) {
+    curandStatePhilox4_32_10_t st;
+    curand_init(seed, stream_id, 4ull * (blk0 + 1 + 2 * g), &st);
+    const float4 a = curand_normal4(&st), b = curand_normal4(&st);
+    const float nrm[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    int cat = -1;
+    if (c0 < zd + nd && c0 + 8 > zd) {
+      curand_init(seed, stream_id, 4ull * blk0, &st);
+      cat = int((unsigned long long)curand(&st) * (unsigned)nd >> 32);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = c0 + j;
+      if (c >= zd && c < zd + nd) v[j] = c - zd == cat ? 1.f : 0.f;
+      else v[j] = c < K ? __bfloat162float(__float2bfloat16_rn(nrm[j])) : (c == K ? 1.f : 0.f);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (c0 + j < K) codes[(long long)r * K + c0 + j] = v[j];
+  } else {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = c0 + j == K ? 1.f : 0.f;
+  }
+  store_bf16x8(out + ((long long)r * groups + g) * 8, v, 0);
+  uint4* row = reinterpret_cast<uint4*>(out) + (long long)r * groups;
+  for (int pg = gz + g; pg < groups; pg += gz) row[pg] = make_uint4(0, 0, 0, 0);
+}
+
 // One block per x_hat image b.  J [HW*C] = image gradient of the logit s_b (the beta chain seeded with 1), xh the image.
 // sigma = sigmoid(s_b), sigma' = sigma (1 - sigma), ||g|| = sigma' ||J|| (the gradient of D's sigmoid output),
 // k = 2 lambda inv_grad (||g|| - K); the tangent seed of the penalty's double backward is

@@ -20,7 +20,9 @@ whose double backward is closed form because the critic is piecewise linear (wgp
 their batch statistics in separate loss passes that stats_reduce can sum over data-parallel ranks.  variant="be" (BEGAN,
 src/be_gan.py:212-258) makes D an autoencoder: the D trunk above with a linear embed_dim-wide conv 5 as the encoder, the
 generator stack with a linear output as the decoder, L1 reconstruction losses (gm_l1_rows) and K and the plateau scheduler
-as device state (be_state, gm_began_control).
+as device state (be_state, gm_began_control).  variant="info" (InfoGAN, src/info_gan.py:130-325) feeds G [z | one-hot |
+continuous code] drawn on the device (gm_info_noise_rows) and adds Q, a second D trunk with a linear code head, trained with
+G by the MI step (q_grad, gm_info_loss_rows) and MI_optimizer's own Adam state for G (apply_mi).
 
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
@@ -123,15 +125,23 @@ class _Net:
 class DcganEngine:
     """One DCGAN (64x64xchannels images) on one GPU; see the module docstring."""
 
-    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None, d_out_act=None, embed_dim=None):
+    def __init__(self, hidden_dim=64, z_dim=100, channels=3, variant="ns", device=None, d_out_act=None, embed_dim=None, disc_dim=None,
+                 cont_dim=None):
         if not torch.cuda.is_available():
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra and be")
+        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be", "info") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra, be and info")
         if embed_dim is not None and (variant != "be" or embed_dim <= 0):
             raise GmError("embed_dim is the positive embedding width of BEGAN's autoencoder D (variant='be')")
+        if variant == "info":
+            disc_dim, cont_dim = 10 if disc_dim is None else int(disc_dim), 10 if cont_dim is None else int(cont_dim)
+            if disc_dim < 1 or cont_dim < 1:
+                # the reference's cross entropy / MSE over zero codes is NaN (src/info_gan.py:295-299)
+                raise GmError("InfoGAN needs disc_dim >= 1 and cont_dim >= 1")
+        elif disc_dim is not None or cont_dim is not None:
+            raise GmError("disc_dim and cont_dim are the code widths of InfoGAN (variant='info')")
         if variant == "be":
             # BEGAN's D is an autoencoder whose reconstruction is linear (src/be_gan.py:73-76)
             if d_out_act not in (None, "none"):
@@ -156,7 +166,10 @@ class DcganEngine:
         # stats_reduce(buf): SUM a float64 statistic buffer over the data-parallel ranks in place (RaNS / Fisher loss
         # moments, DRAGAN's image std, BEGAN's L1 sums); None on one process.  stat_batch (d_grad) is then the global batch.
         self.stats_reduce = None
-        self.zp = (z_dim + 1 + 7) // 8 * 8                       # noise rows: [z | 1 | pad], 16-byte rows
+        # InfoGAN: G's input is [z | one-hot (nd) | continuous code (nc)] (src/info_gan.py:51,325); zin = G's input width
+        self.nd, self.nc = (disc_dim, cont_dim) if variant == "info" else (0, 0)
+        self.zin = z_dim + self.nd + self.nc
+        self.zp = (self.zin + 1 + 7) // 8 * 8                    # noise rows: [z | 1 | pad], 16-byte rows
         hd = hidden_dim
         self.gc = [8 * hd, 4 * hd, 2 * hd, hd, channels]        # generator channels after each layer
         self.dc = [hd, 2 * hd, 4 * hd, 8 * hd]                  # discriminator channels after conv 1..4
@@ -187,11 +200,22 @@ class DcganEngine:
         else:
             self._trim = {"D.l5.weight": 1}
             d_shapes = d_stack("", 16)                           # 1 real output channel (row 0), padded to the MMA's N = 16
-        self.G, self.D = _Net(g_stack("", z_dim), self.device), _Net(d_shapes, self.device)
+        self.G, self.D = _Net(g_stack("", self.zin), self.device), _Net(d_shapes, self.device)
         self.run_G = {i: torch.zeros(2, self.gc[i], device=self.device) for i in range(4)}
         self.run_D = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4) if self.d_bn}
         self.run_dec = {i: torch.zeros(2, self.gc[i], device=self.device) for i in range(4)} if variant == "be" else {}
-        for r in list(self.run_G.values()) + list(self.run_D.values()) + list(self.run_dec.values()):
+        # InfoGAN's Q (src/info_gan.py:78-94): its own D trunk (BatchNorm on conv 2-4) and a linear conv 5 with nd + nc
+        # outputs, zero-padded to qp rows (the N of the fp32 row-major head GEMM); MI_optimizer's own Adam moments for G
+        self.Q, self.run_Q, self.qp = None, {}, 0
+        if variant == "info":
+            self.qp = (self.nd + self.nc + 15) // 16 * 16
+            self._trim["Q.l5.weight"] = self.nd + self.nc
+            self.Q = _Net(d_stack("", self.qp), self.device)
+            self.run_Q = {i: torch.zeros(2, self.dc[i], device=self.device) for i in range(1, 4)}
+            self.g_mi_avg, self.g_mi_avg_sq = torch.zeros_like(self.G.params), torch.zeros_like(self.G.params)
+            self.mi_loss = torch.zeros(1, device=self.device)
+            self.codes_ = {}
+        for r in list(self.run_G.values()) + list(self.run_D.values()) + list(self.run_dec.values()) + list(self.run_Q.values()):
             r[1].fill_(1.0)
         self.loss_buf = torch.zeros(4, device=self.device)      # [D loss, G loss, loss-kernel scratch (sum ds, ..)]
         # BEGAN's device state, the layout of gm_gan_began_state: [K, inv_b, -K inv_b, DX, DG, plateau best, plateau bad
@@ -206,7 +230,7 @@ class DcganEngine:
     def init_weights(self, seed=1234):
         """DCGAN initialisation (N(0, 0.02) conv weights, N(1, 0.02) BN scale, zero BN shift)."""
         g = torch.Generator().manual_seed(seed)
-        for net in (self.G, self.D):
+        for net in self.nets():
             for n in net.names:
                 v = net.view(n)
                 if n.endswith("bias"):
@@ -216,26 +240,33 @@ class DcganEngine:
                 else:
                     v.copy_(0.02 * torch.randn(v.shape, generator=g))
         self.zero_padding()
-        self.G.refresh()
-        self.D.refresh()
+        for net in self.nets():
+            net.refresh()
+
+    def nets(self):
+        """G, D and (InfoGAN) Q"""
+        return (self.G, self.D) if self.Q is None else (self.G, self.D, self.Q)
 
     def zero_padding(self):
         """zero the padding of D's padded weights (the 1-channel output layer's rows 1..15; BEGAN's embedding rows / columns
-        beyond e): their gradients are then zero, so they stay zero and the padded GEMM columns read zeros"""
+        beyond e; InfoGAN's Q head rows beyond nd + nc): their gradients are then zero, so they stay zero and the padded GEMM
+        columns read zeros"""
         if self.variant == "be":
             self.D.view("encoder.l5.weight")[self.e:].zero_()
             self.D.view("decoder.l1.weight")[:, self.e:].zero_()
         else:
             self.D.view("l5.weight")[1:].zero_()
+        if self.Q is not None:
+            self.Q.view("l5.weight")[self.nd + self.nc:].zero_()
 
     def _torch_views(self, which):
         """{torch-style name: view of the G / D tensor in torch's layout} over the flat params (which="params") or grads.
         Conv weights are [Cout, (kh, kw, ci)] here and [Cout, Cin, kh, kw] in torch; transposed-conv weights (G, BEGAN's
         decoder) are [(kh, kw, co), Cin] here and [Cin, Cout, kh, kw] in torch; BatchNorm vectors match.  Padded weights are
         trimmed on torch's dim 0 (_trim: D.l5 keeps output channel 0 of its 16 rows, BEGAN's encoder l5 / decoder l1 the e
-        embedding channels)."""
+        embedding channels, InfoGAN's Q.l5 its nd + nc code outputs)."""
         out = {}
-        for tag, net in (("G", self.G), ("D", self.D)):
+        for tag, net in zip("GDQ", self.nets()):
             for n in net.names:
                 w = net.view(n, getattr(net, which))
                 key = "%s.%s" % (tag, n)
@@ -253,14 +284,14 @@ class DcganEngine:
         return {k: v.detach().cpu().contiguous() for k, v in self._torch_views("params").items()}
 
     def torch_grads(self):
-        """{torch-style name: the current G / D gradient in torch's layout} (views of the device gradients)."""
+        """{torch-style name: the current G / D (/ Q) gradient in torch's layout} (views of the device gradients)."""
         return self._torch_views("grads")
 
     def load_torch_weights(self, sd):
         for k, v in self._torch_views("params").items():
             v.copy_(sd[k].float())
-        self.G.refresh()
-        self.D.refresh()
+        for net in self.nets():
+            net.refresh()
 
     def _buf(self, key, rows, cols, dtype=torch.bfloat16):
         t = self._bufs.get(key)
@@ -273,13 +304,21 @@ class DcganEngine:
     def g_forward(self, n, noise=None, seed=0, stream_id=0, tag="g", net=None, pfx="", x_rows=None, out_mode=C2I_SIGMOID, run=None):
         """G(z) for n samples -> (images [n*4096, ch] NHWC bf16, saved activations).  The same transposed-conv stack runs
         BEGAN's decoder: net / pfx name its weights (default G), x_rows [n, >= K] bf16 are its input rows instead of the
-        noise rows, out_mode is the final col2im's (C2I_NONE: linear output) and run its BatchNorm running statistics."""
+        noise rows, out_mode is the final col2im's (C2I_NONE: linear output) and run its BatchNorm running statistics.
+        InfoGAN without caller noise draws [z | one-hot | continuous] on the device (gm_info_noise_rows); its fp32 copy, the
+        MI loss's targets, is left in self.codes_[tag]."""
         net = self.G if net is None else net
         run = self.run_G if run is None else run
         K = net.shapes[pfx + "l1.weight"][1]
         if x_rows is None:
             x_rows = self._buf(tag + "z", n, self.zp)
-            check(self.h, lib().gm_noise_rows(self.h, _ptr(noise), _ptr(x_rows), n, self.z, self.zp, int(seed), int(stream_id), _stream()))
+            if self.variant == "info" and noise is None:
+                codes = self.codes_[tag] = self._buf(tag + "codes", n, self.zin, torch.float32)
+                check(self.h, lib().gm_info_noise_rows(self.h, _ptr(x_rows), self.zp, _ptr(codes), n, self.z, self.nd, self.nc, int(seed),
+                                                       int(stream_id), _stream()))
+            else:
+                check(self.h, lib().gm_noise_rows(self.h, _ptr(noise), _ptr(x_rows), n, self.zin, self.zp, int(seed), int(stream_id),
+                                                  _stream()))
         sv = {"z": x_rows, "n": n}
         gc = self.gc
         c = self._buf(tag + "c0", n, 16 * gc[0])
@@ -335,10 +374,14 @@ class DcganEngine:
         return dx
 
     # ------------------------------------------------------------------ discriminator
-    def d_forward(self, img, n, logits, tag, pfx=""):
+    def d_forward(self, img, n, logits, tag, pfx="", net=None, run=None):
         """D(img) for n NHWC images; logits: fp32 view [16, ld] (row 0 receives the n logits), or a bf16 [n, ep] buffer that
-        receives BEGAN's linear embedding (pfx "encoder.").  Returns saved activations."""
+        receives BEGAN's linear embedding (pfx "encoder.").  The same trunk runs InfoGAN's Q: net / run name its weights and
+        BatchNorm running statistics (default D's), and Q's head writes fp32 rows [n, qp] into logits.  Returns saved
+        activations."""
         dc = self.dc
+        net = self.D if net is None else net
+        run = self.run_D if run is None else run
         sv = {"n": n, "img": img}
         x, hw, cin = img, 64, self.ch
         for i in range(4):
@@ -348,28 +391,28 @@ class DcganEngine:
             c = self._buf(tag + "c%d" % i, n * hw * hw, dc[i])
             sv["col%d" % i] = col
             if i == 0 or not self.d_bn:
-                gemm_bf16(col, self.D.bf[pfx + "l%d.weight" % (i + 1)], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU epilogue
+                gemm_bf16(col, net.bf[pfx + "l%d.weight" % (i + 1)], c, "nt", act=3, act_slope=SLOPE)   # conv + LeakyReLU epilogue
                 y = c
             else:
-                gemm_bf16(col, self.D.bf[pfx + "l%d.weight" % (i + 1)], c, "nt")
+                gemm_bf16(col, net.bf[pfx + "l%d.weight" % (i + 1)], c, "nt")
                 y = self._buf(tag + "y%d" % i, c.shape[0], dc[i])
                 st = self._buf(tag + "st%d" % i, 2, dc[i], torch.float32)
-                _bn_fwd(c, self.D.view(pfx + "bn%d.weight" % (i + 1)), self.D.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, st,
-                        self.run_D[i])
+                _bn_fwd(c, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, st, run[i])
                 sv["c%d" % i], sv["st%d" % i] = c, st
             sv["y%d" % i] = y
             x, cin = y, dc[i]
         flat = x.view(n, 16 * dc[3])
         sv["flat"] = flat
-        # fp32 [16, ld] with row 0 = logits, or the bf16 embedding rows [n, ep]
-        gemm_bf16(flat, self.D.bf[pfx + "l5.weight"], logits, "nt", transpose=logits.dtype == torch.float32)
+        # D: fp32 [16, ld] with row 0 = logits (transposed store); Q: fp32 rows [n, qp]; BEGAN: the bf16 embedding rows [n, ep]
+        gemm_bf16(flat, net.bf[pfx + "l5.weight"], logits, "nt", transpose=logits.dtype == torch.float32 and net is not self.Q)
         return sv
 
-    def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d", pfx="", dimg_mode=C2I_SIGMOID_GRAD):
-        """ds [n] fp32 = dL/dlogit, or a bf16 [n, ep] upstream gradient of BEGAN's embedding (pfx "encoder.").  Accumulates
-        nothing: writes this pass's D gradient into `grads` (flat, D layout) when need_wgrad; returns dL/d(pre-sigmoid
-        generator output) (dimg_mode C2I_SIGMOID_GRAD) or dL/d(image) (C2I_NONE) when need_dimg."""
-        n, dc, D = sv["n"], self.dc, self.D
+    def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d", pfx="", dimg_mode=C2I_SIGMOID_GRAD, net=None):
+        """ds [n] fp32 = dL/dlogit, or a bf16 [n, ep] upstream gradient of BEGAN's embedding (pfx "encoder.") or of InfoGAN's
+        Q head (net = self.Q, [n, qp]).  Accumulates nothing: writes this pass's D (Q) gradient into `grads` (flat, that net's
+        layout) when need_wgrad; returns dL/d(pre-sigmoid generator output) (dimg_mode C2I_SIGMOID_GRAD) or dL/d(image)
+        (C2I_NONE) when need_dimg."""
+        n, dc, D = sv["n"], self.dc, self.D if net is None else net
         if ds.dtype == torch.bfloat16:
             dy5 = ds
         else:
@@ -405,13 +448,14 @@ class DcganEngine:
             gemm_bf16(d, sv["col0"], D.view(pfx + "l1.weight", grads), "tn")              # [h, 16 ch]
         if not need_dimg:
             return None
-        return self._dimg(sv, d, tag, dimg_mode, pfx)
+        return self._dimg(sv, d, tag, dimg_mode, pfx, D)
 
-    def _dimg(self, sv, d, tag, mode=C2I_SIGMOID_GRAD, pfx=""):
+    def _dimg(self, sv, d, tag, mode=C2I_SIGMOID_GRAD, pfx="", net=None):
         """d = dL/d(conv 1 output) -> dL/d(image) (mode C2I_NONE) or dL/d(pre-sigmoid generator output) (C2I_SIGMOID_GRAD)"""
         n = d.shape[0] // 1024
+        net = self.D if net is None else net
         dcol = self._buf(tag + "dcol0", d.shape[0], 16 * self.ch)
-        gemm_bf16(d, self.D.bf_t[pfx + "l1.weight"], dcol, "nt")
+        gemm_bf16(d, net.bf_t[pfx + "l1.weight"], dcol, "nt")
         dpre = self._buf(tag + ("dpre" if mode == C2I_SIGMOID_GRAD else "dimg"), n * 4096, self.ch)
         _col2im(dcol, n, 32, 32, self.ch, dpre, mode, sv["img"] if mode == C2I_SIGMOID_GRAD else None)
         return dpre
@@ -443,8 +487,9 @@ class DcganEngine:
         return x.view(n * 4096, self.ch)
 
     # the per-row loss each variant's rows share: WGAN-GP's are W's and DRAGAN's NS's (the penalty is separate); the G steps of
-    # RaNS and Fisher are NS's and W's -mean(D(G(z))) (src/ra_gan.py, src/fisher_gan.py train_G)
-    _ROW_LOSS = {"wgp": "w", "dra": "ns", "ra": "ns", "fisher": "w"}
+    # RaNS and Fisher are NS's and W's -mean(D(G(z))) (src/ra_gan.py, src/fisher_gan.py train_G); InfoGAN's D and G steps
+    # are NS's (src/info_gan.py:223-267)
+    _ROW_LOSS = {"wgp": "w", "dra": "ns", "ra": "ns", "fisher": "w", "info": "ns"}
 
     def _loss_rows(self, logits, n, g_step, inv, ds, loss):
         variant = VARIANTS[self._ROW_LOSS.get(self.variant, self.variant)]
@@ -645,6 +690,50 @@ class DcganEngine:
         # BEGAN: both learning rates carry the plateau scale be_state[7]; the reference's two schedulers see the same
         # measure with the same settings (src/be_gan.py:133-136,194-195), so one scale is exact
         (self.G if net == 0 else self.D).adam(hp, self.be_state[7:8] if self.variant == "be" else None)
+
+    # ------------------------------------------------------------------ InfoGAN (src/info_gan.py:269-304)
+    # The MI step's Philox streams: bit 63 set, so that no D draw (2 step) or G draw (2 step + 1) of any step reaches them
+    MI_STREAM = 1 << 63
+
+    def q_grad(self, n, noise=None, inv_global_batch=None, seed=0, step=0, lam=1.0):
+        """train_Q + MI_loss.backward() (src/info_gan.py:269-304): fresh codes (noise [n, zin] fp32, or Philox keyed by (seed,
+        MI_STREAM + step)), G(codes), Q(G(codes)) as fp32 rows, MI_loss = lam (CE(discrete, argmax one-hot) + MSE(continuous,
+        code)).  The gradient reaches Q and G (G's output is not detached): writes Q.grads and G.grads (both carry
+        lam inv_global_batch) and mi_loss[0] (lam times this process's mean)."""
+        if self.variant != "info":
+            raise GmError("q_grad is InfoGAN's MI step (variant='info')")
+        inv = 1.0 / n if inv_global_batch is None else inv_global_batch
+        if noise is not None:
+            noise = noise.reshape(n, self.zin).float().contiguous()
+        fake, gsv = self.g_forward(n, noise, seed, self.MI_STREAM + int(step))
+        codes = self.codes_["g"] if noise is None else noise
+        qrows = self._buf("q_rows", n, self.qp, torch.float32)
+        sv = self.d_forward(fake, n, qrows, "q", net=self.Q, run=self.run_Q)
+        dq = self._buf("q_dq", n, self.qp)
+        check(self.h, lib().gm_info_loss_rows(self.h, _ptr(qrows), self.qp, _ptr(codes), self.zin, self.z, n, self.nd, self.nc, inv * lam,
+                                              _ptr(dq), self.qp, _ptr(self.mi_loss), _stream()))
+        if lam != 1.0:
+            self.mi_loss.mul_(lam)
+        dpre = self.d_backward(sv, dq, self.Q.grads, need_dimg=True, tag="q", net=self.Q)
+        self.g_backward(gsv, dpre)
+        # the step's stored tensors: codes, Q's rows and their gradient, dL/d(pre-sigmoid G output), the saved activations
+        self.q_saved_ = dict(codes=codes, q=qrows, dq=dq, dpre=dpre, qsv=sv, gsv=gsv, fake=fake)
+        return self.mi_loss[0]
+
+    def apply_mi(self, hp):
+        """MI_optimizer.step() (src/info_gan.py:148,205): Adam over G with MI_optimizer's own moments (not G.exp_avg /
+        exp_avg_sq, which are G_optimizer's) and over Q, one step count for both; refreshes both operand copies"""
+        self.Q.adam(hp)
+        adam_step(self.G.params, self.G.grads, self.g_mi_avg, self.g_mi_avg_sq, hp, self.Q.step)
+        self.G.refresh()
+
+    def infer_codes(self, images):
+        """Q(images) (src/info_gan.py:90-94): flat [n, ch*64*64] (NCHW flattened) -> (discrete logits [n, nd], continuous
+        [n, nc]) fp32"""
+        n = images.shape[0]
+        qrows = self._buf("qi_rows", n, self.qp, torch.float32)
+        self.d_forward(self.stage_images(images), n, qrows, "qi", net=self.Q, run=self.run_Q)
+        return qrows[:, :self.nd].clone(), qrows[:, self.nd:self.nd + self.nc].clone()
 
     # ------------------------------------------------------------------ BEGAN (src/be_gan.py:212-258)
     def began_state(self, values=None):

@@ -384,6 +384,17 @@ int gm_began_loss_final(gm_ctx* ctx, const double* sum_x_dev, const double* sum_
 int gm_began_control(gm_ctx* ctx, float* state_dev, float gamma, float lambda, float patience, gm_stream stream);
 int gm_began_dfake_rows(gm_ctx* ctx, const void* T_dev, const void* dr_dev, const void* fake_dev, void* out_dev, int rows, int cols,
                         gm_stream stream);
+/* InfoGAN (src/info_gan.py:269-325) on the conv path.  gm_info_noise_rows: compute_noise on the device, Philox keyed by
+ * (seed, stream_id): out_dev [rows, ld] bf16 = [z (zd) N(0,1) | one-hot of a category uniform over [0, nd) | nc N(0,1) | 1 | 0
+ * ...] (the layout of gm_noise_rows' rows, ld a multiple of 8, > zd + nd + nc) and codes_dev [rows, zd + nd + nc] fp32 = the
+ * same values (every one bf16-representable).  gm_info_loss_rows: on Q's rows q_dev [rows, ldq] fp32 ([0, nd) categorical
+ * logits, [nd, nd + nc) continuous code) and the codes [rows, ldc] (one-hot at [zd, zd + nd), continuous at [zd + nd, zd + nd
+ * + nc)): loss_dev[0] = mean CE + mean squared error over rows x nc, grad_dev [rows, ldo] bf16 = (softmax - onehot) inv and
+ * 2 (q - c) inv / nc (inv = inv_global_batch), zero in columns [nd + nc, ldo). */
+int gm_info_noise_rows(gm_ctx* ctx, void* out_dev, int ld, float* codes_dev, int rows, int zd, int nd, int nc, uint64_t seed,
+                       uint64_t stream_id, gm_stream stream);
+int gm_info_loss_rows(gm_ctx* ctx, const float* q_dev, int ldq, const float* codes_dev, int ldc, int zd, int rows, int nd, int nc,
+                      float inv_global_batch, void* grad_dev, int ldo, float* loss_dev, gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);

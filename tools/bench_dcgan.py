@@ -1,4 +1,4 @@
-"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP, DRAGAN and BEGAN train steps (D_steps = 1) on one GPU, in one process.
+"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP, DRAGAN, BEGAN and InfoGAN train steps (D_steps = 1) on one GPU, in one process.
 
     python tools/bench_dcgan.py [--batch 1024] [--steps 20] [--warmup 5]
 
@@ -9,8 +9,9 @@ all alike.  Prints one JSON line: device name and power limit (read in the same 
 time, images/s, library launches per step, the ratio to NSGAN and achieved TFLOP/s from FLOPs counted from the shapes
 (bench.py's _dcgan_flop_per_img; the penalised critics of WGAN-GP and DRAGAN add one critic forward, one input-gradient
 chain to the image, one tangent forward and one weight-gradient pass = 4 critic forwards; BEGAN's from its autoencoder's
-shapes, began_flop_per_img).  BEGAN's step includes began_control, as its trainer runs it after every G update.  Writes
-nothing but stdout.
+shapes, began_flop_per_img; InfoGAN's from its G, D and Q shapes, info_flop_per_img).  BEGAN's step includes
+began_control, and InfoGAN's the MI step and MI_optimizer's update (q_grad + apply_mi), as their trainers run them after
+every G update.  Writes nothing but stdout.
 """
 import argparse
 import json
@@ -23,8 +24,8 @@ for p in (ROOT, os.path.join(ROOT, "generative-models_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-VARIANTS = ("ns", "ra", "fisher", "wgp", "dra", "be")
-LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4, "be": 1e-4}     # the reference's defaults per variant
+VARIANTS = ("ns", "ra", "fisher", "wgp", "dra", "be", "info")
+LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4, "be": 1e-4, "info": 2e-4}     # the reference's defaults per variant
 
 
 def critic_flop_per_img(hd=64, ch=3):
@@ -47,6 +48,18 @@ def began_flop_per_img(hd=64, z=100, e=100, ch=3):
     ae_dgrad = 2.0 * ae                              # G step: input-gradient chain only, down to the image
     g_bwd = 2.0 * (2 * sum(g_l) - g_l[0])
     return (Gf + 2 * AEf + 2 * ae_bwd) + (Gf + AEf + ae_dgrad + g_bwd)
+
+
+def info_flop_per_img(hd=64, z=100, nd=10, nc=10, ch=3):
+    """algorithmic FLOPs of one InfoGAN step, counted like bench.py's _dcgan_flop_per_img: the NSGAN D and G steps with G's
+    input z + nd + nc wide, then the MI step = G fwd + Q fwd + Q bwd (weight grads everywhere, input grads down to the
+    image) + G bwd"""
+    from bench import _dcgan_flop_per_img
+    gc, dc = [8 * hd, 4 * hd, 2 * hd, hd, ch], [hd, 2 * hd, 4 * hd, 8 * hd]
+    q_l = [1024 * dc[0] * 16 * ch, 256 * dc[1] * 16 * dc[0], 64 * dc[2] * 16 * dc[1], 16 * dc[3] * 16 * dc[2], 16 * dc[3] * (nd + nc)]
+    g_l = [(z + nd + nc) * 16 * gc[0], 16 * gc[0] * 16 * gc[1], 64 * gc[1] * 16 * gc[2], 256 * gc[2] * 16 * gc[3], 1024 * gc[3] * 16 * gc[4]]
+    mi = 2.0 * sum(g_l) + 2.0 * sum(q_l) + 2.0 * (2 * sum(q_l)) + 2.0 * (2 * sum(g_l) - g_l[0])
+    return _dcgan_flop_per_img(hd, z + nd + nc, ch) + mi
 
 
 def power_limit(index):
@@ -83,6 +96,9 @@ def main():
         eng.apply(0, hp)
         if name == "be":
             eng.began_control(0.5, 1e-3, 5 * 4)                 # GAMMA, LAMBDA, patience 5 len(train_iter) of src/be_gan.py
+        if name == "info":
+            eng.q_grad(B, seed=1000, step=s)                    # the MI step and MI_optimizer (src/info_gan.py:196-205)
+            eng.apply_mi(hp)
 
     launches = {}
     for name in VARIANTS:
@@ -111,6 +127,8 @@ def main():
         med = sorted(ms[name])[len(ms[name]) // 2]
         if name == "be":
             flop = began_flop_per_img()
+        elif name == "info":
+            flop = info_flop_per_img()
         else:
             flop = _dcgan_flop_per_img() + (4 * critic_flop_per_img() if name in ("wgp", "dra") else 0.0)
         out[name] = {"median_ms": round(med, 3), "min_ms": round(min(ms[name]), 3), "images_per_s": round(B / med * 1e3, 1),
