@@ -102,7 +102,57 @@ def dcgan_init(module):
             nn.init.zeros_(m.bias)
 
 
-class DCGANTrainer:
+def module_params(nets):
+    """{"<prefix>.<name>": parameter} of the (state_dict prefix, module) pairs nets"""
+    return {"%s.%s" % (tag, k): v.detach() for tag, mod in nets for k, v in mod.named_parameters()}
+
+
+def pull_running_stats(eng, nets):
+    """eng's BatchNorm running statistics -> the bn1..bn4 buffers of the (state_dict prefix, module) pairs nets"""
+    runs = {"G": eng.run_G, "D": eng.run_D, "Q": eng.run_Q}
+    with torch.no_grad():
+        for tag, mod in nets:
+            for i, bn in ((i, getattr(mod, "bn%d" % i, None)) for i in range(1, 5)):       # a critic may have none
+                run = runs[tag].get(i - 1)
+                if bn is not None and run is not None:
+                    bn.running_mean.copy_(run[0].cpu())
+                    bn.running_var.copy_(run[1].cpu())
+
+
+class EngineSync:
+    """Parameter sync between a trainer's DcganEngine (self._engine) and its model's modules (self._nets(): (state_dict
+    prefix, module) pairs); self._dirty marks module parameters newer than the engine's"""
+
+    def _sd(self):
+        return module_params(self._nets())
+
+    def _torch_tensors(self, grads=False):
+        """the engine's parameters (grads=True: gradients) in torch's layouts under the modules' "<prefix>.<name>" names"""
+        return self._engine.torch_grads() if grads else self._engine.torch_weights()
+
+    def _pull(self):
+        """engine -> module parameters (after training; before state_dict / save_model)"""
+        if self._engine is None:
+            return
+        tw = self._torch_tensors()
+        with torch.no_grad():
+            for tag, mod in self._nets():
+                for k, v in mod.named_parameters():
+                    v.copy_(tw["%s.%s" % (tag, k)].to(v.device))
+        pull_running_stats(self._engine, self._nets())
+
+    def _fused_loss(self, mods, loss_val):
+        """loss_val as a 0-dim loss whose backward() puts the engine's current gradients of the (tag, module) pairs `mods`
+        on those modules' parameters"""
+        tg = self._torch_tensors(grads=True)
+        named = [(tag, k, p) for tag, mod in mods for k, p in mod.named_parameters()]
+        params = [p for _, _, p in named]
+        flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for tag, k, p in named])
+        self._dirty = True                                            # the caller's optimizer will change the module parameters
+        return _FusedLoss.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat, params)
+
+
+class DCGANTrainer(EngineSync):
     """ Object to hold data iterators, train a GAN variant (surface of src/ns_gan.py:77-290) """
     variant = "ns"
 
@@ -125,13 +175,6 @@ class DCGANTrainer:
         """(state_dict prefix, module) of every network the engine trains"""
         return [("G", self.model.G), ("D", self.model.D)]
 
-    def _sd(self):
-        out = {}
-        for tag, mod in self._nets():
-            for k, v in mod.named_parameters():
-                out["%s.%s" % (tag, k)] = v.detach()
-        return out
-
     def _engine_synced(self):
         m = self.model
         if self._engine is None:
@@ -143,23 +186,6 @@ class DCGANTrainer:
             self._engine.load_torch_weights(self._sd())
             self._dirty = False
         return self._engine
-
-    def _pull(self):
-        """engine -> module parameters (after training; before state_dict / save_model)"""
-        if self._engine is None:
-            return
-        eng = self._engine
-        tw = eng.torch_weights()
-        runs = {"G": eng.run_G, "D": eng.run_D, "Q": eng.run_Q}
-        with torch.no_grad():
-            for tag, mod in self._nets():
-                for k, v in mod.named_parameters():
-                    v.copy_(tw["%s.%s" % (tag, k)].to(v.device))
-                for i, bn in ((i, getattr(mod, "bn%d" % i, None)) for i in range(1, 5)):       # a critic may have none
-                    run = runs[tag].get(i - 1)
-                    if bn is not None and run is not None:
-                        bn.running_mean.copy_(run[0].cpu())
-                        bn.running_var.copy_(run[1].cpu())
 
     # ------------------------------------------------------------------ reference surface
     def train(self, num_epochs, G_lr=2e-4, D_lr=2e-4, D_steps=1):
@@ -215,16 +241,6 @@ class DCGANTrainer:
 
     def _loss(self, net, loss_val):
         return self._fused_loss([("G", self.model.G)] if net == 0 else [("D", self.model.D)], loss_val)
-
-    def _fused_loss(self, mods, loss_val):
-        """loss_val as a 0-dim loss whose backward() puts the engine's current gradients of the (tag, module) pairs `mods`
-        on those modules' parameters"""
-        tg = self._engine.torch_grads()
-        named = [(tag, k, p) for tag, mod in mods for k, p in mod.named_parameters()]
-        params = [p for _, _, p in named]
-        flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for tag, k, p in named])
-        self._dirty = True                                            # the caller's optimizer will change the module parameters
-        return _FusedLoss.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat, params)
 
     def train_D(self, images):
         """ Run 1 step of training for discriminator (src/ns_gan.py:172-194): returns D_loss; .backward() delivers the gradients """

@@ -151,6 +151,10 @@ def lib():
     L.gm_began_dfake_rows.argtypes = [vp, vp, vp, vp, vp, i, i, vp]
     L.gm_info_noise_rows.argtypes = [vp, vp, i, vp, i, i, i, i, u64, u64, vp]
     L.gm_info_loss_rows.argtypes = [vp, vp, i, vp, i, i, i, i, i, f, vp, i, vp, vp]
+    L.gm_sse_sigmoid_rows.argtypes = [vp, vp, vp, i, i, f, vp, vp, vp]
+    L.gm_vae_latent_rows.argtypes = [vp, vp, i, vp, vp, vp, i, i, i, u64, u64, vp, vp]
+    L.gm_vae_dlatent_rows.argtypes = [vp, vp, i, vp, i, vp, vp, i, i, i, f, vp]
+    L.gm_bn_forward_eval.argtypes = [vp, vp, ll, i, i, vp, vp, vp, f, i, f, vp, i, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]

@@ -626,6 +626,61 @@ __global__ void __launch_bounds__(256) l1_sum_kernel(const double* __restrict__ 
   if (threadIdx.x == 0) out[0] = s;
 }
 
+// ---- The VAE's reconstruction loss (src/vae.py:203) through the conv decoder's sigmoid output
+// out = sigmoid(pre) and x: `groups` 16-byte groups of bf16 (NHWC image rows back to back; out as col2im's C2I_SIGMOID mode
+// stores it).  grad = 2 scale (out - x) out (1 - out) = d(scale sum (x - out)^2)/d(pre) as bf16, and the block's partial of
+// sum (x - out)^2 in double (x - out of two bf16 values is exact in double); l1_sum_kernel adds the partials in fixed order.
+constexpr int kSseUnroll = 2;
+__global__ void __launch_bounds__(256) sse_sigmoid_rows_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ x,
+                                                               uint32_t groups, float scale, __nv_bfloat16* __restrict__ grad,
+                                                               double* __restrict__ part) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  const float k = 2.f * scale;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  double acc = 0.0;
+  for (uint32_t i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < groups; i0 += stride * kSseUnroll) {
+    uint4 ov[kSseUnroll], xv[kSseUnroll];
+#pragma unroll
+    for (int u = 0; u < kSseUnroll; ++u) {
+      const uint32_t i = i0 + u * stride;
+      ov[u] = xv[u] = make_uint4(0, 0, 0, 0);
+      if (i < groups && i >= i0) {
+        ov[u] = __ldg(reinterpret_cast<const uint4*>(out) + i);
+        xv[u] = __ldg(reinterpret_cast<const uint4*>(x) + i);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kSseUnroll; ++u) {
+      const uint32_t i = i0 + u * stride;
+      if (i >= groups || i < i0) continue;
+      const uint32_t a[4] = {ov[u].x, ov[u].y, ov[u].z, ov[u].w}, b[4] = {xv[u].x, xv[u].y, xv[u].z, xv[u].w};
+      float o[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const float oo = (q & 1) ? bf16_hi(a[q >> 1]) : bf16_lo(a[q >> 1]);
+        const float xx = (q & 1) ? bf16_hi(b[q >> 1]) : bf16_lo(b[q >> 1]);
+        const double d = double(oo) - double(xx);
+        acc = fma(d, d, acc);
+        o[q] = k * (oo - xx) * oo * (1.f - oo);
+      }
+      store_bf16x8(grad + size_t(i) * 8, o, 0);
+    }
+  }
+  acc = block_sum<256>(acc, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = acc;
+}
+
+// Inference-mode BatchNorm2d's (mean, invstd) from the running statistics: stats[c] = running[0][c], stats[C + c] =
+// 1 / sqrt(running[1][c] + eps), in bn_finalize_kernel's layout and precision, for bn_apply_kernel
+__global__ void bn_eval_stats_kernel(const float* __restrict__ running, int C, float eps, float* __restrict__ stats) {
+  griddep_sync();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  stats[c] = running[c];
+  stats[C + c] = float(1.0 / sqrt(double(running[C + c]) + double(eps)));
+}
+
 // ---- InfoGAN's structured generator input (compute_noise, src/info_gan.py:306-325) drawn on the device
 // Row r of the bf16 GEMM operand out [rows, ld] is [z (zd) | one-hot (nd) | continuous code (nc) | 1 | 0 ...], and codes
 // [rows, K = zd + nd + nc] fp32 holds the same K values (the MI loss's targets).  The N(0, 1) values are rounded to bf16

@@ -22,7 +22,11 @@ src/be_gan.py:212-258) makes D an autoencoder: the D trunk above with a linear e
 generator stack with a linear output as the decoder, L1 reconstruction losses (gm_l1_rows) and K and the plateau scheduler
 as device state (be_state, gm_began_control).  variant="info" (InfoGAN, src/info_gan.py:130-325) feeds G [z | one-hot |
 continuous code] drawn on the device (gm_info_noise_rows) and adds Q, a second D trunk with a linear code head, trained with
-G by the MI step (q_grad, gm_info_loss_rows) and MI_optimizer's own Adam state for G (apply_mi).
+G by the MI step (q_grad, gm_info_loss_rows) and MI_optimizer's own Adam state for G (apply_mi).  variant="vae" (the VAE
+of src/vae.py:47-212 with conv nets) makes D the encoder - the D trunk with a linear head of 2 z outputs, mu then log_var -
+and G the decoder; vae_grad runs compute_batch + (recon + kl).backward() with the reparameterisation and KL
+(gm_vae_latent_rows, gm_vae_dlatent_rows) and the sum of squared errors through the sigmoid output (gm_sse_sigmoid_rows) on
+the device, and train=False forwards (model.eval()) run every BatchNorm on its running statistics (gm_bn_forward_eval).
 
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
@@ -72,6 +76,12 @@ def _bn_fwd(x, gamma, beta, act, y, stats, running):
     h = _lib.ctx()
     check(h, lib().gm_bn_forward(h, _ptr(x), x.shape[0], x.shape[1], x.stride(0), _ptr(gamma), _ptr(beta), BN_EPS, act, SLOPE,
                                  _ptr(y), y.stride(0), _ptr(stats), _ptr(running), BN_MOMENTUM, _stream()))
+
+
+def _bn_fwd_eval(x, gamma, beta, act, y, running):
+    h = _lib.ctx()
+    check(h, lib().gm_bn_forward_eval(h, _ptr(x), x.shape[0], x.shape[1], x.stride(0), _ptr(gamma), _ptr(beta), _ptr(running), BN_EPS, act,
+                                      SLOPE, _ptr(y), y.stride(0), _stream()))
 
 
 def _bn_bwd(dy, x, stats, gamma, beta, act, dx, dgb):
@@ -131,8 +141,8 @@ class DcganEngine:
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be", "info") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra, be and info")
+        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be", "info", "vae") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra, be, info and vae")
         if embed_dim is not None and (variant != "be" or embed_dim <= 0):
             raise GmError("embed_dim is the positive embedding width of BEGAN's autoencoder D (variant='be')")
         if variant == "info":
@@ -142,7 +152,12 @@ class DcganEngine:
                 raise GmError("InfoGAN needs disc_dim >= 1 and cont_dim >= 1")
         elif disc_dim is not None or cont_dim is not None:
             raise GmError("disc_dim and cont_dim are the code widths of InfoGAN (variant='info')")
-        if variant == "be":
+        if variant == "vae":
+            # the VAE's encoder ends in the linear mu / log_var heads (src/vae.py:55-61)
+            if d_out_act is not None:
+                raise GmError("the VAE's encoder heads are linear; d_out_act is a discriminator option")
+            d_out_act = "none"
+        elif variant == "be":
             # BEGAN's D is an autoencoder whose reconstruction is linear (src/be_gan.py:73-76)
             if d_out_act not in (None, "none"):
                 raise GmError("the BEGAN autoencoder's output is linear (d_out_act='none')")
@@ -192,11 +207,17 @@ class DcganEngine:
 
         self.e = z_dim if embed_dim is None else int(embed_dim)  # BEGAN's embedding width (N_h = N_z in the BEGAN paper)
         self.ep = (self.e + 15) // 16 * 16                       # embedding rows: [e | 0 pad], N of a bf16-output GEMM
+        self.mp = (2 * z_dim + 15) // 16 * 16                    # VAE encoder head rows: [mu | log_var | 0 pad]
         if variant == "be":
             # D = encoder (the DCGAN D trunk, l5: e outputs, zero-padded to ep rows) + decoder (the generator stack with e
             # in place of z, l1's input columns zero-padded to ep); the torch views trim the padding (_TRIM)
             self._trim = {"D.encoder.l5.weight": self.e, "D.decoder.l1.weight": self.e}
             d_shapes = d_stack("encoder.", self.ep) + g_stack("decoder.", self.ep)
+        elif variant == "vae":
+            # the VAE's encoder: l5 is the mu head (rows [0, z)) stacked on the log_var head (rows [z, 2z)), zero-padded to mp
+            # rows (the N of the fp32 row-major head GEMM)
+            self._trim = {"D.l5.weight": 2 * z_dim}
+            d_shapes = d_stack("", self.mp)
         else:
             self._trim = {"D.l5.weight": 1}
             d_shapes = d_stack("", 16)                           # 1 real output channel (row 0), padded to the MMA's N = 16
@@ -223,6 +244,7 @@ class DcganEngine:
         self.be_state = torch.zeros(11, device=self.device)
         if variant == "be":
             self.began_init(0.0, 1)
+        self.vae_loss = torch.zeros(2, device=self.device)       # VAE: (recon, kl) of the last vae_grad, this process's sums
         self._bufs = {}
         self.init_weights()
 
@@ -249,13 +271,13 @@ class DcganEngine:
 
     def zero_padding(self):
         """zero the padding of D's padded weights (the 1-channel output layer's rows 1..15; BEGAN's embedding rows / columns
-        beyond e; InfoGAN's Q head rows beyond nd + nc): their gradients are then zero, so they stay zero and the padded GEMM
-        columns read zeros"""
+        beyond e; InfoGAN's Q head rows beyond nd + nc; the VAE encoder's head rows beyond 2 z): their gradients are then zero,
+        so they stay zero and the padded GEMM columns read zeros"""
         if self.variant == "be":
             self.D.view("encoder.l5.weight")[self.e:].zero_()
             self.D.view("decoder.l1.weight")[:, self.e:].zero_()
         else:
-            self.D.view("l5.weight")[1:].zero_()
+            self.D.view("l5.weight")[self._trim["D.l5.weight"]:].zero_()
         if self.Q is not None:
             self.Q.view("l5.weight")[self.nd + self.nc:].zero_()
 
@@ -301,12 +323,14 @@ class DcganEngine:
         return t[:rows]
 
     # ------------------------------------------------------------------ generator
-    def g_forward(self, n, noise=None, seed=0, stream_id=0, tag="g", net=None, pfx="", x_rows=None, out_mode=C2I_SIGMOID, run=None):
+    def g_forward(self, n, noise=None, seed=0, stream_id=0, tag="g", net=None, pfx="", x_rows=None, out_mode=C2I_SIGMOID, run=None,
+                  train=True):
         """G(z) for n samples -> (images [n*4096, ch] NHWC bf16, saved activations).  The same transposed-conv stack runs
         BEGAN's decoder: net / pfx name its weights (default G), x_rows [n, >= K] bf16 are its input rows instead of the
         noise rows, out_mode is the final col2im's (C2I_NONE: linear output) and run its BatchNorm running statistics.
         InfoGAN without caller noise draws [z | one-hot | continuous] on the device (gm_info_noise_rows); its fp32 copy, the
-        MI loss's targets, is left in self.codes_[tag]."""
+        MI loss's targets, is left in self.codes_[tag].  train=False (inference mode, the VAE's model.eval()) normalises with the
+        running statistics and leaves them unchanged; its activations are not for g_backward."""
         net = self.G if net is None else net
         run = self.run_G if run is None else run
         K = net.shapes[pfx + "l1.weight"][1]
@@ -328,7 +352,10 @@ class DcganEngine:
         for i in range(4):
             a = self._buf(tag + "a%d" % i, x.shape[0], gc[i])
             st = self._buf(tag + "st%d" % i, 2, gc[i], torch.float32)
-            _bn_fwd(x, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_RELU, a, st, run[i])
+            if train:
+                _bn_fwd(x, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_RELU, a, st, run[i])
+            else:
+                _bn_fwd_eval(x, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_RELU, a, run[i])
             sv["c%d" % i], sv["a%d" % i], sv["st%d" % i] = x, a, st
             col = self._buf(tag + "col%d" % i, a.shape[0], 16 * gc[i + 1])
             gemm_bf16(a, net.bf[pfx + "l%d.weight" % (i + 2)], col, "nt")
@@ -338,10 +365,11 @@ class DcganEngine:
         sv["img"] = x
         return x, sv
 
-    def g_backward(self, sv, dpre, net=None, pfx="", grads=None, need_wgrad=True, need_dx=False, tag="g"):
+    def g_backward(self, sv, dpre, net=None, pfx="", grads=None, need_wgrad=True, need_dx=False, tag="g", dx_dtype=torch.bfloat16):
         """dpre [n*4096, ch] = dL/d(pre-sigmoid output) -> flat G gradient (self.G.grads, zeroed first).  For BEGAN's decoder
         (net / pfx, see g_forward) dpre is dL/d(linear output) and the weight gradients go to the flat D-layout `grads` when
-        need_wgrad; need_dx returns dL/d(input rows) [n, ep] bf16 instead (one more GEMM, with l1's transposed copy)."""
+        need_wgrad; need_dx returns dL/d(input rows) [n, K] (K = l1's input columns) instead, bf16 (BEGAN's embedding
+        gradient) or dx_dtype=torch.float32 (the VAE's dL/dz) (one more GEMM, with l1's transposed copy)."""
         n, gc = sv["n"], self.gc
         net = self.G if net is None else net
         if grads is None and need_wgrad:
@@ -369,16 +397,17 @@ class DcganEngine:
             gemm_bf16(d.view(n, 16 * gc[0]), sv["z"], net.view(w1, grads), "tn", N=net.shapes[w1][1])   # [(kh,kw,co), z]
         if not need_dx:
             return grads
-        dx = self._buf(tag + "dx", n, net.shapes[w1][1])
+        dx = self._buf(tag + ("dx" if dx_dtype == torch.bfloat16 else "dx32"), n, net.shapes[w1][1], dx_dtype)
         gemm_bf16(d.view(n, 16 * gc[0]), net.bf_t[w1], dx, "nt")                             # [n, ep] = d Wm
         return dx
 
     # ------------------------------------------------------------------ discriminator
-    def d_forward(self, img, n, logits, tag, pfx="", net=None, run=None):
+    def d_forward(self, img, n, logits, tag, pfx="", net=None, run=None, train=True):
         """D(img) for n NHWC images; logits: fp32 view [16, ld] (row 0 receives the n logits), or a bf16 [n, ep] buffer that
         receives BEGAN's linear embedding (pfx "encoder.").  The same trunk runs InfoGAN's Q: net / run name its weights and
-        BatchNorm running statistics (default D's), and Q's head writes fp32 rows [n, qp] into logits.  Returns saved
-        activations."""
+        BatchNorm running statistics (default D's), and Q's head writes fp32 rows [n, qp] into logits; the VAE encoder's head
+        writes fp32 rows [n, mp].  train=False (the VAE's model.eval()) normalises with the running statistics and leaves them
+        unchanged.  Returns saved activations."""
         dc = self.dc
         net = self.D if net is None else net
         run = self.run_D if run is None else run
@@ -397,14 +426,19 @@ class DcganEngine:
                 gemm_bf16(col, net.bf[pfx + "l%d.weight" % (i + 1)], c, "nt")
                 y = self._buf(tag + "y%d" % i, c.shape[0], dc[i])
                 st = self._buf(tag + "st%d" % i, 2, dc[i], torch.float32)
-                _bn_fwd(c, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, st, run[i])
+                if train:
+                    _bn_fwd(c, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, st, run[i])
+                else:
+                    _bn_fwd_eval(c, net.view(pfx + "bn%d.weight" % (i + 1)), net.view(pfx + "bn%d.bias" % (i + 1)), ACT_LRELU, y, run[i])
                 sv["c%d" % i], sv["st%d" % i] = c, st
             sv["y%d" % i] = y
             x, cin = y, dc[i]
         flat = x.view(n, 16 * dc[3])
         sv["flat"] = flat
-        # D: fp32 [16, ld] with row 0 = logits (transposed store); Q: fp32 rows [n, qp]; BEGAN: the bf16 embedding rows [n, ep]
-        gemm_bf16(flat, net.bf[pfx + "l5.weight"], logits, "nt", transpose=logits.dtype == torch.float32 and net is not self.Q)
+        # D: fp32 [16, ld] with row 0 = logits (transposed store); Q and the VAE encoder: fp32 rows [n, qp] / [n, mp]; BEGAN:
+        # the bf16 embedding rows [n, ep]
+        gemm_bf16(flat, net.bf[pfx + "l5.weight"], logits, "nt",
+                  transpose=logits.dtype == torch.float32 and net is not self.Q and self.variant != "vae")
         return sv
 
     def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d", pfx="", dimg_mode=C2I_SIGMOID_GRAD, net=None):
@@ -533,6 +567,8 @@ class DcganEngine:
         WGAN-GP: eps [n] fp32 (None = on-device Philox keyed by (seed, step)).  DRAGAN: gp_k, dra_c (None = self.gp_k,
         self.dra_c), delta [n] and u [n, ch*64*64] (the reference's NCHW-flattened layout) or None for Philox.  RaNS, Fisher
         and DRAGAN: stat_batch = the batch the statistics run over (None = n; the global batch under stats_reduce)."""
+        if self.variant == "vae":
+            raise GmError("the VAE has no D step: its train step is vae_grad")
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         lam = self.gp_lambda if gp_lambda is None else float(gp_lambda)
         stat_batch = n if stat_batch is None else int(stat_batch)
@@ -674,6 +710,8 @@ class DcganEngine:
 
     def g_grad(self, n, noise=None, inv_global_batch=None, seed=0, step=0):
         """train_G + backward (src/ns_gan.py:196-216,155): G gradients only."""
+        if self.variant == "vae":
+            raise GmError("the VAE has no G step: its train step is vae_grad")
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         fake, gsv = self.g_forward(n, noise, seed, 2 * step + 1)
         if self.variant == "be":
@@ -686,7 +724,14 @@ class DcganEngine:
         self.g_backward(gsv, dpre)
         return self.loss_buf[1]
 
-    def apply(self, net, hp):
+    def apply(self, net, hp=None):
+        """Adam on G (net 0) or D (net 1) with hp.  The VAE's apply(hp) steps both: its one optimizer over encoder and decoder
+        (src/vae.py:139-142) is elementwise, so an Adam step per net with the same step count is that optimizer exactly."""
+        if self.variant == "vae":
+            hp = net if hp is None else hp
+            self.D.adam(hp)
+            self.G.adam(hp)
+            return
         # BEGAN: both learning rates carry the plateau scale be_state[7]; the reference's two schedulers see the same
         # measure with the same settings (src/be_gan.py:133-136,194-195), so one scale is exact
         (self.G if net == 0 else self.D).adam(hp, self.be_state[7:8] if self.variant == "be" else None)
@@ -734,6 +779,87 @@ class DcganEngine:
         qrows = self._buf("qi_rows", n, self.qp, torch.float32)
         self.d_forward(self.stage_images(images), n, qrows, "qi", net=self.Q, run=self.run_Q)
         return qrows[:, :self.nd].clone(), qrows[:, self.nd:self.nd + self.nc].clone()
+
+    # ------------------------------------------------------------------ VAE (src/vae.py:94-106,193-212)
+    # Forward-only draws of eps (vae_forward without a caller eps): a stream with bit 56 set, which no train step (stream =
+    # step) reaches; vae_reparam_kernel offsets Philox by 64 stream_id, so the stream stays below 2^58
+    VAE_FWD_STREAM = 1 << 56
+
+    def _vae_only(self, what):
+        if self.variant != "vae":
+            raise GmError("%s is the VAE's (variant='vae')" % what)
+
+    def _vae_latent(self, mulv, n, eps, seed, stream_id, kl, tag):
+        """gm_vae_latent_rows on the encoder head's rows mulv [n, mp]: (the decoder's bf16 input rows [n, zp] = [z | 1 | 0],
+        the eps used [n, z] fp32); kl[0] = this process's sum of the KL terms"""
+        zrows = self._buf(tag + "z", n, self.zp)
+        eps_used = self._buf(tag + "eps", n, self.z, torch.float32)
+        if eps is not None:
+            eps = eps.reshape(n, self.z).to(self.device, torch.float32).contiguous()
+        check(self.h, lib().gm_vae_latent_rows(self.h, _ptr(mulv), self.mp, _ptr(eps), _ptr(eps_used), _ptr(zrows), self.zp, n, self.z,
+                                               int(seed), int(stream_id), _ptr(kl), _stream()))
+        return zrows, eps_used
+
+    def sse_sigmoid_rows(self, out, x, n, scale, grad, total):
+        """the VAE's reconstruction term on n NHWC images: total[0] = sum (x - out)^2, grad = 2 scale (out - x) out (1 - out)"""
+        check(self.h, lib().gm_sse_sigmoid_rows(self.h, _ptr(out), _ptr(x), n, 4096 * self.ch, float(scale), _ptr(grad), _ptr(total),
+                                                _stream()))
+
+    def vae_grad(self, img_rows, n, eps=None, seed=0, step=0):
+        """compute_batch + (recon + kl).backward() (src/vae.py:150-161,193-212) for n NHWC image rows (stage_images): the encoder
+        forward with the heads as fp32 rows, z = mu + eps e^(lv/2) (eps [n, z] given, or Philox keyed by (seed, step)), the
+        decoder, recon = sum (x - out)^2 and KL = sum 0.5 (mu^2 + e^lv - lv - 1).  Both losses are sums, so the gradients carry
+        scale 1 and sum exactly over data-parallel ranks.  Writes G.grads (decoder), D.grads (encoder) and vae_loss = (recon,
+        kl), this process's sums."""
+        self._vae_only("vae_grad")
+        z, mp = self.z, self.mp
+        sums = self._buf("vae_sums", 1, 2, torch.float64)[0]
+        mulv = self._buf("vae_mulv", n, mp, torch.float32)
+        sve = self.d_forward(img_rows, n, mulv, "ve")
+        zrows, eps_used = self._vae_latent(mulv, n, eps, seed, step, sums[1:2], "vae_")
+        out, svd = self.g_forward(n, tag="vd", x_rows=zrows)
+        dpre = self._buf("vae_dpre", n * 4096, self.ch)
+        self.sse_sigmoid_rows(out, img_rows, n, 1.0, dpre, sums[0:1])
+        dz = self.g_backward(svd, dpre, need_dx=True, tag="vd", dx_dtype=torch.float32)
+        dml = self._buf("vae_dml", n, mp)
+        check(self.h, lib().gm_vae_dlatent_rows(self.h, _ptr(mulv), mp, _ptr(dz), dz.stride(0), _ptr(eps_used), _ptr(dml), mp, n, z, 1.0,
+                                                _stream()))
+        self.d_backward(sve, dml, self.D.grads, tag="ve")
+        self.vae_loss.copy_(sums)
+        # the step's stored tensors: the head rows, eps, z rows, the reconstruction, dpre, dz, the head upstream, activations
+        self.vae_saved_ = dict(mulv=mulv, eps=eps_used, zrows=zrows, out=out, dpre=dpre, dz=dz, dml=dml, sve=sve, svd=svd, sums=sums)
+        return self.vae_loss
+
+    def vae_forward(self, img_rows, n, eps=None, train=True, seed=0, step=0):
+        """VAE.forward + compute_batch's losses without a backward (src/vae.py:94-98,193-208) for n NHWC image rows: (the
+        reconstruction flat [n, ch*64*64] (NCHW flattened) fp32, mu [n, z], log_var [n, z], losses fp32 [2] = (recon, kl) sums).
+        eps: [n, z] or None for Philox keyed by (seed, VAE_FWD_STREAM + step).  train=False runs every BatchNorm in inference
+        mode (model.eval()); train=True takes batch statistics and updates the running statistics, as torch does."""
+        self._vae_only("vae_forward")
+        sums = self._buf("vaef_sums", 1, 2, torch.float64)[0]
+        mulv = self._buf("vaef_mulv", n, self.mp, torch.float32)
+        self.d_forward(img_rows, n, mulv, "vfe", train=train)
+        zrows, _ = self._vae_latent(mulv, n, eps, seed, self.VAE_FWD_STREAM + int(step), sums[1:2], "vaef_")
+        out, _ = self.g_forward(n, tag="vfd", x_rows=zrows, train=train)
+        dpre = self._buf("vaef_dpre", n * 4096, self.ch)
+        self.sse_sigmoid_rows(out, img_rows, n, 1.0, dpre, sums[0:1])
+        rec = out.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
+        return rec, mulv[:, :self.z].clone(), mulv[:, self.z:2 * self.z].clone(), sums.float()
+
+    def encode(self, images, train=True):
+        """Encoder.forward (src/vae.py:58-61): flat [n, ch*64*64] (NCHW flattened) -> (mu, log_var) fp32 [n, z]"""
+        self._vae_only("encode")
+        n = images.shape[0]
+        mulv = self._buf("vaee_mulv", n, self.mp, torch.float32)
+        self.d_forward(self.stage_images(images), n, mulv, "vee", train=train)
+        return mulv[:, :self.z].clone(), mulv[:, self.z:2 * self.z].clone()
+
+    def decode(self, z, train=True):
+        """Decoder.forward (src/vae.py:74-77): z [n, z] -> images flat [n, ch*64*64] (NCHW flattened) fp32"""
+        self._vae_only("decode")
+        n = z.shape[0]
+        img, _ = self.g_forward(n, z.to(self.device, torch.float32).contiguous(), tag="vdd", train=train)
+        return img.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
 
     # ------------------------------------------------------------------ BEGAN (src/be_gan.py:212-258)
     def began_state(self, values=None):

@@ -395,6 +395,24 @@ int gm_info_noise_rows(gm_ctx* ctx, void* out_dev, int ld, float* codes_dev, int
                        uint64_t stream_id, gm_stream stream);
 int gm_info_loss_rows(gm_ctx* ctx, const float* q_dev, int ldq, const float* codes_dev, int ldc, int zd, int rows, int nd, int nc,
                       float inv_global_batch, void* grad_dev, int ldo, float* loss_dev, gm_stream stream);
+/* The VAE (src/vae.py:94-106,193-212) on the conv path.  gm_sse_sigmoid_rows: on contiguous rows [rows, cols] (cols a multiple
+ * of 8, 16-byte aligned) of the decoder's sigmoid output out_dev and the target x_dev (bf16): sum_dev[0] = sum (x - out)^2
+ * (one double, a fixed-order reduction, for data-parallel ranks to SUM) and grad_dev = 2 scale (out - x) out (1 - out) as
+ * bf16, dL/d(pre-sigmoid output).  gm_vae_latent_rows: on the encoder head's fp32 rows mulv_dev [rows, ldm] ([0, z) mu,
+ * [z, 2z) log_var), z = mu + eps e^(lv/2) with eps from eps_in_dev [rows, z] or Philox keyed by (seed, stream_id) (stream_id
+ * below 2^58), eps_out_dev [rows, z] = the eps used, zrows_dev [rows, ldz] bf16 = [z | 1 | 0 ...] (ldz a multiple of 8 above
+ * z), kl_sum_dev[0] = sum 0.5 (mu^2 + e^lv - lv - 1) (one double, fixed order).  gm_vae_dlatent_rows: from dz_dev [rows,
+ * lddz] fp32 = dL/dz, out_dev [rows, ld] bf16 = scale [mu + dz | 0.5 (e^lv - 1) + 0.5 dz eps e^(lv/2) | 0 ...], the upstream
+ * of the encoder head.  gm_bn_forward_eval: nn.BatchNorm2d in inference mode over NHWC rows, fused with the activation like
+ * gm_bn_forward, with the running statistics running_dev [2][C] (mean, var), which it does not update. */
+int gm_sse_sigmoid_rows(gm_ctx* ctx, const void* out_dev, const void* x_dev, int rows, int cols, float scale, void* grad_dev,
+                        double* sum_dev, gm_stream stream);
+int gm_vae_latent_rows(gm_ctx* ctx, const float* mulv_dev, int ldm, const float* eps_in_dev, float* eps_out_dev, void* zrows_dev, int ldz,
+                       int rows, int z, uint64_t seed, uint64_t stream_id, double* kl_sum_dev, gm_stream stream);
+int gm_vae_dlatent_rows(gm_ctx* ctx, const float* mulv_dev, int ldm, const float* dz_dev, int lddz, const float* eps_dev, void* out_dev,
+                        int ld, int rows, int z, float scale, gm_stream stream);
+int gm_bn_forward_eval(gm_ctx* ctx, const void* x_dev, long long rows, int C, int ld, const float* gamma_dev, const float* beta_dev,
+                       const float* running_dev, float eps, int act, float slope, void* y_dev, int ldy, gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);

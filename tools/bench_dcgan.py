@@ -1,4 +1,5 @@
-"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP, DRAGAN, BEGAN and InfoGAN train steps (D_steps = 1) on one GPU, in one process.
+"""Conv NSGAN, RaNSGAN, Fisher GAN, WGAN-GP, DRAGAN, BEGAN and InfoGAN train steps (D_steps = 1) and the conv VAE step on one
+GPU, in one process.
 
     python tools/bench_dcgan.py [--batch 1024] [--steps 20] [--warmup 5]
 
@@ -9,9 +10,10 @@ all alike.  Prints one JSON line: device name and power limit (read in the same 
 time, images/s, library launches per step, the ratio to NSGAN and achieved TFLOP/s from FLOPs counted from the shapes
 (bench.py's _dcgan_flop_per_img; the penalised critics of WGAN-GP and DRAGAN add one critic forward, one input-gradient
 chain to the image, one tangent forward and one weight-gradient pass = 4 critic forwards; BEGAN's from its autoencoder's
-shapes, began_flop_per_img; InfoGAN's from its G, D and Q shapes, info_flop_per_img).  BEGAN's step includes
-began_control, and InfoGAN's the MI step and MI_optimizer's update (q_grad + apply_mi), as their trainers run them after
-every G update.  Writes nothing but stdout.
+shapes, began_flop_per_img; InfoGAN's from its G, D and Q shapes, info_flop_per_img; the VAE's from its encoder and
+decoder shapes, vae_flop_per_img).  BEGAN's step includes began_control, and InfoGAN's the MI step and MI_optimizer's update
+(q_grad + apply_mi), as their trainers run them after every G update.  The VAE step is vae_grad + apply (one Adam over
+encoder and decoder, lr 1e-3, weight decay 1e-5, src/vae.py:139-142) on the same images.  Writes nothing but stdout.
 """
 import argparse
 import json
@@ -24,8 +26,8 @@ for p in (ROOT, os.path.join(ROOT, "generative-models_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-VARIANTS = ("ns", "ra", "fisher", "wgp", "dra", "be", "info")
-LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4, "be": 1e-4, "info": 2e-4}     # the reference's defaults per variant
+VARIANTS = ("ns", "ra", "fisher", "wgp", "dra", "be", "info", "vae")
+LR = {"ns": 2e-4, "ra": 2e-4, "fisher": 1e-4, "wgp": 1e-4, "dra": 1e-4, "be": 1e-4, "info": 2e-4, "vae": 1e-3}   # the reference's defaults
 
 
 def critic_flop_per_img(hd=64, ch=3):
@@ -62,6 +64,16 @@ def info_flop_per_img(hd=64, z=100, nd=10, nc=10, ch=3):
     return _dcgan_flop_per_img(hd, z + nd + nc, ch) + mi
 
 
+def vae_flop_per_img(hd=64, z=100, ch=3):
+    """algorithmic FLOPs of one VAE step, counted like bench.py's _dcgan_flop_per_img: encoder fwd (the D trunk with the
+    2z-wide head) + decoder fwd (the generator) + decoder bwd (weight grads everywhere, input grads down to z) + encoder bwd
+    (weight grads everywhere, no input gradient into the image)"""
+    gc, dc = [8 * hd, 4 * hd, 2 * hd, hd, ch], [hd, 2 * hd, 4 * hd, 8 * hd]
+    enc = [1024 * dc[0] * 16 * ch, 256 * dc[1] * 16 * dc[0], 64 * dc[2] * 16 * dc[1], 16 * dc[3] * 16 * dc[2], 16 * dc[3] * 2 * z]
+    dec = [z * 16 * gc[0], 16 * gc[0] * 16 * gc[1], 64 * gc[1] * 16 * gc[2], 256 * gc[2] * 16 * gc[3], 1024 * gc[3] * 16 * gc[4]]
+    return 2.0 * sum(enc) + 2.0 * sum(dec) + 2.0 * (2 * sum(dec)) + 2.0 * (2 * sum(enc) - enc[0])
+
+
 def power_limit(index):
     try:
         out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
@@ -85,11 +97,15 @@ def main():
     g = torch.Generator(device="cuda").manual_seed(77)
     pool = (torch.rand(4 * B * 4096, 3, device="cuda", generator=g) < 0.3).to(torch.bfloat16)
     engines = {v: gm_b200.DcganEngine(64, 100, 3, variant=v) for v in VARIANTS}
-    hps = {v: gm_b200.AdamHP.make(LR[v]) for v in VARIANTS}
+    hps = {v: gm_b200.AdamHP.make(LR[v], weight_decay=1e-5 if v == "vae" else 0.0) for v in VARIANTS}
 
     def step(name, s):
         eng, hp = engines[name], hps[name]
         x = pool[(s % 4) * B * 4096:(s % 4 + 1) * B * 4096]
+        if name == "vae":
+            eng.vae_grad(x, B, seed=1000, step=s)              # compute_batch + (recon + kl).backward(), optimizer.step()
+            eng.apply(hp)
+            return
         eng.d_grad(x, B, seed=1000, step=s)
         eng.apply(1, hp)
         eng.g_grad(B, seed=1000, step=s)
@@ -129,11 +145,14 @@ def main():
             flop = began_flop_per_img()
         elif name == "info":
             flop = info_flop_per_img()
+        elif name == "vae":
+            flop = vae_flop_per_img()
         else:
             flop = _dcgan_flop_per_img() + (4 * critic_flop_per_img() if name in ("wgp", "dra") else 0.0)
         out[name] = {"median_ms": round(med, 3), "min_ms": round(min(ms[name]), 3), "images_per_s": round(B / med * 1e3, 1),
                      "launches_per_step": launches[name], "gflop_per_image": round(flop / 1e9, 3),
-                     "tflops": round(flop * B / med / 1e9, 1), "last_losses": [float(v) for v in engines[name].loss_buf.tolist()]}
+                     "tflops": round(flop * B / med / 1e9, 1),
+                     "last_losses": [float(v) for v in (engines[name].vae_loss if name == "vae" else engines[name].loss_buf).tolist()]}
     for name in VARIANTS[1:]:
         out[name]["over_ns_images_per_s"] = round(out[name]["images_per_s"] / out["ns"]["images_per_s"], 3)
     print(json.dumps(out))
