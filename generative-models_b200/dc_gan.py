@@ -22,6 +22,7 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
+from gm_b200.dcgan import DevicePool
 from gm_b200.gan_api import to_cuda, _FusedLoss
 
 
@@ -122,6 +123,9 @@ def pull_running_stats(eng, nets):
 class EngineSync:
     """Parameter sync between a trainer's DcganEngine (self._engine) and its model's modules (self._nets(): (state_dict
     prefix, module) pairs); self._dirty marks module parameters newer than the engine's"""
+    # device_dataset: keep train_iter's images in HBM as 8-bit codes (gm_b200.dcgan.DevicePool) and draw each train() batch on
+    # the device, when the loader is eligible.  Off by default: train() then fetches every batch through the host loader.
+    device_dataset = False
 
     def _sd(self):
         return module_params(self._nets())
@@ -140,6 +144,14 @@ class EngineSync:
                 for k, v in mod.named_parameters():
                     v.copy_(tw["%s.%s" % (tag, k)].to(v.device))
         pull_running_stats(self._engine, self._nets())
+
+    def _device_pool(self):
+        """train_iter's images as a DevicePool when device_dataset is on and the loader is eligible (kept for later train()
+        calls), else None: the batches then come from the host loader"""
+        if not self.device_dataset:
+            return None
+        self._pool = DevicePool.from_loader(self.train_iter, self.model.channels, getattr(self, "_pool", None))
+        return self._pool
 
     def _fused_loss(self, mods, loss_val):
         """loss_val as a 0-dim loss whose backward() puts the engine's current gradients of the (tag, module) pairs `mods`
@@ -204,17 +216,22 @@ class DCGANTrainer(EngineSync):
         eng.stats_reduce = par.sum_gradients if world > 1 else None
         self._pre_train(eng)
         seed = par.rank_seed(self._seed, rank)
+        pool = self._device_pool()
         epoch_steps = int(np.ceil(len(self.train_iter) / D_steps))
         for epoch in range(1, num_epochs + 1):
             self.model.train()
             ring = torch.zeros(D_steps + 1, epoch_steps, device="cuda")
             for i in range(epoch_steps):
                 for k in range(D_steps):
-                    images = self.process_batch(self.train_iter)
-                    n = images.shape[0]
+                    if pool is not None:                            # the first batch of a freshly shuffled loader, on the device
+                        n = min(pool.batch_size, pool.n)
+                        rows = eng.stage_pool(pool, n, seed ^ DevicePool.SEED_MIX, self._step * D_steps + k)
+                    else:
+                        images = self.process_batch(self.train_iter)
+                        n = images.shape[0]
+                        rows = eng.stage_images(images)
                     inv = par.inv_global_batch(n, world)
-                    ring[k, i] = eng.d_grad(eng.stage_images(images), n, inv_global_batch=inv, seed=seed, step=self._step * D_steps + k,
-                                            stat_batch=n * world)
+                    ring[k, i] = eng.d_grad(rows, n, inv_global_batch=inv, seed=seed, step=self._step * D_steps + k, stat_batch=n * world)
                     par.sum_gradients(eng.D.grads)                  # NCCL SUM of the flat D gradient (no-op on one GPU)
                     eng.apply(1, hpD)
                 ring[D_steps, i] = eng.g_grad(n, inv_global_batch=inv, seed=seed, step=self._step)

@@ -33,6 +33,7 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
+from gm_b200.dcgan import DevicePool
 from gm_b200.gan_api import to_cuda
 from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats
 
@@ -242,13 +243,12 @@ class DCVAETrainer(EngineSync):
                 dist.broadcast(net.params, src=0)
                 net.refresh()
         seed = par.rank_seed(self._seed, rank)
+        pool = self._device_pool()
         for epoch in range(1, num_epochs + 1):
             self.model.train()
             per_step = []
-            for batch in self.train_iter:
-                images = self._images(batch)
-                n = images.shape[0]
-                per_step.append(eng.vae_grad(eng.stage_images(images), n, seed=seed, step=self._step).clone())
+            for rows, n in (self._pool_batches(eng, pool, seed) if pool is not None else self._host_batches(eng)):
+                per_step.append(eng.vae_grad(rows, n, seed=seed, step=self._step).clone())
                 par.sum_gradients(eng.G.grads)                      # NCCL SUM (no-op on one GPU): the losses are sums
                 par.sum_gradients(eng.D.grads)
                 eng.apply(hp)
@@ -270,6 +270,20 @@ class DCVAETrainer(EngineSync):
             if self.viz:
                 self.sample_images(epoch)
         self._pull()
+
+    def _host_batches(self, eng):
+        """one epoch of train_iter: (NHWC bf16 rows, n) per batch"""
+        for batch in self.train_iter:
+            images = self._images(batch)
+            yield eng.stage_images(images), images.shape[0]
+
+    def _pool_batches(self, eng, pool, seed):
+        """one epoch drawn on the device from the DevicePool: batch k stages rows [kB, min((k+1)B, N)) of this epoch's
+        permutation (round = the epochs trained so far), so every image is used once per epoch, as by a shuffling loader"""
+        B = pool.batch_size
+        for k in range(len(self.train_iter)):
+            n = min(B, pool.n - k * B)
+            yield eng.stage_pool(pool, n, seed ^ DevicePool.SEED_MIX, self.num_epochs, offset=k * B), n
 
     def _images(self, batch):
         images, _ = batch

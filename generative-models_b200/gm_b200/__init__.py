@@ -9,5 +9,5 @@ from .engine import GanEngine, InfoGanEngine, VaeEngine  # noqa: F401
 
 HAS_SPLIT_PRECISION = True       # fp32-grade split-bf16 operand mode (gm_prec GM_PREC_SPLIT)
 from .graph import GraphedGanStep, graphed_gan_step  # noqa: E402,F401
-from .dcgan import DcganEngine  # noqa: E402,F401
+from .dcgan import DcganEngine, DevicePool  # noqa: E402,F401
 from .ae import AeEngine  # noqa: E402,F401

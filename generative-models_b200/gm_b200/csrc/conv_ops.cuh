@@ -846,4 +846,51 @@ __global__ void __launch_bounds__(256) lrelu_mask_rows_kernel(const __nv_bfloat1
   }
 }
 
+// ---------------------------------------------------------------- device-resident dataset pool (DESIGN.md §6b)
+// The pool keeps each image as row_vals one-byte codes in NHWC order, and a 256-entry table of bf16 bit patterns maps a
+// code to the value stage_images would write.  Batch row r reads pool row sampler_index(smp, smp.offset + r) (kernels.cuh:
+// Sampler) and becomes bf16 NHWC row r of out [rows, row_vals].  One block walks one row: each thread issues its 16-byte
+// code loads (16 values each) before it looks them up in the shared table and writes two 16-byte stores per load; the
+// next row's pool index is computed while this row is in flight.  row_vals % 16 == 0 and 16-byte aligned rows (host checks).
+constexpr int kPoolThreads = 256, kPoolUnroll = 4;
+__global__ void __launch_bounds__(kPoolThreads) stage_pool_rows_kernel(const uint8_t* __restrict__ codes, int row_vals,
+                                                                       const uint16_t* __restrict__ table, const Sampler smp, int rows,
+                                                                       __nv_bfloat16* __restrict__ out, int* __restrict__ idx_out) {
+  __shared__ uint16_t lut[256];
+  griddep_sync();
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = table[i];
+  __syncthreads();
+  const int groups = row_vals >> 4;
+  unsigned int src_next = blockIdx.x < rows ? sampler_index(smp, smp.offset + blockIdx.x) : 0u;
+  for (int r = blockIdx.x; r < rows; r += gridDim.x) {
+    const unsigned int src = src_next;
+    if (r + gridDim.x < rows) src_next = sampler_index(smp, smp.offset + (unsigned long long)(r + gridDim.x));
+    if (idx_out && threadIdx.x == 0) idx_out[r] = int(src);
+    const uint4* crow = reinterpret_cast<const uint4*>(codes + size_t(src) * row_vals);
+    uint4* orow = reinterpret_cast<uint4*>(out + size_t(r) * row_vals);
+    for (int g0 = threadIdx.x; g0 < groups; g0 += kPoolThreads * kPoolUnroll) {
+      uint4 v[kPoolUnroll];
+#pragma unroll
+      for (int u = 0; u < kPoolUnroll; ++u) {
+        const int g = g0 + u * kPoolThreads;
+        v[u] = g < groups ? __ldg(crow + g) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < kPoolUnroll; ++u) {
+        const int g = g0 + u * kPoolThreads;
+        if (g >= groups) break;
+        const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+        uint32_t o[8];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {      // byte j of a word is value 4q + j; bf16 pairs pack the lower-addressed value low
+          o[2 * q] = uint32_t(lut[w[q] & 0xFFu]) | (uint32_t(lut[(w[q] >> 8) & 0xFFu]) << 16);
+          o[2 * q + 1] = uint32_t(lut[(w[q] >> 16) & 0xFFu]) | (uint32_t(lut[w[q] >> 24]) << 16);
+        }
+        orow[2 * g] = make_uint4(o[0], o[1], o[2], o[3]);
+        orow[2 * g + 1] = make_uint4(o[4], o[5], o[6], o[7]);
+      }
+    }
+  }
+}
+
 }  // namespace gm

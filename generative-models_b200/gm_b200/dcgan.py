@@ -132,6 +132,88 @@ class _Net:
         self.refresh()
 
 
+class DevicePool:
+    """A training set held in HBM as one byte per value, batches drawn on the device (DESIGN.md §6b).
+
+    Image datasets hold few distinct values (k/255 from ToTensor, {0, 1} when binarised, (k/255 - 0.5)/0.5 normalised), and
+    every value reaches the kernels as bf16.  So a dataset with at most 256 distinct bf16 bit patterns is stored as codes
+    [n, 4096 ch] uint8 in NHWC order plus table [256], the bf16 bit patterns as int16: table[codes] is what stage_images makes
+    of the images, bit for bit (-0.0 and +0.0 are distinct patterns).  DcganEngine.stage_pool turns rows of the on-device
+    Feistel permutation (kernels.cuh: Sampler) into a batch; indices_host evaluates the same permutation on the host."""
+    SEED_MIX = 0x5DEECE66D       # sampler seed = the trainer's Philox seed ^ SEED_MIX: the two streams are keyed apart
+
+    def __init__(self, codes, table, channels, batch_size, drop_last, source):
+        self.codes, self.table, self.ch = codes, table, channels
+        self.n, self.row_vals = codes.shape
+        self.batch_size, self.drop_last, self._source = batch_size, drop_last, source
+        self.num_batches = self.n // batch_size if drop_last else -(-self.n // batch_size)
+
+    def __len__(self):
+        return self.num_batches
+
+    @staticmethod
+    def pack(images, channels, device=None, chunk_rows=4096):
+        """images [n, ch*64*64] (NCHW flattened) or [n, ch, 64, 64] -> (codes [n, 4096 ch] uint8 NHWC, table [256] int16),
+        or None when the bf16 values hold more than 256 distinct bit patterns.  The values become bf16 as process_batch +
+        stage_images make them (.float(), then bf16).  Runs chunk by chunk on `device` (default: the images' own)."""
+        n = images.shape[0]
+        dev = images.device if device is None else torch.device(device)
+
+        def bits(i):                                   # the chunk's bf16 bit patterns in NHWC order, int32
+            c = images[i:i + chunk_rows].to(dev, non_blocking=True).float().reshape(-1, channels, 64, 64)
+            return c.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous().view(torch.int16).to(torch.int32).reshape(c.shape[0], -1)
+
+        uniq = torch.empty(0, dtype=torch.int32, device=dev)
+        for i in range(0, n, chunk_rows):
+            uniq = torch.unique(torch.cat([uniq, torch.unique(bits(i))]))
+            if uniq.numel() > 256:
+                return None
+        codes = torch.empty(n, 4096 * channels, dtype=torch.uint8, device=dev)
+        for i in range(0, n, chunk_rows):
+            codes[i:i + chunk_rows] = torch.searchsorted(uniq, bits(i)).to(torch.uint8)
+        table = torch.zeros(256, dtype=torch.int16, device=dev)
+        table[:uniq.numel()] = uniq.to(torch.int16)
+        return codes, table
+
+    @staticmethod
+    def from_loader(loader, channels, cached=None, budget=None):
+        """A pool of loader's images, or None when the loader is not eligible (the caller then keeps the host path): a
+        DataLoader over a TensorDataset whose first tensor holds 64*64*channels values per row, drawn by a RandomSampler
+        without replacement over the whole dataset, with at most 256 distinct bf16 values and codes within `budget` bytes
+        (default: half the free device memory).  `cached`, the pool of an earlier train() call, is returned while the loader
+        serves the same tensor with the same batch size and drop_last."""
+        from torch.utils.data import DataLoader, RandomSampler, TensorDataset
+        if not isinstance(loader, DataLoader) or not isinstance(loader.dataset, TensorDataset) or loader.batch_size is None:
+            return None
+        smp = loader.sampler
+        if type(smp) is not RandomSampler or smp.replacement or smp._num_samples is not None:
+            return None
+        images = loader.dataset.tensors[0]
+        n = images.shape[0]
+        if n == 0 or n > 0x7FFFFFFF or images.numel() != n * 4096 * channels:
+            return None
+        if cached is not None and cached._source is images and cached.batch_size == loader.batch_size and \
+                cached.drop_last == loader.drop_last and cached.ch == channels:
+            return cached
+        if budget is None:
+            budget = torch.cuda.mem_get_info()[0] // 2
+        if n * 4096 * channels > budget:
+            return None
+        dev = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else images.device
+        packed = DevicePool.pack(images, channels, dev)
+        if packed is None:
+            return None
+        return DevicePool(packed[0], packed[1], channels, loader.batch_size, loader.drop_last, images)
+
+    def indices_host(self, seed, round, offset, count):
+        """the pool rows perm_{seed,round}(offset + r), r < count, that gm_stage_pool_rows draws (int64 CPU tensor)"""
+        out = (C.c_int * count)()
+        rc = lib().gm_sampler_indices_host(self.n, int(seed), int(round), int(offset), int(count), out)
+        if rc != 0:
+            raise GmError("gm_sampler_indices_host: bad argument (rc=%d)" % rc)
+        return torch.tensor(list(out), dtype=torch.int64)
+
+
 class DcganEngine:
     """One DCGAN (64x64xchannels images) on one GPU; see the module docstring."""
 
@@ -519,6 +601,17 @@ class DcganEngine:
         n = images.shape[0]
         x = images.view(n, self.ch, 64, 64).permute(0, 2, 3, 1).to(torch.bfloat16).contiguous()
         return x.view(n * 4096, self.ch)
+
+    def stage_pool(self, pool, n, seed, round, offset=0, idx_out=None):
+        """n images of a DevicePool drawn on the device -> NHWC bf16 rows [n*4096, ch] (a reused buffer), the rows stage_images
+        makes of pool images perm_{seed,round}(offset + r), r < n (gm_stage_pool_rows).  idx_out: int32 [>= n] device tensor
+        that receives the drawn pool indices."""
+        if pool.ch != self.ch:
+            raise GmError("the pool holds %d-channel images; this engine takes %d channels" % (pool.ch, self.ch))
+        x = self._buf("pool_x", n * 4096, self.ch)
+        check(self.h, lib().gm_stage_pool_rows(self.h, _ptr(pool.codes), pool.n, pool.row_vals, _ptr(pool.table), int(seed), int(round),
+                                               int(offset), int(n), _ptr(x), _ptr(idx_out), _stream()))
+        return x
 
     # the per-row loss each variant's rows share: WGAN-GP's are W's and DRAGAN's NS's (the penalty is separate); the G steps of
     # RaNS and Fisher are NS's and W's -mean(D(G(z))) (src/ra_gan.py, src/fisher_gan.py train_G); InfoGAN's D and G steps

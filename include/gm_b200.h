@@ -323,6 +323,14 @@ int gm_pack_col0(gm_ctx* ctx, const float* v_dev, int rows, void* out_dev, int l
 /* process_batch (src/ns_gan.py:222-226, src/ae.py:150-151) as a standalone step: images -> bf16 rows [rows, ld], ones column at x */
 int gm_stage_images(gm_ctx* ctx, const void* images_dev, int img_fmt, const int* gather_idx_dev, void* out_dev, int rows, int x, int ld,
                     gm_stream stream);
+/* A batch drawn from a device-resident dataset of 8-bit codes (gm_b200.dcgan.DevicePool): codes_dev [n_pool, row_vals] uint8
+ * (one image per row, NHWC order, row_vals a multiple of 16, 16-byte aligned) and table_bf16_dev [256] bf16 bit patterns.
+ * Batch row r reads pool row perm_{seed,round}(offset + r), the permutation of gm_sampler_indices_host, and out_bf16_dev
+ * [rows, row_vals] (16-byte aligned) receives table[code] for each of its values - the NHWC bf16 rows stage_images makes of
+ * that image.  idx_out_dev (nullable) receives the rows' pool indices.  GM_ERR_ARG, with nothing launched, unless
+ * 0 < rows <= n_pool <= 2^31 - 1 and offset + rows <= n_pool. */
+int gm_stage_pool_rows(gm_ctx* ctx, const uint8_t* codes_dev, long long n_pool, int row_vals, const uint16_t* table_bf16_dev, uint64_t seed,
+                       uint64_t round, uint64_t offset, int rows, void* out_bf16_dev, int* idx_out_dev, gm_stream stream);
 /* generator noise rows as a bf16 GEMM operand: Philox N(0,1) (noise_dev NULL) or a caller tensor [rows, z] fp32 */
 int gm_noise_rows(gm_ctx* ctx, const float* noise_dev, void* out_dev, int rows, int z, int ld, uint64_t seed, uint64_t stream_id,
                   gm_stream stream);
