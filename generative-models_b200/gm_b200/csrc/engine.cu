@@ -179,6 +179,8 @@ static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
   cfg.numAttrs = na;
   GemmParams prm = pl.p;
   prm.tma_store = pl.tmc_state == 1 ? 1 : 0;
+  // fp32 rows take float4 stores only where every row of every split starts on 16 bytes (ldc = 30: row 1 is at byte 120)
+  prm.f32_vec = prm.epi == EPI_F32 && !(reinterpret_cast<uintptr_t>(prm.part) & 15) && prm.ldp % 4 == 0 && prm.part_stride % 4 == 0;
   return cudaLaunchKernelEx(&cfg, kern, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2, prm);
 }
 
@@ -341,11 +343,14 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
   return GM_OK;
 }
 
-__global__ void reduce_partials_kernel(const float* __restrict__ part, int nsplit, long long stride, long long n,
-                                       float* __restrict__ out) {
+// out[r * ld + c] = sum over splits of part[split * stride + r * ld + c] for the logical [rows, cols] block only: columns
+// [cols, ld) belong to the caller and are left as they are (no split writes them, so their partials are stale scratch)
+__global__ void reduce_partials_kernel(const float* __restrict__ part, int nsplit, long long stride, long long rows, int cols,
+                                       int ld, float* __restrict__ out) {
   griddep_sync();
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= rows * cols) return;
+  const long long i = cols == ld ? k : (k / cols) * ld + k % cols;
   float t = 0.f;
   for (int s0 = 0; s0 < nsplit; s0 += 8) {     // eight partials in flight, summed in split order
     float a[8];
@@ -467,7 +472,32 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
   GemmPlan pl;
   const bool f32 = d->out_kind == 1;
   const int ncover = f32 ? d->N : (d->out_cols > d->N ? d->out_cols : d->N);
-  if (!f32 && (d->N % 16)) return fail(c, GM_ERR_ARG, "bf16 output needs N %% 16 == 0 (N=%d)", d->N);
+  // every descriptor the kernels cannot run as written is refused here, before anything is launched
+  auto misaligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) != 0; };
+  if (d->out_kind != 0 && d->out_kind != 1) return fail(c, GM_ERR_ARG, "gemm: out_kind %d is not 0 (bf16) or 1 (fp32)", d->out_kind);
+  if (d->mode != 0 && d->mode != 1) return fail(c, GM_ERR_ARG, "gemm: mode %d is not 0 (NT) or 1 (TN)", d->mode);
+  if (d->mode == 1 && !f32) return fail(c, GM_ERR_ARG, "gemm: a TN (mode 1) product has an fp32 output only");
+  if (d->act < ACT_NONE || d->act > ACT_LRELU) return fail(c, GM_ERR_ARG, "gemm: act %d is outside 0..3", d->act);
+  if (d->aux_mode < AUX_NONE || d->aux_mode > AUX_VAE_OUT) return fail(c, GM_ERR_ARG, "gemm: aux_mode %d is outside 0..3", d->aux_mode);
+  if ((d->aux_mode != AUX_NONE) != (d->aux_dev != nullptr)) return fail(c, GM_ERR_ARG, "gemm: aux_dev needs a nonzero aux_mode and the reverse");
+  if (!d->C_dev || misaligned(d->C_dev)) return fail(c, GM_ERR_ARG, "gemm: C_dev must be a 16-byte aligned pointer");
+  if (misaligned(d->aux_dev) || misaligned(d->bias_dev) || misaligned(d->dot_w_dev))
+    return fail(c, GM_ERR_ARG, "gemm: aux_dev, bias_dev and dot_w_dev must be 16-byte aligned");
+  if (f32) {
+    if (d->pad_one || d->bias_dev || d->act != ACT_NONE || d->aux_dev || d->dot_w_dev || d->dot_out_dev || (d->out_cols != 0 && d->out_cols != d->N))
+      return fail(c, GM_ERR_ARG, "gemm: an fp32 output takes no epilogue (out_cols, pad_one, bias, act, aux, dot)");
+    const int row_len = d->transpose ? d->M : d->N;
+    if (d->ldc < row_len) return fail(c, GM_ERR_ARG, "gemm: fp32 ldc %d is below the stored row length %d", d->ldc, row_len);
+  } else {
+    if (d->N % 16) return fail(c, GM_ERR_ARG, "bf16 output needs N %% 16 == 0 (N=%d)", d->N);
+    if (d->transpose) return fail(c, GM_ERR_ARG, "gemm: transpose applies to an fp32 output only");
+    if (ncover % 8 || d->ldc % 8 || d->ldc < ncover)
+      return fail(c, GM_ERR_ARG, "gemm: bf16 output needs out_cols %% 8 == 0, ldc %% 8 == 0 and ldc >= out_cols (out_cols=%d ldc=%d)", ncover, d->ldc);
+    if (d->aux_dev && (d->ld_aux % 8 || d->ld_aux < ncover))
+      return fail(c, GM_ERR_ARG, "gemm: aux needs ld_aux %% 8 == 0 and ld_aux >= out_cols (ld_aux=%d out_cols=%d)", d->ld_aux, ncover);
+    if (d->dot_w_dev && !d->dot_out_dev) return fail(c, GM_ERR_ARG, "gemm: dot_w_dev needs dot_out_dev");
+    if (d->dot_out_dev && d->dot_ld < d->M) return fail(c, GM_ERR_ARG, "gemm: dot_ld %d is below M %d", d->dot_ld, d->M);
+  }
   int rc = plan_gemm(c, &pl, d->mode, d->M, d->N, d->K, d->A_dev, d->lda, d->B_dev, d->ldb, ncover, f32 ? 64 : 1);
   if (rc) return rc;
   GemmParams& p = pl.p;
@@ -483,7 +513,7 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
     p.act_slope = d->act_slope;
     p.aux = static_cast<const __nv_bfloat16*>(d->aux_dev);
     p.ld_aux = d->ld_aux;
-    p.aux_mode = d->aux_dev ? d->aux_mode : AUX_NONE;
+    p.aux_mode = d->aux_mode;
     p.dot_w = d->dot_w_dev;
     p.dot_out = d->dot_out_dev;
     p.dot_ld = d->dot_ld;
@@ -510,8 +540,10 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
   p.part_stride = per;
   rc = launch_plan(c, pl, s);
   if (rc) return rc;
-  launch_pdl("reduce_partials_kernel", reduce_partials_kernel, unsigned((per + 255) / 256), 256, 0, s, c->scratch, p.splits, per, per,
-                                                                     static_cast<float*>(d->C_dev));
+  const long long rows = d->transpose ? d->N : d->M;
+  const int cols = d->transpose ? d->M : d->N;
+  launch_pdl("reduce_partials_kernel", reduce_partials_kernel, unsigned((rows * cols + 255) / 256), 256, 0, s, c->scratch, p.splits, per,
+             rows, cols, d->ldc, static_cast<float*>(d->C_dev));
   c->launches++;
   CU_OK(c, cudaGetLastError());
   return GM_OK;

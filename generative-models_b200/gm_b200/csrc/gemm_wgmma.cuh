@@ -83,6 +83,7 @@ struct GemmParams {
   long long part_stride;
   int ldp;
   int transpose;
+  int f32_vec;          // set at launch: every row of every split starts on 16 bytes, so 16 columns leave as 4 float4
   // optional phase timing (tools/time_phases.py): CTA 0 writes SM-clock stamps, see the kernel
   long long* dbg;
   // ---- split-bf16 operands (SPLIT kernels, gm_prec GM_PREC_SPLIT): A = A_hi + A_lo, B = B_hi + B_lo as bf16 planes
@@ -670,7 +671,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
                 for (int j = 0; j < 16; ++j)
                   if (col0 + j < p.N) base[size_t(col0 + j) * p.ldp + row] = v[j];
-              } else if (col0 + 16 <= p.N) {
+              } else if (p.f32_vec && col0 + 16 <= p.N) {
                 float4* o = reinterpret_cast<float4*>(base + size_t(row) * p.ldp + col0);
 #pragma unroll
                 for (int k4 = 0; k4 < 4; ++k4) o[k4] = make_float4(v[4 * k4], v[4 * k4 + 1], v[4 * k4 + 2], v[4 * k4 + 3]);

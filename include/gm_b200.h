@@ -77,12 +77,26 @@ int gm_ctx_num_sms(const gm_ctx* ctx);
  *   mode 1 "TN": A_dev [K, lda] (M contiguous), B_dev [K, ldb] (N contiguous);
  *                (contraction over batch rows: dW = X^T dY; any K)
  * out_kind 0: bf16 C_dev [M, ldc] with optional bias[N], act (0 none, 1 relu,
- *             2 sigmoid), aux (bf16 [M, ld_aux]; aux_mode 1: *= aux(1-aux),
- *             2: *= (aux > 0)); columns [N, out_cols) are written as padding
- *             (col N = 1 if pad_one).  dot_w/dot_out: optional fused row-dot,
- *             dot_out holds 2*ceil(out_cols/208) partial slots of dot_ld floats.
+ *             2 sigmoid, 3 LeakyReLU(act_slope)), aux (bf16 [M, ld_aux];
+ *             aux_mode 1: *= aux(1-aux), 2: *= (aux > 0), 3: v = sigmoid
+ *             output, aux = target x: stores -2 (x - v) v (1 - v) and adds
+ *             sum (x - v)^2 over the row's columns < N to its dot_out slots);
+ *             columns [N, out_cols) are written as padding (col N = 1 if
+ *             pad_one).  dot_w/dot_out: optional fused row-dot of the stored
+ *             values; dot_out holds 2*ceil(out_cols/BN) partial slots of dot_ld
+ *             floats (BN = 64 if out_cols <= 64, else 208) whose sum is the row's
+ *             value.  Rows >= M and columns [out_cols, ldc) are not written.
  * out_kind 1: fp32 C_dev (ldc floats; transposed store if transpose), split-K
- *             partials summed by the library into C_dev. */
+ *             partials summed by the library into C_dev.  Only the logical
+ *             block ([M, N], or [N, M] transposed) is written.
+ * Refused with GM_ERR_ARG before any launch: mode outside 0..1; mode 1 with a
+ * bf16 output; act outside 0..3 or aux_mode outside 0..3; aux_mode without
+ * aux_dev or the reverse; an fp32 output with any epilogue field (out_cols
+ * other than 0 or N, pad_one, bias, act, aux, dot_w, dot_out); transpose on a
+ * bf16 output; a bf16 output with N % 16, out_cols % 8, ldc % 8 or ld_aux % 8
+ * not 0, ldc < out_cols or ld_aux < out_cols; an fp32 ldc below the stored
+ * row length (N, or M transposed); C_dev, aux_dev, bias_dev or dot_w_dev not
+ * 16-byte aligned; dot_w_dev without dot_out_dev; dot_ld < M. */
 typedef struct {
   int mode, M, N, K;
   const void* A_dev; int lda;

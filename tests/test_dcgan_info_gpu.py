@@ -184,52 +184,54 @@ def test_g_and_mi_backward_match_float64_at_the_device_forward_points():
     and for the MI step (Q's backward from the MI rows' gradient, with weight gradients, down to the image, sigmoid', G's
     backward), restated in float64 with torch.nn.grad at the device's OWN stored activations, masks and BatchNorm inputs
     (the BEGAN test's restatement of the two stacks).  Both sides then differentiate the same function, so what remains is
-    the bf16 rounding of the device's backward tensors."""
+    the bf16 rounding of the device's backward tensors.  (z, nd, nc) = (20, 7, 3) gives G 30 input columns, so G's l1
+    weight gradient is an fp32 output whose rows start 120 bytes apart (not on 16 bytes)."""
     from test_dcgan_began_gpu import _at, _stack_backward, _trunk_backward, _tw
-    n, nd, nc = 8, 10, 10
-    eng, _, _, _, g = _engine()
-    tw = _tw(eng)
-    w = {tag: {k[2:]: v for k, v in tw.items() if k.startswith(tag + ".")} for tag in "GDQ"}
-    rep = {}
-    # G step: the body of DcganEngine.g_grad, keeping its saved tensors
-    fake, gsv = eng.g_forward(n, _noise(n, 100, nd, nc, g).cuda())
-    logits = torch.zeros(16, n, device="cuda")
-    sf = eng.d_forward(fake, n, logits, "df")
-    ds = torch.zeros(n, device="cuda")
-    eng._loss_rows(logits, n, 1, 1.0 / n, ds, C.c_void_p(eng.loss_buf.data_ptr() + 4))
-    dpre = eng.d_backward(sf, ds, None, need_wgrad=False, need_dimg=True, tag="df")
-    eng.g_backward(gsv, dpre)
-    dy = ds.to(torch.bfloat16).double().cpu().view(n, 1)                  # the bf16 column d_backward packs
-    _, T = _trunk_backward(eng, sf, dy, w["D"], "")
-    f = _at(fake, 64, CH)
-    rep["Gstep_dpre"] = nrel(_at(dpre, 64, CH), T * f * (1 - f))
-    gref, _ = _stack_backward(eng, gsv, T * f * (1 - f), w["G"], "")
-    tg = eng.torch_grads()
-    for name, r in gref.items():
-        rep["Gstep_G." + name] = nrel(tg["G." + name], r)
-    # MI step
-    eng.q_grad(n, noise=_noise(n, 100, nd, nc, g).cuda())
-    s = eng.q_saved_
-    qref, T = _trunk_backward(eng, s["qsv"], s["dq"][:, :nd + nc].double().cpu(), w["Q"], "")
-    f = _at(s["fake"], 64, CH)
-    rep["MI_dpre"] = nrel(_at(s["dpre"], 64, CH), T * f * (1 - f))
-    gref, _ = _stack_backward(eng, s["gsv"], T * f * (1 - f), w["G"], "")
-    tg = eng.torch_grads()
-    for name, r in qref.items():
-        rep["MI_Q." + name] = nrel(tg["Q." + name], r)
-    for name, r in gref.items():
-        rep["MI_G." + name] = nrel(tg["G." + name], r)
-    # Q.l1's weight gradient sums 8 x 1024 output positions of an upstream whose signs alternate, so the bf16 rounding of
-    # that upstream (which the chain above does not model) reads larger there than anywhere else; from the device's own
-    # stored upstream the same GEMM agrees to fp32 accumulation
-    from torch.nn.grad import conv2d_weight
-    d0 = _at(eng._bufs["qdprev1"][:n * 1024], 32, eng.dc[0])
-    rep["MI_Q.l1.weight_from_stored_upstream"] = nrel(tg["Q.l1.weight"], conv2d_weight(_at(s["fake"], 64, CH), w["Q"]["l1.weight"].shape, d0, 2, 1))
-    _REPORT.add("float64_at_device_points", rep)
-    assert len([k for k in rep if k.startswith("MI_Q.")]) == 12 and len([k for k in rep if k.startswith("MI_G.")]) == 13
-    assert rep["MI_Q.l1.weight_from_stored_upstream"] < 1e-4, rep
-    for k, v in rep.items():
-        assert v < (0.04 if k == "MI_Q.l1.weight" else 0.02), (k, v, rep)
+    n = 8
+    for z, nd, nc in ((100, 10, 10), (20, 7, 3)):
+        eng, _, _, _, g = _engine(z=z, nd=nd, nc=nc)
+        tw = _tw(eng)
+        w = {tag: {k[2:]: v for k, v in tw.items() if k.startswith(tag + ".")} for tag in "GDQ"}
+        rep = {}
+        # G step: the body of DcganEngine.g_grad, keeping its saved tensors
+        fake, gsv = eng.g_forward(n, _noise(n, z, nd, nc, g).cuda())
+        logits = torch.zeros(16, n, device="cuda")
+        sf = eng.d_forward(fake, n, logits, "df")
+        ds = torch.zeros(n, device="cuda")
+        eng._loss_rows(logits, n, 1, 1.0 / n, ds, C.c_void_p(eng.loss_buf.data_ptr() + 4))
+        dpre = eng.d_backward(sf, ds, None, need_wgrad=False, need_dimg=True, tag="df")
+        eng.g_backward(gsv, dpre)
+        dy = ds.to(torch.bfloat16).double().cpu().view(n, 1)                  # the bf16 column d_backward packs
+        _, T = _trunk_backward(eng, sf, dy, w["D"], "")
+        f = _at(fake, 64, CH)
+        rep["Gstep_dpre"] = nrel(_at(dpre, 64, CH), T * f * (1 - f))
+        gref, _ = _stack_backward(eng, gsv, T * f * (1 - f), w["G"], "")
+        tg = eng.torch_grads()
+        for name, r in gref.items():
+            rep["Gstep_G." + name] = nrel(tg["G." + name], r)
+        # MI step
+        eng.q_grad(n, noise=_noise(n, z, nd, nc, g).cuda())
+        s = eng.q_saved_
+        qref, T = _trunk_backward(eng, s["qsv"], s["dq"][:, :nd + nc].double().cpu(), w["Q"], "")
+        f = _at(s["fake"], 64, CH)
+        rep["MI_dpre"] = nrel(_at(s["dpre"], 64, CH), T * f * (1 - f))
+        gref, _ = _stack_backward(eng, s["gsv"], T * f * (1 - f), w["G"], "")
+        tg = eng.torch_grads()
+        for name, r in qref.items():
+            rep["MI_Q." + name] = nrel(tg["Q." + name], r)
+        for name, r in gref.items():
+            rep["MI_G." + name] = nrel(tg["G." + name], r)
+        # Q.l1's weight gradient sums 8 x 1024 output positions of an upstream whose signs alternate, so the bf16 rounding of
+        # that upstream (which the chain above does not model) reads larger there than anywhere else; from the device's own
+        # stored upstream the same GEMM agrees to fp32 accumulation
+        from torch.nn.grad import conv2d_weight
+        d0 = _at(eng._bufs["qdprev1"][:n * 1024], 32, eng.dc[0])
+        rep["MI_Q.l1.weight_from_stored_upstream"] = nrel(tg["Q.l1.weight"], conv2d_weight(_at(s["fake"], 64, CH), w["Q"]["l1.weight"].shape, d0, 2, 1))
+        _REPORT.add("float64_at_device_points" + ("" if z == 100 else "_z%d_nd%d_nc%d" % (z, nd, nc)), rep)
+        assert len([k for k in rep if k.startswith("MI_Q.")]) == 12 and len([k for k in rep if k.startswith("MI_G.")]) == 13
+        assert rep["MI_Q.l1.weight_from_stored_upstream"] < 1e-4, rep
+        for k, v in rep.items():
+            assert v < (0.04 if k == "MI_Q.l1.weight" else 0.02), (k, v, rep)
 
 
 def test_apply_mi_keeps_its_own_g_moments():
