@@ -22,7 +22,7 @@ import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step
 from dc_gan import Generator, DCGAN, DCGANTrainer
 
 
@@ -78,6 +78,7 @@ class DCBEGAN(DCGAN):
 class DCBEGANTrainer(DCGANTrainer):
     """ Object to hold data iterators, train the conv BEGAN (surface of src/be_gan.py:93-337) """
     variant = "be"
+    _custom_step_limit = "BEGAN's discriminator is an autoencoder, and custom losses are built for one score per image"
 
     def train(self, num_epochs, G_lr=1e-4, D_lr=1e-4, D_steps=1, GAMMA=0.50, LAMBDA=1e-3, K=0.00):
         """ Trainer.train (src/be_gan.py:109-205): DCGANTrainer's loop; after each G update K, the convergence measure and
@@ -108,6 +109,7 @@ class DCBEGANTrainer(DCGANTrainer):
                     bn.running_mean.copy_(runs[i - 1][0].cpu())
                     bn.running_var.copy_(runs[i - 1][1].cpu())
 
+    @builtin_step
     def train_D(self, images, K):
         """ Run 1 step of training for D (src/be_gan.py:212-238): returns (D_loss, DX_loss, DG_loss); .backward() on D_loss
         delivers the gradients """

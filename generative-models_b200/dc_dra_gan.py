@@ -19,7 +19,7 @@ import torch.nn as nn  # noqa: F401
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step
 from dc_gan import Generator, DCGAN, DCGANTrainer  # noqa: F401
 from dc_w_gp_gan import Discriminator as _Critic
 
@@ -46,6 +46,7 @@ class DCDRAGANTrainer(DCGANTrainer):
         """ Trainer.train (src/dra_gan.py:94-172) with LAMBDA = 10, K = 1, C = 1 and delta, u drawn on the device per rank """
         super().train(num_epochs, G_lr=G_lr, D_lr=D_lr, D_steps=D_steps)
 
+    @builtin_step
     def train_D(self, images, LAMBDA=10, K=1, C=1):
         """ Run 1 step of training for D (src/dra_gan.py:174-225): returns D_loss; .backward() delivers the gradients """
         images = to_cuda(images)

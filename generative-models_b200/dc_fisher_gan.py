@@ -17,7 +17,7 @@ import torch.nn as nn  # noqa: F401
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step
 from dc_gan import Generator, Discriminator, DCGAN, DCGANTrainer  # noqa: F401
 
 
@@ -41,6 +41,7 @@ class DCFisherGANTrainer(DCGANTrainer):
     def _pre_train(self, eng):
         eng.fisher_state(0.0, self._rho)                                # src/fisher_gan.py:117-118
 
+    @builtin_step
     def train_D(self, images):
         """ Run 1 step of training for D (src/fisher_gan.py:193-229): returns (D_loss, IPM_ratio); .backward() on D_loss
         delivers the gradients.  LAMBDA moves on the device in the same step.  IPM_ratio is the reference's logging

@@ -14,6 +14,10 @@ in the sm_90a kernels behind gm_b200.DcganEngine (im2col / col2im + wgmma GEMMs,
 nn.Conv2d / nn.ConvTranspose2d / nn.BatchNorm2d members only hold the parameters in torch's layouts, so state_dict()
 has the usual DCGAN keys and shapes.  Under torchrun the trainer is data-parallel: per-rank batches and noise, NCCL
 all-reduce (SUM) of the flat G and D gradients before each Adam step.
+
+A subclass may override train_D / train_G with its own torch loss, as the reference's README invites (README.md:31):
+under grad mode model.G / model.D are autograd nodes whose forward and backward are the same kernels, and train() then
+runs the reference's loop (src/ns_gan.py:107-156) on one process with Adam over the module parameters (FusedAdam).
 """
 import numpy as np
 import torch
@@ -23,7 +27,64 @@ from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
-from gm_b200.gan_api import to_cuda, _FusedLoss
+from gm_b200.gan_api import to_cuda, _FusedLoss, FusedAdam, builtin_step, reference_loop
+from torch.autograd.function import once_differentiable
+
+
+def _first_order(backward):
+    """a create_graph=True backward through a conv node raises here, before the kernels run, instead of returning
+    gradients that a second differentiation would see as constants"""
+    def wrapper(ctx, *grads):
+        if torch.is_grad_enabled():
+            raise RuntimeError("the conv Generator / Discriminator nodes have no double backward (create_graph=True)")
+        return backward(ctx, *grads)
+    return wrapper
+
+
+def _grads_for(grads, tag, mod, names):
+    """the node's gradients {"<tag>.<name>": tensor} in the order of names, on the module's parameters' device"""
+    params = dict(mod.named_parameters())
+    return [grads["%s.%s" % (tag, k)].contiguous().to(params[k].device) for k in names]
+
+
+class _DcGForward(torch.autograd.Function):
+    """Generator.forward under grad mode: G(z) and its backward on the conv kernels (DcganEngine.custom_g_forward /
+    custom_g_backward); autograd routes dL/dG(z) in and the parameter gradients out"""
+
+    @staticmethod
+    def forward(ctx, noise, eng, mod, names, *params):
+        out, ctx.handle = eng.custom_g_forward(noise)
+        ctx.eng, ctx.mod, ctx.names = eng, mod, names
+        return out
+
+    @staticmethod
+    @_first_order
+    @once_differentiable        # the backward is a kernel chain: create_graph=True gets an error, not a missing term
+    def backward(ctx, dimages):
+        grads = ctx.eng.custom_g_backward(ctx.handle, dimages.float().contiguous())
+        return (None, None, None, None, *_grads_for(grads, "G", ctx.mod, ctx.names))
+
+
+class _DcDForward(torch.autograd.Function):
+    """Discriminator.forward under grad mode: D(x) and its backward, with dL/dx when x requires grad (D(G(z)))"""
+
+    @staticmethod
+    def forward(ctx, x, eng, mod, names, *params):
+        scores, ctx.handle = eng.custom_d_forward(x)
+        ctx.eng, ctx.mod, ctx.names = eng, mod, names
+        return scores
+
+    @staticmethod
+    @_first_order
+    @once_differentiable
+    def backward(ctx, dscore):
+        grads, dx = ctx.eng.custom_d_backward(ctx.handle, dscore.float(), ctx.needs_input_grad[0])
+        return (dx, None, None, None, *_grads_for(grads, "D", ctx.mod, ctx.names))
+
+
+def _node_args(mod):
+    names, params = zip(*mod.named_parameters())
+    return (mod, names) + params
 
 
 class Generator(nn.Module):
@@ -44,7 +105,10 @@ class Generator(nn.Module):
         tr = self._owner
         if tr is None:
             raise GmError("Generator is not attached to a CUDA engine yet: construct the DCGANTrainer first")
-        return tr._engine_synced().generate(to_cuda(x).float())
+        eng = tr._engine_synced()
+        if torch.is_grad_enabled() and eng.supports_custom_loss:
+            return _DcGForward.apply(to_cuda(x).float(), eng, *_node_args(self))
+        return eng.generate(to_cuda(x).float())
 
 
 class Discriminator(nn.Module):
@@ -73,7 +137,10 @@ class Discriminator(nn.Module):
         tr = self._owner
         if tr is None:
             raise GmError("Discriminator is not attached to a CUDA engine yet: construct its trainer first")
-        return tr._engine_synced().discriminate(to_cuda(x).float().reshape(x.shape[0], -1))
+        eng = tr._engine_synced()
+        if torch.is_grad_enabled() and eng.supports_custom_loss:
+            return _DcDForward.apply(to_cuda(x).float().reshape(x.shape[0], -1), eng, *_node_args(self))
+        return eng.discriminate(to_cuda(x).float().reshape(x.shape[0], -1))
 
 
 class DCGAN(nn.Module):
@@ -201,8 +268,11 @@ class DCGANTrainer(EngineSync):
 
     # ------------------------------------------------------------------ reference surface
     def train(self, num_epochs, G_lr=2e-4, D_lr=2e-4, D_steps=1):
-        """ Trainer.train (src/ns_gan.py:94-170): same loop and logging on the fused conv step """
+        """ Trainer.train (src/ns_gan.py:94-170): same loop and logging on the fused conv step, or on the overriding
+        train_D / train_G (_train_custom) """
         import torch.distributed as dist
+        if self._has_custom_step():
+            return self._train_custom(num_epochs, G_lr, D_lr, D_steps)
         eng = self._engine_synced()
         hpG, hpD = AdamHP.make(G_lr), AdamHP.make(D_lr)
         for net in (eng.G, eng.D):                                  # fresh optimizers per train() call (src/ns_gan.py:107-110)
@@ -246,6 +316,32 @@ class DCGANTrainer(EngineSync):
             self.num_epochs += 1
         self._pull()
 
+    # a trainer whose losses need more than one score per image from D (BEGAN's autoencoder) or more than G and D (InfoGAN's
+    # coded input and Q) names what is missing here: an override of its steps is refused, not silently ignored
+    _custom_step_limit = None
+
+    def _has_custom_step(self):
+        """True when a subclass overrides train_D / train_G (/ train_Q) with a method not marked @builtin_step"""
+        steps = [getattr(type(self), m) for m in ("train_D", "train_G", "train_Q") if hasattr(type(self), m)]
+        return not all(getattr(f, "_gm_builtin", False) for f in steps)
+
+    def _train_custom(self, num_epochs, G_lr, D_lr, D_steps):
+        """The reference loop over the overriding train_D / train_G: their torch losses run model.G / model.D as autograd
+        nodes over the conv kernels; Adam (FusedAdam) steps the module parameters, which the next forward loads"""
+        if self._custom_step_limit is not None:
+            raise GmError("%s: an overridden train_D / train_G is not supported: %s" % (type(self).__name__, self._custom_step_limit))
+        if par.world_size() > 1:
+            raise GmError("an overridden train_D / train_G trains on one process; data-parallel training runs the built-in steps")
+        eng = self._engine_synced()
+        self.model.to(eng.device)                   # the reference's to_cuda(model) (src/ns_gan.py:81): Adam runs on the device
+
+        def after_step():
+            self._dirty = True                      # the module parameters are newer than the engine's
+        G_optimizer = FusedAdam(self.model.G.parameters(), lr=G_lr)
+        D_optimizer = FusedAdam(self.model.D.parameters(), lr=D_lr)
+        reference_loop(self, num_epochs, G_optimizer, D_optimizer, D_steps, after_step)
+        pull_running_stats(eng, self._nets())
+
     def _epoch_line(self, eng, epoch, num_epochs, G_losses, D_losses):
         return "Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses))
 
@@ -259,6 +355,7 @@ class DCGANTrainer(EngineSync):
     def _loss(self, net, loss_val):
         return self._fused_loss([("G", self.model.G)] if net == 0 else [("D", self.model.D)], loss_val)
 
+    @builtin_step
     def train_D(self, images):
         """ Run 1 step of training for discriminator (src/ns_gan.py:172-194): returns D_loss; .backward() delivers the gradients """
         images = to_cuda(images)
@@ -268,6 +365,7 @@ class DCGANTrainer(EngineSync):
         loss = eng.d_grad(eng.stage_images(images.reshape(n, -1).float()), n, noise=noise.float().contiguous())
         return self._loss(1, loss.clone())
 
+    @builtin_step
     def train_G(self, images):
         """ Run 1 step of training for generator (src/ns_gan.py:196-216) """
         eng = self._engine_synced()

@@ -22,7 +22,7 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError
 from gm_b200 import parallel as par
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step
 from dc_gan import DCGAN, DCGANTrainer, dcgan_init
 
 
@@ -64,6 +64,7 @@ class DCInfoGAN(DCGAN):
 class DCInfoGANTrainer(DCGANTrainer):
     """ Object to hold data iterators, train the conv InfoGAN (surface of src/info_gan.py:112-395) """
     variant = "info"
+    _custom_step_limit = "InfoGAN's coded generator input and Q network have no per-call autograd nodes"
 
     def __init__(self, model, train_iter, val_iter, test_iter, viz=False):
         super().__init__(model, train_iter, val_iter, test_iter, viz)
@@ -108,6 +109,7 @@ class DCInfoGANTrainer(DCGANTrainer):
         m = self.model
         return self.compute_noise(n, m.z_dim, m.disc_dim, m.cont_dim).float().contiguous()
 
+    @builtin_step
     def train_D(self, images):
         """ Run 1 step of training for discriminator (src/info_gan.py:223-246): returns D_loss; .backward() delivers the
         gradients """
@@ -117,6 +119,7 @@ class DCInfoGANTrainer(DCGANTrainer):
         loss = eng.d_grad(eng.stage_images(images.reshape(n, -1).float()), n, noise=self._noise(n))
         return self._loss(1, loss.clone())
 
+    @builtin_step
     def train_G(self, images):
         """ Run 1 step of training for generator (src/info_gan.py:248-267) """
         eng = self._engine_synced()
@@ -124,6 +127,7 @@ class DCInfoGANTrainer(DCGANTrainer):
         loss = eng.g_grad(n, noise=self._noise(n))
         return self._loss(0, loss.clone())
 
+    @builtin_step
     def train_Q(self, images, LAMBDA=1):
         """ Run 1 step of training for the auxiliary network (src/info_gan.py:269-304): returns MI_loss; .backward()
         delivers the gradients to G's and Q's parameters """

@@ -17,7 +17,7 @@ import torch
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step
 import dc_gan
 from dc_gan import Generator, DCGAN, DCGANTrainer  # noqa: F401
 
@@ -46,6 +46,7 @@ class DCWGPGANTrainer(DCGANTrainer):
         """ Trainer.train (src/w_gp_gan.py:96-175) with LAMBDA = 10 and eps drawn on the device per rank """
         super().train(num_epochs, G_lr=G_lr, D_lr=D_lr, D_steps=D_steps)
 
+    @builtin_step
     def train_D(self, images, LAMBDA=10):
         """ Run 1 step of training for the critic (src/w_gp_gan.py:177-220): returns D_loss; .backward() delivers the gradients """
         images = to_cuda(images)

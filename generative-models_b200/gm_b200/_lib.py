@@ -135,6 +135,8 @@ def lib():
     L.gm_pack_col0.argtypes = [vp, vp, i, vp, i, vp]
     L.gm_stage_images.argtypes = [vp, vp, i, vp, vp, i, i, i, vp]
     L.gm_stage_pool_rows.argtypes = [vp, vp, ll, i, vp, u64, u64, u64, i, vp, vp, vp]
+    L.gm_image_to_rows.argtypes = [vp, vp, vp, i, i, vp, vp]
+    L.gm_rows_to_image.argtypes = [vp, vp, i, i, vp, vp]
     L.gm_noise_rows.argtypes = [vp, vp, vp, i, i, i, u64, u64, vp]
     L.gm_loss_rows.argtypes = [vp, i, i, vp, i, i, f, vp, vp, vp, vp]
     L.gm_gp_interp_rows.argtypes = [vp, vp, i, vp, i, i, i, i, vp, vp, u64, u64, vp, i, vp]

@@ -893,4 +893,77 @@ __global__ void __launch_bounds__(kPoolThreads) stage_pool_rows_kernel(const uin
   }
 }
 
+// ---------------------------------------------------------------- the image layout at the autograd boundary
+// The drop-in classes see images as NCHW-flattened fp32 [n, ch*64*64]; the kernels take NHWC bf16 rows [n*4096, ch].  One
+// block converts kLayoutPix pixels of one image: the ch planes go through a shared tile [ch][kLayoutPix] so that both
+// sides move 16 bytes per access (float4 per plane, 8 bf16 of the interleaved rows).  ch <= 4, 16-byte aligned pointers
+// (host checks).
+constexpr int kLayoutPix = 1024, kLayoutThreads = 256, kLayoutTiles = 4096 / kLayoutPix;
+
+// dst = bf16_rn(x), or bf16_rn((x * f) * (1 - f)) with f = aux (NHWC bf16, the generator's stored sigmoid output): the
+// upstream of the pre-sigmoid output from dL/dG(z), rounded once, in the order torch evaluates g * f * (1 - f)
+__global__ void __launch_bounds__(kLayoutThreads) image_to_rows_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ aux,
+                                                                       int ch, __nv_bfloat16* __restrict__ dst) {
+  __shared__ float tile[4 * kLayoutPix];
+  griddep_sync();
+  const int b = blockIdx.x / kLayoutTiles, p0 = (blockIdx.x % kLayoutTiles) * kLayoutPix;
+  for (int i = threadIdx.x; i < ch * (kLayoutPix / 4); i += kLayoutThreads) {
+    const int c = i / (kLayoutPix / 4), q = i % (kLayoutPix / 4);
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x + (size_t(b) * ch + c) * 4096 + p0) + q);
+    *reinterpret_cast<float4*>(tile + c * kLayoutPix + 4 * q) = v;
+  }
+  __syncthreads();
+  const size_t base = (size_t(b) * 4096 + p0) * ch;
+  for (int k = threadIdx.x; k < kLayoutPix * ch / 8; k += kLayoutThreads) {
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int e = 8 * k + j, p = e / ch;
+      f[j] = tile[(e - p * ch) * kLayoutPix + p];
+    }
+    if (aux) {
+      const uint4 a = __ldg(reinterpret_cast<const uint4*>(aux + base) + k);
+      const __nv_bfloat162* s = reinterpret_cast<const __nv_bfloat162*>(&a);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 sf = __bfloat1622float2(s[j]);
+        f[2 * j] = __fmul_rn(__fmul_rn(f[2 * j], sf.x), __fsub_rn(1.f, sf.x));
+        f[2 * j + 1] = __fmul_rn(__fmul_rn(f[2 * j + 1], sf.y), __fsub_rn(1.f, sf.y));
+      }
+    }
+    uint4 o;
+    uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);     // .x (the lower address) = f[2j]
+      ow[j] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    reinterpret_cast<uint4*>(dst + base)[k] = o;
+  }
+}
+
+// dst = float(src): NHWC bf16 rows -> NCHW-flattened fp32, exact
+__global__ void __launch_bounds__(kLayoutThreads) rows_to_image_kernel(const __nv_bfloat16* __restrict__ src, int ch, float* __restrict__ dst) {
+  __shared__ float tile[4 * kLayoutPix];
+  griddep_sync();
+  const int b = blockIdx.x / kLayoutTiles, p0 = (blockIdx.x % kLayoutTiles) * kLayoutPix;
+  const size_t base = (size_t(b) * 4096 + p0) * ch;
+  for (int k = threadIdx.x; k < kLayoutPix * ch / 8; k += kLayoutThreads) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(src + base) + k);
+    const __nv_bfloat162* s = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 sf = __bfloat1622float2(s[j]);
+      const int e = 8 * k + 2 * j, p = e / ch, q = (e + 1) / ch;
+      tile[(e - p * ch) * kLayoutPix + p] = sf.x;
+      tile[(e + 1 - q * ch) * kLayoutPix + q] = sf.y;
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < ch * (kLayoutPix / 4); i += kLayoutThreads) {
+    const int c = i / (kLayoutPix / 4), q = i % (kLayoutPix / 4);
+    reinterpret_cast<float4*>(dst + (size_t(b) * ch + c) * 4096 + p0)[q] = *reinterpret_cast<const float4*>(tile + c * kLayoutPix + 4 * q);
+  }
+}
+
 }  // namespace gm

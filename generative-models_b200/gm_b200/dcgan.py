@@ -328,6 +328,8 @@ class DcganEngine:
             self.began_init(0.0, 1)
         self.vae_loss = torch.zeros(2, device=self.device)       # VAE: (recon, kl) of the last vae_grad, this process's sums
         self._bufs = {}
+        self._calls = {"d": 0, "g": 0}                           # custom_d_forward / custom_g_forward calls so far
+        self._slot_gen = {"d": [0] * self.D_SLOTS, "g": [0] * self.G_SLOTS}   # the call that holds each slot
         self.init_weights()
 
     # ------------------------------------------------------------------ parameters
@@ -364,15 +366,19 @@ class DcganEngine:
             self.Q.view("l5.weight")[self.nd + self.nc:].zero_()
 
     def _torch_views(self, which):
-        """{torch-style name: view of the G / D tensor in torch's layout} over the flat params (which="params") or grads.
+        """{torch-style name: view of the G / D tensor in torch's layout} over the flat params (which="params"), grads
+        (which="grads") or, for which = {"G" / "D" / "Q": flat buffer in that net's layout}, over those buffers only.
         Conv weights are [Cout, (kh, kw, ci)] here and [Cout, Cin, kh, kw] in torch; transposed-conv weights (G, BEGAN's
         decoder) are [(kh, kw, co), Cin] here and [Cin, Cout, kh, kw] in torch; BatchNorm vectors match.  Padded weights are
         trimmed on torch's dim 0 (_trim: D.l5 keeps output channel 0 of its 16 rows, BEGAN's encoder l5 / decoder l1 the e
         embedding channels, InfoGAN's Q.l5 its nd + nc code outputs)."""
         out = {}
         for tag, net in zip("GDQ", self.nets()):
+            flat = which.get(tag) if isinstance(which, dict) else getattr(net, which)
+            if flat is None:
+                continue
             for n in net.names:
-                w = net.view(n, getattr(net, which))
+                w = net.view(n, flat)
                 key = "%s.%s" % (tag, n)
                 if n.split(".")[-2].startswith("l"):
                     if tag == "G" or n.startswith("decoder."):
@@ -541,7 +547,7 @@ class DcganEngine:
             if need_wgrad:
                 for i in range(4):
                     gemm_bf16(betas[i], sv["col%d" % i], D.view("l%d.weight" % (i + 1), grads), "tn")
-            return self._dimg(sv, betas[0], tag) if need_dimg else None
+            return self._dimg(sv, betas[0], tag, dimg_mode) if need_dimg else None
         dflat = self._buf(tag + "dflat", n, 16 * dc[3])
         gemm_bf16(dy5, D.bf_t[pfx + "l5.weight"], dflat, "nt", K=dy5.shape[1])
         d, hw = dflat.view(n * 16, dc[3]), 4
@@ -595,12 +601,33 @@ class DcganEngine:
         return betas
 
     # ------------------------------------------------------------------ the train step (src/ns_gan.py:126-156)
+    def _image_arg(self, images):
+        """images [n, ch*64*64] or [n, ch, 64, 64] -> fp32 [n, ch*64*64] on the device, contiguous and 16-byte aligned"""
+        n = images.shape[0]
+        if images.numel() != n * 4096 * self.ch:
+            raise GmError("expected %d-channel 64x64 images, got shape %s" % (self.ch, tuple(images.shape)))
+        x = images.to(self.device).reshape(n, -1).float().contiguous()
+        return x if x.data_ptr() % 16 == 0 else x.clone()
+
+    def image_to_rows(self, images, out_rows=None, dst=None):
+        """images (see _image_arg) -> NHWC bf16 rows [n*4096, ch] (gm_image_to_rows): x rounded to bf16, or with out_rows
+        (G's stored sigmoid output rows) x * f * (1 - f) rounded once.  dst: the rows to write (default a new tensor)."""
+        x = self._image_arg(images)
+        n = x.shape[0]
+        dst = torch.empty(n * 4096, self.ch, device=self.device, dtype=torch.bfloat16) if dst is None else dst
+        check(self.h, lib().gm_image_to_rows(self.h, _ptr(x), _ptr(out_rows), n, self.ch, _ptr(dst), _stream()))
+        return dst
+
+    def rows_to_image(self, rows, n):
+        """NHWC bf16 rows of n images -> fp32 [n, ch*64*64] (NCHW flattened), exact (gm_rows_to_image)"""
+        out = torch.empty(n, 4096 * self.ch, device=self.device)
+        check(self.h, lib().gm_rows_to_image(self.h, _ptr(rows), n, self.ch, _ptr(out), _stream()))
+        return out
+
     def stage_images(self, images):
         """[n, ch*64*64] flat (the reference's process_batch layout: NCHW flattened, src/ns_gan.py:225) or
         [n, ch, 64, 64] -> NHWC bf16 rows [n*4096, ch]."""
-        n = images.shape[0]
-        x = images.view(n, self.ch, 64, 64).permute(0, 2, 3, 1).to(torch.bfloat16).contiguous()
-        return x.view(n * 4096, self.ch)
+        return self.image_to_rows(images)
 
     def stage_pool(self, pool, n, seed, round, offset=0, idx_out=None):
         """n images of a DevicePool drawn on the device -> NHWC bf16 rows [n*4096, ch] (a reused buffer), the rows stage_images
@@ -936,7 +963,7 @@ class DcganEngine:
         out, _ = self.g_forward(n, tag="vfd", x_rows=zrows, train=train)
         dpre = self._buf("vaef_dpre", n * 4096, self.ch)
         self.sse_sigmoid_rows(out, img_rows, n, 1.0, dpre, sums[0:1])
-        rec = out.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
+        rec = self.rows_to_image(out, n)
         return rec, mulv[:, :self.z].clone(), mulv[:, self.z:2 * self.z].clone(), sums.float()
 
     def encode(self, images, train=True):
@@ -952,7 +979,7 @@ class DcganEngine:
         self._vae_only("decode")
         n = z.shape[0]
         img, _ = self.g_forward(n, z.to(self.device, torch.float32).contiguous(), tag="vdd", train=train)
-        return img.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
+        return self.rows_to_image(img, n)
 
     # ------------------------------------------------------------------ BEGAN (src/be_gan.py:212-258)
     def began_state(self, values=None):
@@ -1041,16 +1068,93 @@ class DcganEngine:
         """BEGAN's D(images): flat [n, ch*64*64] (NCHW flattened) -> the reconstructions in the same layout (fp32)"""
         n = images.shape[0]
         rec, _, _ = self.autoencode(self.stage_images(images), n, "ber")
-        return rec.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
+        return self.rows_to_image(rec, n)
 
     def generate(self, noise):
         n = noise.shape[0]
         img, _ = self.g_forward(n, noise.float().contiguous(), tag="gen")
-        return img.view(n, 64, 64, self.ch).permute(0, 3, 1, 2).float().reshape(n, -1)
+        return self.rows_to_image(img, n)
 
     def discriminate(self, images):
         n = images.shape[0]
         logits = self._buf("logits_i", 16, n, torch.float32)
         self.d_forward(self.stage_images(images), n, logits, "di")
-        s = logits[0, :n].view(n, 1)
+        return self._out_act(logits[0, :n].view(n, 1))
+
+    def _out_act(self, s):
         return torch.sigmoid(s) if self.d_out_act == "sigmoid" else (torch.relu(s) if self.d_out_act == "relu" else s.clone())
+
+    # ------------------------------------------------------------------ per-call forward / backward (user-written losses)
+    # A user's train_D / train_G (README.md:31) calls model.D / model.G as its loss needs and back-propagates through the
+    # drop-ins' autograd nodes (dc_gan._DcDForward / _DcGForward).  Each call keeps its saved activations in a slot of a ring,
+    # D_SLOTS discriminator and G_SLOTS generator calls, allocated on first use; a backward whose slot a later call has taken
+    # raises instead of reading that call's tensors.  The losses that need these are the ones whose D returns one score per
+    # image; BEGAN's autoencoder D, InfoGAN's coded input and Q and the VAE have none.
+    D_SLOTS, G_SLOTS = 4, 2
+
+    @property
+    def supports_custom_loss(self):
+        return self.variant not in ("be", "info", "vae")
+
+    def _take_slot(self, kind):
+        if not self.supports_custom_loss:
+            raise GmError("per-call forwards with a backward are built for the discriminators with one score per image "
+                          "(not %s)" % self.variant)
+        gens = self._slot_gen[kind]
+        self._calls[kind] += 1
+        slot = (self._calls[kind] - 1) % len(gens)
+        gens[slot] = self._calls[kind]
+        return dict(kind=kind, slot=slot, gen=self._calls[kind])
+
+    def _check_live(self, handle, what):
+        if self._slot_gen[handle["kind"]][handle["slot"]] != handle["gen"]:
+            raise RuntimeError("%s activations were overwritten: at most %d %s.forward results can await their backward"
+                               % (what, len(self._slot_gen[handle["kind"]]), what))
+
+    def custom_d_forward(self, images):
+        """D(images) in training mode (batch statistics; the running statistics move per call, as nn.BatchNorm2d.train()):
+        images [n, ch*64*64] (NCHW flattened) -> (scores [n, 1] fp32 = out_act(logits), the handle for custom_d_backward:
+        slot, generation, saved activations sv)"""
+        x = self._image_arg(images)
+        n = x.shape[0]
+        h = self._take_slot("d")
+        tag = "cd%d" % h["slot"]
+        rows = self.image_to_rows(x, dst=self._buf(tag + "x", n * 4096, self.ch))
+        logits = self._buf(tag + "logits", 16, n, torch.float32)
+        h.update(n=n, sv=self.d_forward(rows, n, logits, tag), s=logits[0, :n])
+        return self._out_act(h["s"].view(n, 1)), h
+
+    def custom_d_backward(self, handle, dscore, need_dx):
+        """dscore [n] = dL/d(score) of custom_d_forward's call -> ({"D.<name>": weight / BatchNorm gradient in torch's layout},
+        dL/d(images) [n, ch*64*64] fp32 or None).  dL/dlogit = dscore act'(s) is formed on the n logits."""
+        self._check_live(handle, "Discriminator")
+        n, s = handle["n"], handle["s"]
+        d = dscore.reshape(n).to(self.device, torch.float32)
+        if self.d_out_act == "sigmoid":
+            p = torch.sigmoid(s)
+            d = d * (p * (1 - p))
+        elif self.d_out_act == "relu":
+            d = d * (s > 0).float()
+        grads = torch.zeros(self.D.total, device=self.device)   # d_backward writes, never adds: one buffer per call
+        dimg = self.d_backward(handle["sv"], d.contiguous(), grads, need_dimg=need_dx, tag="cdb", dimg_mode=C2I_NONE)
+        return self._torch_views({"D": grads}), (self.rows_to_image(dimg, n) if need_dx else None)
+
+    def custom_g_forward(self, noise):
+        """G(noise) in training mode: noise [n, z] -> (images [n, ch*64*64] fp32, NCHW flattened; the handle for
+        custom_g_backward)"""
+        n = noise.shape[0]
+        z = noise.to(self.device, torch.float32).reshape(n, self.zin).contiguous()
+        h = self._take_slot("g")
+        img, sv = self.g_forward(n, z, tag="cg%d" % h["slot"])
+        h.update(n=n, sv=sv)
+        return self.rows_to_image(img, n), h
+
+    def custom_g_backward(self, handle, dimages):
+        """dimages [n, ch*64*64] = dL/dG(z) of custom_g_forward's call -> {"G.<name>": gradient in torch's layout}.  The
+        upstream of the pre-sigmoid output, dimages G(z) (1 - G(z)), is rounded to bf16 once (gm_image_to_rows)."""
+        self._check_live(handle, "Generator")
+        sv, n = handle["sv"], handle["n"]
+        dpre = self.image_to_rows(dimages, sv["img"], self._buf("cgdpre", n * 4096, self.ch))
+        grads = torch.zeros(self.G.total, device=self.device)
+        self.g_backward(sv, dpre, grads=grads)
+        return self._torch_views({"G": grads})

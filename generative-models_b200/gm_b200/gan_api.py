@@ -259,6 +259,43 @@ class FusedAdam(torch.optim.Optimizer):
                 _lib.adam_step(p.data, p.grad.contiguous(), st["exp_avg"], st["exp_avg_sq"], hp, st["step"])
 
 
+def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step=None):
+    """The reference's loop verbatim (src/ns_gan.py:107-156) for a Trainer tr whose train_D / train_G were overridden: the
+    override's torch loss drives the CUDA forward / backward kernels through model.G / model.D and their autograd nodes.
+    after_step(), when given, runs after every optimizer step (the conv trainers mark their modules' parameters as newer
+    than their engine's)."""
+    epoch_steps = int(np.ceil(len(tr.train_iter) / D_steps))
+    for epoch in range(1, num_epochs + 1):
+        tr.model.train()
+        G_losses, D_losses = [], []
+        for _ in range(epoch_steps):
+            D_step_loss = []
+            for _ in range(D_steps):
+                images = tr.process_batch(tr.train_iter)
+                D_optimizer.zero_grad()
+                D_loss = tr.train_D(images)
+                D_loss.backward()
+                D_optimizer.step()
+                if after_step is not None:
+                    after_step()
+                D_step_loss.append(D_loss.detach())
+            D_losses.append(torch.stack(D_step_loss).mean())
+            G_optimizer.zero_grad()
+            G_loss = tr.train_G(images)
+            G_losses.append(G_loss.detach())
+            G_loss.backward()
+            G_optimizer.step()
+            if after_step is not None:
+                after_step()
+        G_losses, D_losses = torch.stack(G_losses).tolist(), torch.stack(D_losses).tolist()
+        tr.Glosses.extend(G_losses)
+        tr.Dlosses.extend(D_losses)
+        print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
+        tr.num_epochs += 1
+        if tr.viz:
+            tr.generate_images(epoch)
+
+
 class _FusedLoss(torch.autograd.Function):
     """0-dim loss whose backward() hands the gradients the fused kernels already
     computed to the parameters' .grad (the reference calls loss.backward() then
@@ -528,39 +565,12 @@ class GANTrainerBase:
         return not (getattr(type(self).train_D, "_gm_builtin", False) and getattr(type(self).train_G, "_gm_builtin", False))
 
     def _train_reference_loop(self, num_epochs, G_lr, D_lr, D_steps, clip):
-        """The reference's loop verbatim (src/ns_gan.py:107-156) for Trainers whose train_D /
-        train_G were overridden: the override's torch loss drives the CUDA forward / backward
-        kernels through Generator.forward / Discriminator.forward and their autograd nodes."""
+        """reference_loop for Trainers whose train_D / train_G were overridden"""
         bs = getattr(self.train_iter, "batch_size", None) or next(iter(self.train_iter))[0].shape[0]
         self._ensure_engine(bs)
         G_optimizer = FusedAdam(self.model.G.parameters(), lr=G_lr)
         D_optimizer = FusedAdam(self.model.D.parameters(), lr=D_lr, clamp=clip)
-        epoch_steps = int(np.ceil(len(self.train_iter) / D_steps))
-        for epoch in range(1, num_epochs + 1):
-            self.model.train()
-            G_losses, D_losses = [], []
-            for _ in range(epoch_steps):
-                D_step_loss = []
-                for _ in range(D_steps):
-                    images = self.process_batch(self.train_iter)
-                    D_optimizer.zero_grad()
-                    D_loss = self.train_D(images)
-                    D_loss.backward()
-                    D_optimizer.step()
-                    D_step_loss.append(D_loss.detach())
-                D_losses.append(torch.stack(D_step_loss).mean())
-                G_optimizer.zero_grad()
-                G_loss = self.train_G(images)
-                G_losses.append(G_loss.detach())
-                G_loss.backward()
-                G_optimizer.step()
-            G_losses, D_losses = torch.stack(G_losses).tolist(), torch.stack(D_losses).tolist()
-            self.Glosses.extend(G_losses)
-            self.Dlosses.extend(D_losses)
-            print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
-            self.num_epochs += 1
-            if self.viz:
-                self.generate_images(epoch)
+        reference_loop(self, num_epochs, G_optimizer, D_optimizer, D_steps)
 
     def _pre_train(self, num_epochs, hpG, hpD, D_steps, extra):
         # fresh optimizers each train() call, like src/ns_gan.py:107-110; parameters may have

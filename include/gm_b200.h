@@ -345,6 +345,15 @@ int gm_stage_images(gm_ctx* ctx, const void* images_dev, int img_fmt, const int*
  * 0 < rows <= n_pool <= 2^31 - 1 and offset + rows <= n_pool. */
 int gm_stage_pool_rows(gm_ctx* ctx, const uint8_t* codes_dev, long long n_pool, int row_vals, const uint16_t* table_bf16_dev, uint64_t seed,
                        uint64_t round, uint64_t offset, int rows, void* out_bf16_dev, int* idx_out_dev, gm_stream stream);
+/* The image layout at the autograd boundary of the conv drop-ins (Generator / Discriminator forward and backward):
+ * NCHW-flattened fp32 [n, ch*64*64], as the reference's process_batch flattens images (src/ns_gan.py:222-226), and the
+ * kernels' NHWC bf16 rows [n*4096, ch].  gm_image_to_rows writes dst = x rounded to nearest even (tensor.to(bfloat16)),
+ * or, with out_nhwc_dev (the generator's stored sigmoid output f), (x * f) * (1 - f) rounded once: the upstream of the
+ * pre-sigmoid output from dL/dG(z).  gm_rows_to_image widens exactly.  GM_ERR_ARG, with nothing launched, unless n > 0,
+ * 1 <= ch <= 4 and every pointer is 16-byte aligned. */
+int gm_image_to_rows(gm_ctx* ctx, const float* x_nchw_dev, const void* out_nhwc_dev /* nullable */, int n, int ch, void* dst_nhwc_dev,
+                     gm_stream stream);
+int gm_rows_to_image(gm_ctx* ctx, const void* src_nhwc_dev, int n, int ch, float* dst_nchw_dev, gm_stream stream);
 /* generator noise rows as a bf16 GEMM operand: Philox N(0,1) (noise_dev NULL) or a caller tensor [rows, z] fp32 */
 int gm_noise_rows(gm_ctx* ctx, const float* noise_dev, void* out_dev, int rows, int z, int ld, uint64_t seed, uint64_t stream_id,
                   gm_stream stream);

@@ -12,7 +12,12 @@ epoch time is the training loop plus one evaluation batch.  Beside that:
   - the host path's batch alone: process_batch + stage_images, ending in a synchronise (median of 5);
   - gm_stage_pool_rows alone: CUDA events around --launches launches at B, as bytes moved (the codes read once, the bf16
     rows written) per second against the H100 SXM's 3.35 TB/s;
-  - the one-off packing of the pool (DevicePool.from_loader).
+  - the one-off packing of the pool (DevicePool.from_loader);
+  - a user-written loss: DCGANTrainer subclassed with the reference's NS train_D / train_G in torch (src/ns_gan.py:172-216),
+    so train() runs the reference loop through the autograd nodes, against the fused DCGANTrainer.train on the same host
+    loader, alternated for --rounds rounds, with the bytes the engine holds per D and per G call slot;
+  - stage_images before (the torch expression it replaced) and after gm_image_to_rows: CUDA events around --launches calls
+    at B on a device-resident fp32 batch.
 Prints one JSON line with the device name and power limit read in the same run.  Writes nothing but stdout.
 """
 import argparse
@@ -144,7 +149,67 @@ def main():
         out["stage_pool_rows"].append({"rows": rows, "launches": a.launches, "us": round(ms * 1e3, 2), "bytes": moved,
                                        "tb_per_s": round(moved / (ms * 1e-3) / 1e12, 3),
                                        "of_hbm_peak": round(moved / (ms * 1e-3) / HBM_PEAK, 3)})
+    out["custom_loss"] = custom_loss_leg(a, loader, B, N)
     print(json.dumps(out))
+
+
+def custom_loss_leg(a, loader, B, N):
+    import torch
+    import dc_gan
+
+    class NSOverride(dc_gan.DCGANTrainer):
+        """the reference's NS losses (src/ns_gan.py:172-216) as a user override"""
+
+        def train_D(self, images):
+            noise = self.compute_noise(images.shape[0], self.model.z_dim)
+            G_output = self.model.G(noise)
+            DX_score, DG_score = self.model.D(images), self.model.D(G_output)
+            return torch.sum(-torch.mean(torch.log(DX_score + 1e-8) + torch.log(1 - DG_score + 1e-8)))
+
+        def train_G(self, images):
+            noise = self.compute_noise(images.shape[0], self.model.z_dim)
+            return -torch.mean(torch.log(self.model.D(self.model.G(noise)) + 1e-8))
+
+    torch.manual_seed(2)
+    trainers = {"fused": dc_gan.DCGANTrainer(dc_gan.DCGAN(hidden_dim=64, z_dim=100), loader, loader, loader),
+                "custom": NSOverride(dc_gan.DCGAN(hidden_dim=64, z_dim=100), loader, loader, loader)}
+    assert trainers["custom"]._has_custom_step() and not trainers["fused"]._has_custom_step()
+
+    def train(tr):
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        with contextlib.redirect_stdout(io.StringIO()):
+            tr.train(num_epochs=1)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t
+    for tr in trainers.values():
+        train(tr)
+    wall = {k: [] for k in trainers}
+    for _ in range(a.rounds):
+        for k, tr in trainers.items():
+            wall[k].append(train(tr))
+    eng = trainers["custom"]._engine
+    slot_bytes = {kind: sum(t.numel() * t.element_size() for key, t in eng._bufs.items() if key.startswith(pfx))
+                  for kind, pfx in (("d_slot", "cd0"), ("g_slot", "cg0"), ("d_backward_shared", "cdb"))}
+    out = {k: {"s": [round(v, 4) for v in w], "images_per_s": round(N / _median(w), 1)} for k, w in wall.items()}
+    out["custom_over_fused_time"] = round(_median(wall["custom"]) / _median(wall["fused"]), 3)
+    out["bytes"] = slot_bytes
+    g = torch.Generator(device="cuda").manual_seed(3)
+    x = torch.rand(B, 3 * 4096, device="cuda", generator=g)
+    legs = {"torch_expression": lambda i: x.view(B, 3, 64, 64).permute(0, 2, 3, 1).to(torch.bfloat16).contiguous(),
+            "gm_image_to_rows": lambda i: eng.stage_images(x)}
+    for fn in legs.values():
+        for i in range(10):
+            fn(i)
+    times = {k: [] for k in legs}
+    for _ in range(3):
+        for k, fn in legs.items():
+            times[k].append(_event_ms(fn, a.launches))
+    moved = B * 4096 * 3 * (4 + 2)                                    # fp32 read, bf16 written
+    out["stage_images"] = {k: {"us": round(_median(v) * 1e3, 2), "tb_per_s": round(moved / (_median(v) * 1e-3) / 1e12, 3)}
+                           for k, v in times.items()}
+    out["stage_images"]["bytes"] = moved
+    return out
 
 
 if __name__ == "__main__":
