@@ -318,23 +318,41 @@ int gm_vae_decode(gm_vae* vae, const float* z_dev, int n, float* out_images_dev,
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
  * gm_im2col_k4s2 + gm_gemm_bf16, a transposed convolution gm_gemm_bf16 + gm_col2im_k4s2; their gradients are the same
- * two data movements with the roles swapped.  The DCGAN engine that sequences them is gm_b200/dcgan.py. */
+ * two data movements with the roles swapped.  The DCGAN engine that sequences them is gm_b200/dcgan.py.
+ * Every entry point below checks its arguments before it launches or allocates anything: GM_ERR_ARG for a NULL, non-positive,
+ * out-of-range or misaligned argument, GM_ERR_UNSUPPORTED for a size the kernels' 32-bit indices cannot hold.
+ * gm_im2col_k4s2: x [B*H*W, ldx] -> col [B*(H/2)*(W/2), ldc], columns (kh, kw, c).  Refused: odd H or W, ldx < C, ldc < 16 C;
+ * when C is a multiple of 8 (the 16-byte path) ldx or ldc not a multiple of 8 or x / col not 16-byte aligned;
+ * GM_ERR_UNSUPPORTED for 2^31 or more items (an item is 16 bytes of col, or one tap of one pixel when C % 8 != 0). */
 int gm_im2col_k4s2(gm_ctx* ctx, const void* x_dev, int B, int H, int W, int C, int ldx, void* col_dev, int ldc, gm_stream stream);
-/* mode 0: sum of taps, 1: sigmoid(sum), 2: sum * LeakyReLU'(aux), 3: sum * aux (1 - aux) */
+/* col [B*Hi*Wi, ldc] -> y [B*2Hi*2Wi, ldy].  mode 0: sum of taps, 1: sigmoid(sum), 2: sum * LeakyReLU'(aux), 3: sum * aux (1 - aux),
+ * aux [B*2Hi*2Wi, ld_aux] read in modes 2 and 3 only (aux > 0 selects slope 1; +0, -0 and negative values select `slope`).
+ * Refused: mode outside 0..3, modes 2 / 3 without aux or with ld_aux < C, ldc < 16 C, ldy < C; when C is a multiple of 8 a
+ * leading dimension (ld_aux in modes 2 / 3) not a multiple of 8 or col / y / aux not 16-byte aligned; GM_ERR_UNSUPPORTED for C
+ * above 8 that is not a multiple of 8, and for 2^31 or more output items (pixels x C/8 groups). */
 int gm_col2im_k4s2(gm_ctx* ctx, const void* col_dev, int ldc, int B, int Hi, int Wi, int C, void* y_dev, int ldy, int mode,
                    const void* aux_dev, int ld_aux, float slope, gm_stream stream);
-/* nn.BatchNorm2d in training mode over NHWC rows, fused with the following activation (act 0 none, 1 ReLU, 2 LeakyReLU) */
+/* nn.BatchNorm2d in training mode over NHWC rows x [rows, ld], fused with the following activation (act 0 none, 1 ReLU,
+ * 2 LeakyReLU) into y [rows, ldy].  gm_bn_backward reads BOTH dy and x with leading dimension ld and writes dx [rows, lddx];
+ * it expects the stats gm_bn_forward stored.  Refused by the three gm_bn_* calls: C, ld, ldy / lddx not multiples of 8, a
+ * leading dimension below C, act outside 0..2, x / y / dy / dx not 16-byte aligned; GM_ERR_UNSUPPORTED for C > 2048. */
 int gm_bn_forward(gm_ctx* ctx, const void* x_dev, long long rows, int C, int ld, const float* gamma_dev, const float* beta_dev, float eps,
                   int act, float slope, void* y_dev, int ldy, float* stats_dev /* [2][C]: mean, invstd */,
                   float* running_dev /* [2][C] or NULL */, float momentum, gm_stream stream);
 int gm_bn_backward(gm_ctx* ctx, const void* dy_dev, const void* x_dev, long long rows, int C, int ld, const float* stats_dev,
                    const float* gamma_dev, const float* beta_dev, int act, float slope, void* dx_dev, int lddx,
                    float* dgb_dev /* [2][C]: dbeta, dgamma */, gm_stream stream);
-/* fp32 [R, C] -> bf16 [R, ld] and / or its transpose [C, ld_t] (the two GEMM operand forms of a weight matrix) */
+/* fp32 [R, C] -> bf16 [R, ld] and / or its transpose [C, ld_t] (the two GEMM operand forms of a weight matrix), rounded to
+ * nearest even.  Refused: both outputs NULL, ld < C with dst, ld_t < R with dst_t; GM_ERR_UNSUPPORTED for R C >= 2^31. */
 int gm_cast_bf16(gm_ctx* ctx, const float* src_dev, int R, int C, void* dst_dev, int ld, void* dst_t_dev, int ld_t, gm_stream stream);
-/* out [rows, ld] bf16 with column 0 = v[r], the rest 0 */
+/* out [rows, ld] bf16 with column 0 = v[r], the rest 0; GM_ERR_UNSUPPORTED for rows ld >= 2^31 */
 int gm_pack_col0(gm_ctx* ctx, const float* v_dev, int rows, void* out_dev, int ld, gm_stream stream);
-/* process_batch (src/ns_gan.py:222-226, src/ae.py:150-151) as a standalone step: images -> bf16 rows [rows, ld], ones column at x */
+/* process_batch (src/ns_gan.py:222-226, src/ae.py:150-151) as a standalone step: images [*, x] -> bf16 rows [rows, ld], a ones
+ * column at x and zeros up to ld; row r reads image gather_idx_dev[r] (r when NULL).  GM_IMG_F32 rounds to nearest even.
+ * GM_IMG_U8 and GM_IMG_BITS binarise: a u8 value becomes 1 when it is non-zero (255 and 3 alike), and the bit format is one
+ * bit per value over the whole [*, x] array in np.packbits order (most significant bit first; rows are not byte aligned
+ * unless x is a multiple of 8).  Refused: img_fmt outside gm_img_fmt, ld <= x or not a multiple of 8, out not 16-byte aligned,
+ * fp32 images or gather_idx not 4-byte aligned. */
 int gm_stage_images(gm_ctx* ctx, const void* images_dev, int img_fmt, const int* gather_idx_dev, void* out_dev, int rows, int x, int ld,
                     gm_stream stream);
 /* A batch drawn from a device-resident dataset of 8-bit codes (gm_b200.dcgan.DevicePool): codes_dev [n_pool, row_vals] uint8
@@ -354,11 +372,14 @@ int gm_stage_pool_rows(gm_ctx* ctx, const uint8_t* codes_dev, long long n_pool, 
 int gm_image_to_rows(gm_ctx* ctx, const float* x_nchw_dev, const void* out_nhwc_dev /* nullable */, int n, int ch, void* dst_nhwc_dev,
                      gm_stream stream);
 int gm_rows_to_image(gm_ctx* ctx, const void* src_nhwc_dev, int n, int ch, float* dst_nchw_dev, gm_stream stream);
-/* generator noise rows as a bf16 GEMM operand: Philox N(0,1) (noise_dev NULL) or a caller tensor [rows, z] fp32 */
+/* generator noise rows as a bf16 GEMM operand out [rows, ld]: columns [0, z) Philox N(0,1) keyed by (seed, stream_id)
+ * (noise_dev NULL) or a caller tensor [rows, z] fp32 rounded to nearest even, column z = 1, zeros up to ld.  Refused: ld <= z
+ * or not a multiple of 8, out not 16-byte aligned; GM_ERR_UNSUPPORTED for rows ceil((z + 1) / 8) >= 2^31. */
 int gm_noise_rows(gm_ctx* ctx, const float* noise_dev, void* out_dev, int rows, int z, int ld, uint64_t seed, uint64_t stream_id,
                   gm_stream stream);
 /* the adversarial loss + dL/dlogit on a logit vector (train_D: batch real then batch fake rows; train_G: batch fake rows);
- * row-wise variants only (NS, MM, W, LS, f-GAN) */
+ * row-wise variants only (NS, MM, W, LS, f-GAN): GM_ERR_UNSUPPORTED for the other gm_variant values, GM_ERR_ARG for a variant
+ * or out_act outside their enums and for batch outside 1..2^30.  loss_dev[0] = loss, [1] = sum of ds (a fixed-order sum). */
 int gm_loss_rows(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, int g_step, float inv_global_batch,
                  float* ds_dev, float* d_out_dev, float* loss_dev, gm_stream stream);
 /* WGAN-GP on the batch-norm-free conv critic (src/w_gp_gan.py:197-218; gm_b200/dcgan.py sequences it).
@@ -370,10 +391,12 @@ int gm_gp_interp_rows(gm_ctx* ctx, const void* xr_dev, int ldr, const void* xf_d
  * (0 when ||g_b|| = 0) as bf16, and loss_dev[0] += lambda inv_loss sum_b (||g_b|| - 1)^2 (loss_dev nullable) */
 int gm_gp_penalty(gm_ctx* ctx, const void* g_dev, int ldg, int B, int HW, int C, float lambda, float inv_grad, float inv_loss,
                   void* r_dev, int ldr, float* norm_dev, float* loss_dev, gm_stream stream);
-/* gm_im2col_k4s2 of x * LeakyReLU'(m) (the sign of m selects slope 1 or `slope`); C a multiple of 8 */
+/* gm_im2col_k4s2 of x * LeakyReLU'(m) (m > 0 selects slope 1, anything else `slope`), the product rounded once.  Refused like
+ * gm_im2col_k4s2, and: C, ldx, ldm or ldc not a multiple of 8, ldm < C, x / m / col not 16-byte aligned. */
 int gm_im2col_k4s2_lrelu_mask(gm_ctx* ctx, const void* x_dev, int B, int H, int W, int C, int ldx, const void* m_dev, int ldm, float slope,
                               void* col_dev, int ldc, gm_stream stream);
-/* out = x * LeakyReLU'(m) over rows [rows, C]; C a multiple of 8; out may alias x or m */
+/* out = x * LeakyReLU'(m) over rows [rows, C]; out may alias x or m.  Refused: C or a leading dimension not a multiple of 8 or
+ * below C, x / m / out not 16-byte aligned; GM_ERR_UNSUPPORTED for rows C / 8 >= 2^31. */
 int gm_lrelu_mask_rows(gm_ctx* ctx, const void* x_dev, int ldx, const void* m_dev, int ldm, long long rows, int C, float slope,
                        void* out_dev, int ldo, gm_stream stream);
 /* Batch-statistic D losses (RaNS src/ra_gan.py:204-205, Fisher src/fisher_gan.py:214-223) on a logit vector [real B | fake B],
