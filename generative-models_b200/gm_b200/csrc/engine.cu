@@ -151,24 +151,49 @@ static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 gri
 template <int BN, bool AMN, bool BMN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false>
 static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
   using Cfg = GemmCfg<BN, !AMN>;
+  constexpr int CL = kGemmCluster<BN, AMN, BMN>;
   auto kern = gemm_wgmma_kernel<BN, AMN, BMN, ACT_T, AUX_T, BIAS_T, DOT_T, SPLIT>;
-  // the opt-in to > 48 KB dynamic shared memory is per (function, device)
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
-  }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3(pl.grid);
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
   cfg.stream = s;
-  cudaLaunchAttribute at[1];
+  cudaLaunchAttribute at[2];
   int na = 0;
+  if (CL > 1) {
+    at[na].id = cudaLaunchAttributeClusterDimension;
+    at[na].val.clusterDim.x = CL;
+    at[na].val.clusterDim.y = 1;
+    at[na].val.clusterDim.z = 1;
+    ++na;
+  }
+  // the opt-in to > 48 KB dynamic shared memory is per (function, device); so is the number of clusters that fit at once
+  static bool configured[64] = {};
+  static int max_clusters[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const bool cached = dev >= 0 && dev < 64;
+  int mc = cached ? max_clusters[dev] : 0;
+  if (!cached || !configured[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    if (CL > 1) {
+      cfg.gridDim = dim3(CL);
+      cfg.attrs = at;
+      cfg.numAttrs = na;
+      e = cudaOccupancyMaxActiveClusters(&mc, kern, &cfg);
+      if (e != cudaSuccess) return e;
+      if (mc < 1) return cudaErrorInvalidConfiguration;
+    }
+    if (cached) { max_clusters[dev] = mc; configured[dev] = true; }
+  }
+  if (CL > 1) {
+    // persistent: one cluster per item, up to the clusters the device holds at once (a GPC may hold an odd number of SMs)
+    const GemmParams& q = pl.p;
+    const int items = cdiv(q.m_tiles, CL) * q.n_tiles * q.splits;
+    cfg.gridDim = dim3(CL * (items < mc ? items : mc));
+  }
   static const char* skip_gemm = getenv("GM_PDL_SKIP");
   if (g_pdl && !(skip_gemm && strstr(skip_gemm, "gemm") != nullptr)) {
     at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -291,7 +316,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
   int bn, boxn = 0;
   if (mode == 0) {
     if (ncover <= 64) { pl->kind = PK_NT_64; bn = 64; boxn = 64; }
-    else { pl->kind = PK_NT_208; bn = 208; boxn = 208; }
+    else { pl->kind = PK_NT_208; bn = 208; boxn = 208 / kGemmCluster<208, false, false>; }   // each CTA's share of the B tile
     int rc = make_tmap(c, &pl->tmA, A, K, M, lda, BK, BM);
     if (rc) return rc;
     rc = make_tmap(c, &pl->tmB, B, K, N, ldb, BK, boxn);

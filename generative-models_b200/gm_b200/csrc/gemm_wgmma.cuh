@@ -17,7 +17,8 @@
 // fp32 scratch tile, and lane L takes row L & 15 and the 32-column block of parity L >> 4 through
 // the per-row epilogue; the scratch is then reused as the bf16 staging of the store.  Meanwhile
 // the producer keeps filling the smem ring with the next tile's operands.  Pipelines: smem ring
-// full/empty mbarriers (TMA <-> wgmma), static round-robin tile scheduler (grid = #SMs).
+// full/empty mbarriers (TMA <-> wgmma), static round-robin tile scheduler (grid = #SMs).  The 128 x 208
+// K-major kernel runs as 2-CTA clusters that share the B tile (kGemmCluster).
 #pragma once
 #include "ptx.cuh"
 
@@ -137,6 +138,12 @@ struct GemmCfg {
   static_assert(BN < 208 || STAGES >= 4, "the 208- and 256-wide kernels need a 4-stage ring to hide TMA latency");
 };
 
+// CTAs per cluster.  The 128 x 208 K-major kernel runs as 2-CTA clusters on adjacent m-tiles of one n-tile: both read
+// the same B tile (a slice of the weight matrix), so each CTA loads BN / 2 of its rows and multicasts them into both
+// CTAs' stage.  That cuts the bytes L2 feeds each CTA per k-block from 43 008 to 29 696, which bound the long-K mainloop.
+template <int BN, bool A_MN, bool B_MN>
+constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 2 : 1;
+
 // Epilogue specialisation: ACT_T / AUX_T / BIAS_T / DOT_T >= 0 fix the fused epilogue at
 // compile time (small code: the whole kernel must stay inside the instruction cache);
 // -1 selects the universal variant that reads the choice from GemmParams at run time.
@@ -149,7 +156,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   static_assert(!SPLIT || ACT_T < 0, "split operands: universal epilogue only");
   using Cfg = GemmCfg<BN, !A_MN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int CL = kGemmCluster<BN, A_MN, B_MN>;
   static_assert(!B_MN || BN % 64 == 0, "MN-major B needs 64-wide atoms");
+  // each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for one box
+  static_assert(CL == 1 || (!B_MN && (BN / CL) % 8 == 0 && (Cfg::B_BYTES / CL) % 1024 == 0), "multicast B share");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -169,15 +179,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (p.tma_store) tma_prefetch_desc(&tmC);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kConsumerWarps);   // every consumer warp releases the slot
+      // every consumer warp of every CTA in the cluster releases the slot: the peers' multicasts also write it
+      mbar_init(empty_bar(s), CL * kConsumerWarps);
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  // the barriers are initialised in every CTA of the cluster before any peer arrives on them or multicasts into them
+  if constexpr (CL > 1) cluster_sync();
+  else __syncthreads();
   griddep_wait();     // barrier init above overlapped the previous grid's tail
 
-  const int tiles = p.m_tiles * p.n_tiles;   // work items walk (split, m-tile, n-tile)
+  // Work items walk (split, m-group, n-tile) with one item per cluster; CTA rank r of a cluster takes m-tile CL * group + r.
+  // m-tiles are rounded up to whole groups: a CTA on a tile past M loads its share of B, computes on zero-filled A rows
+  // and stores nothing (every store is guarded by row < M or clipped at the tensor extent), so both CTAs walk the same
+  // k-blocks through the ring.
+  const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
+  const int tiles = (p.m_tiles + CL - 1) / CL * p.n_tiles;
   const int total = tiles * p.splits;
+  const int first = blockIdx.x / CL, stride = gridDim.x / CL;
 
   if (warp < kProducerThreads / 32) {
     // =========================== TMA producer ===========================
@@ -188,10 +207,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       int stage = 0;
       uint32_t phase = 0;
       const bool leader = elect_one();
-      for (int item = blockIdx.x; item < total; item += gridDim.x) {
+      for (int item = first; item < total; item += stride) {
         const int split = item / tiles;
         const int rem = item - split * tiles;
-        const int m0 = (rem / p.n_tiles) * BM;
+        const int m0 = ((rem / p.n_tiles) * CL + rank) * BM;
         const int n0 = (rem % p.n_tiles) * BN;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
@@ -213,7 +232,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               for (int a = 0; a < BM / 64; ++a)
                 tma_load_2d(a_dst + a * (BK * 128), ta, full_bar(stage), m0 + a * 64, k0);
             }
-            if constexpr (!B_MN) {
+            if constexpr (CL > 1) {   // rows [n0 + r BN/CL, +BN/CL) into this and the peer CTA; the full barrier expects both shares
+              tma_load_2d_multicast(b_dst + rank * (Cfg::B_BYTES / CL), tb, full_bar(stage), k0, n0 + rank * (BN / CL), (1u << CL) - 1);
+            } else if constexpr (!B_MN) {
               tma_load_2d(b_dst, tb, full_bar(stage), k0, n0);
             } else {
 #pragma unroll
@@ -295,15 +316,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
       }
     };
+    // a stage this warp has finished reading is released in this CTA and in its cluster peer (whose producer multicasts into it)
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(empty_bar(s));
+        if constexpr (CL > 1) mbar_arrive_cluster(mapa_shared(empty_bar(s), uint32_t(rank ^ 1)));
+      }
+    };
     int stage = 0;
     uint32_t phase = 0;
     int acc_iter = 0;
 #pragma unroll 1
-    for (int item = blockIdx.x; item < total; item += gridDim.x, ++acc_iter) {
+    for (int item = first; item < total; item += stride, ++acc_iter) {
       const int split = item / tiles;
       const int rem = item - split * tiles;
       const int n_tile = rem % p.n_tiles;
-      const int m0 = (rem / p.n_tiles) * BM;
+      const int m0 = ((rem / p.n_tiles) * CL + rank) * BM;
       const int n0 = n_tile * BN;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
@@ -332,19 +361,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         wgmma_commit();
         wgmma_wait<1>();
         wgmma_pin(acc);
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(prev));
-        }
+        if (prev >= 0) release(prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
       wgmma_wait<0>();
       wgmma_pin(acc);
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(prev));
-      }
+      if (prev >= 0) release(prev);
       const long long tm1 = phase_clock();
       if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && acc_iter < 16 && threadIdx.x == kProducerThreads) {
         long long* d = p.dbg + acc_iter * 4;   // [tile][0, mainloop, 0, start stamp]
@@ -415,10 +438,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           aux_fetch(0);
           // pull the aux tile of the NEXT tile this warp will process (same rows of the tile)
           // into L2 now: its loads are otherwise HBM-latency-bound
-          const int nitem = item + gridDim.x;
+          const int nitem = item + stride;
           if (nitem < total) {
             const int nrem = nitem - (nitem / tiles) * tiles;
-            const int nm0 = (nrem / p.n_tiles) * BM + wg * 64 + (cw & 3) * 16;
+            const int nm0 = ((nrem / p.n_tiles) * CL + rank) * BM + wg * 64 + (cw & 3) * 16;
             const int nn0 = (nrem % p.n_tiles) * BN;
             // 16 rows x 416 B: four 128-byte lines per row
             for (int t = lane; t < kEpiRows * 4; t += 32) {
@@ -688,7 +711,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     stage_acquire();   // the last bulk store has read its staging tile before shared memory goes away
   }
-  __syncthreads();
+  // no CTA exits while a peer may still arrive on its barriers (its multicasts have all landed: every stage was consumed)
+  if constexpr (CL > 1) cluster_sync();
+  else __syncthreads();
 }
 
 }  // namespace gm
