@@ -77,7 +77,6 @@ def lib():
     L.gm_launch_count.restype = C.c_longlong
     L.gm_prof_enable.argtypes = [vp, i]
     L.gm_prof_report.argtypes = [vp, C.c_char_p, i]
-    L.gm_debug_phase_buffer.argtypes = [vp, vp]
     L.gm_prof_collect.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_longlong)]
     L.gm_gemm_bf16.argtypes = [vp, C.POINTER(GemmDesc), vp]
     L.gm_adam_step.argtypes = [vp, vp, vp, vp, vp, i, C.POINTER(AdamHP), i, vp]

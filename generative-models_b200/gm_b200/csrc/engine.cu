@@ -28,7 +28,6 @@ struct gm_ctx {
   size_t scratch_bytes = 0;
   // optional per-launch GEMM timing (bench.py roofline): CUDA events on the launch stream
   bool prof = false;
-  long long* dbg = nullptr;   // phase-timing buffer handed to the next generic GEMM (tools/time_phases.py)
   void* red = nullptr;        // scratch of the conv building blocks' two-stage reductions (engine_conv.inl)
   size_t red_bytes = 0;
   void* loss_zero = nullptr;  // 64 zero bytes: bias / Fisher state / completion counter for gm_loss_rows
@@ -129,11 +128,9 @@ static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 gri
     }
     ~Scope() { if (on) { cudaEventRecord(r.e1, s); g_prof_all_recs.push_back(r); } }
   } scope(name, s);
-  // GM_PDL_SKIP=name1,name2: launch those kernels WITHOUT the programmatic-serialization attribute (tuning / bisecting)
   // xhat_kernel never takes the attribute: launched early behind the generator's output GEMM its CTAs would pile up on
   // the first SMs that GEMM frees instead of spreading over the whole chip
-  static const char* skip = getenv("GM_PDL_SKIP");
-  const bool pdl = g_pdl && !(skip && strstr(skip, name) != nullptr) && strcmp(name, "xhat_kernel") != 0;
+  const bool pdl = g_pdl && strcmp(name, "xhat_kernel") != 0;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = grid;
@@ -194,8 +191,7 @@ static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
     const int items = cdiv(q.m_tiles, CL) * q.n_tiles * q.splits;
     cfg.gridDim = dim3(CL * (items < mc ? items : mc));
   }
-  static const char* skip_gemm = getenv("GM_PDL_SKIP");
-  if (g_pdl && !(skip_gemm && strstr(skip_gemm, "gemm") != nullptr)) {
+  if (g_pdl) {
     at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
@@ -226,7 +222,6 @@ static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
   if (bias && !dot && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0>(pl, s);
   if (bias && !dot && aux == AUX_NONE && p.act == ACT_SIGMOID) return launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0>(pl, s);
   if (bias && dot && p.dot_mask == 1 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 3>(pl, s);
-  if (bias && dot && p.dot_mask == 2 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 4>(pl, s);
   if (bias && dot && p.dot_mask == 3 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 5>(pl, s);
   if (p.dot_mask) return launch_inst<208, false, false>(pl, s);
   if (bias && dot && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 1>(pl, s);
@@ -433,13 +428,6 @@ extern "C" long long gm_launch_count(gm_ctx* c, int reset) {
   return n;
 }
 
-// debug aid: 128 int64 SM-clock stamps written by CTA 0 of subsequent gm_gemm_bf16 calls
-extern "C" int gm_debug_phase_buffer(gm_ctx* c, long long* dbg_dev) {
-  if (!c) return GM_ERR_ARG;
-  c->dbg = dbg_dev;
-  return GM_OK;
-}
-
 extern "C" int gm_prof_enable(gm_ctx* c, int on) {
   if (!c) return GM_ERR_ARG;
   c->prof = on == 1;
@@ -526,7 +514,6 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
   int rc = plan_gemm(c, &pl, d->mode, d->M, d->N, d->K, d->A_dev, d->lda, d->B_dev, d->ldb, ncover, f32 ? 64 : 1);
   if (rc) return rc;
   GemmParams& p = pl.p;
-  p.dbg = c->dbg;
   if (!f32) {
     p.epi = EPI_BF16;
     p.out = static_cast<__nv_bfloat16*>(d->C_dev);
@@ -683,10 +670,9 @@ struct gm_gan {
   float* dw2sum = nullptr;       // [3][HP]: loss path, penalty T path, DRAGAN ds_gp path
   float *dw2p2 = nullptr, *dw2p3 = nullptr, *slots_v = nullptr, *coef = nullptr, *stats = nullptr;
   double *gp_part = nullptr, *mom_part = nullptr;
-  int nreg = 2;                  // row regions of Xall/Aall/DHall: real, fake (, xhat, R)
-  // WGAN-GP: D's first layer is linear, so the penalty's hidden pre-activation is eps a(x) + (1-eps) a(G(z)): the x_hat
-  // rows and their third of the D-layer GEMM are not formed (gp_hat_kernel).  GM_WGP_XHAT=1 keeps the materialised rows.
-  bool wgp_linear = false;
+  // row regions of Xall/Aall/DHall: real, fake (, xhat, R).  Only DRAGAN has the xhat region: WGAN-GP's D layer is linear, so
+  // the penalty's hidden pre-activation eps a(x) + (1-eps) a(G(z)) comes from the real / fake rows (gp_hat_kernel)
+  int nreg = 2;
   // InfoGAN: auxiliary network Q (image -> hidden -> disc+cont codes), its own Adam state and a
   // SECOND Adam state for G (MI_optimizer spans G and Q, src/info_gan.py:146-148)
   NetLayout Qn;
@@ -770,10 +756,8 @@ extern "C" int gm_gan_create(gm_ctx* c, const gm_gan_desc* d, gm_gan** out) {
   g->D.init(g->X, g->H, d->variant == GM_BEGAN ? g->X : 1);
   g->region_rows = g->Bmax;
   g->nreg = d->variant == GM_WGP ? 3 : (d->variant == GM_DRA ? 4 : 2);
-  {
-    const char* e = getenv("GM_WGP_XHAT");
-    g->wgp_linear = d->variant == GM_WGP && !(e && atoi(e) != 0) && g->HP <= 64 * kGpHatGroups * 4;   // gp_hat_kernel: <= 2 column groups per lane
-  }
+  // WGAN-GP always runs gp_hat_kernel: every hidden width this function accepts (hidden_dim + 1 <= 448) must fit its lanes
+  static_assert(448 <= 64 * kGpHatGroups * 4, "gp_hat_kernel covers at most 64 * kGpHatGroups * 4 hidden columns");
   const size_t B = g->Bmax;
   const size_t NR = g->nreg;
   int rc = GM_OK;
@@ -955,7 +939,6 @@ extern "C" int gm_gan_materialize_grads(gm_gan* g, gm_stream stream) {
 static void set_bf16_epi(GemmParams& p, __nv_bfloat16* out, int ldo, int out_cols, int pad_one, const float* bias, int act) {
   p.epi = EPI_BF16; p.out = out; p.ldo = ldo; p.out_cols = out_cols; p.pad_one = pad_one; p.bias = bias; p.act = act;
   p.aux = nullptr; p.aux_mode = AUX_NONE; p.dot_w = nullptr; p.dot_out = nullptr; p.dot_sq = 0; p.row_scale = nullptr; p.row_split = 0; p.dot_mask = 0; p.row_vec = nullptr;
-  p.mask_row0 = 0; p.out_alt = nullptr;
 }
 
 static int build_plans(gm_gan* g, int B, StepPlans** out) {
@@ -980,18 +963,14 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
   if ((rc = plan_gemm(c, &sp.g2, 0, B, X, H, g->Hg, HP, g->W2g_s, H, XP, 1))) return rc;
   set_bf16_epi(sp.g2.p, Xfake, XP, XP, 1, pG + g->G.off_b2, ACT_SIGMOID);
   // D layer 1 (+ fused 400->1 row-dot) on [real; fake] (D step) and on fake only (G step)
-  const int nfwd = (g->nreg > 2 && !g->wgp_linear) ? 3 : 2;      // GP variants also score the interpolated rows (when they exist)
+  const int nfwd = g->d.variant == GM_DRA ? 3 : 2;      // DRAGAN also scores the interpolated rows
   if ((rc = plan_gemm(c, &sp.d1_d, 0, nfwd * B, H, X, g->Xall, XP, g->W1d_s, X, H, 1))) return rc;
   set_bf16_epi(sp.d1_d.p, g->Aall, HP, H, 0, pD + g->D.off_b1, ACT_RELU);
   sp.d1_d.p.dot_w = pD + g->D.off_w2; sp.d1_d.p.dot_out = g->slots; sp.d1_d.p.dot_ld = slot_ld;
-  if (g->wgp_linear) {
+  if (g->d.variant == GM_WGP) {
     // WGAN-GP: the real / fake rows keep their PRE-activations (ReLU inside the row-dot and in dh_kernel): gp_hat_kernel
     // forms a_hat = eps a(x) + (1-eps) a(G(z)) from them
     sp.d1_d.p.dot_mask = 3;
-  } else if (g->nreg == 3) {
-    // WGAN-GP with materialised x_hat rows: they leave D's first layer directly as U = w2 * relu'(a_hat) (the penalty's
-    // first-gradient operand, SURVEY A.2) in the U region of DHall - no separate pass over their activations
-    sp.d1_d.p.dot_mask = 2; sp.d1_d.p.mask_row0 = 2 * B; sp.d1_d.p.out_alt = g->DHall + size_t(2) * B * HP;
   }
   if ((rc = plan_gemm(c, &sp.d1_g, 0, B, H, X, Xfake, XP, g->W1d_s, X, H, 1))) return rc;
   set_bf16_epi(sp.d1_g.p, Afake, HP, H, 0, pD + g->D.off_b1, ACT_RELU);
@@ -1334,21 +1313,18 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   const int H = g->H, HP = g->HP, X = g->X, XP = g->XP;
   const float* w2 = g->par[GM_NET_D] + g->D.off_w2;
   const size_t dh_smem = size_t(g->dh_rows_per_iter) * HP * sizeof(float);
-  if (gp && !g->wgp_linear) {
-    // interpolated rows (region 2): WGAN-GP between real and fake, DRAGAN around the real data
-    const int mode = g->d.variant == GM_DRA ? 1 : 0;
-    if (mode == 1) {
-      launch_pdl("moments_kernel", moments_kernel, c->num_sms * 2, 256, 0, s, g->Xall, B, X, XP, g->mom_part);
-      exchange_stats(g, g->mom_part, c->num_sms * 2, 2, 2, s);     // images.std() over the global batch
-      launch_pdl("moments_final_kernel", moments_final_kernel, 1, 256, 0, s, g->mom_part, c->num_sms * 2, float(double(B) * X * stat_world(g)), g->stats);
-      c->launches += 2;
-    }
-    launch_pdl("xhat_kernel", xhat_kernel, c->num_sms * 8, 256, 0, s, g->Xall, g->Xall + size_t(B) * XP, g->Xall + size_t(2) * B * XP, B, X, XP,
-                                           mode, aux, g->stats, seed, g->dev_step ? 0 : 2 * step, g->lc.dra_c, g->lo, dptr);
-    c->launches++;
+  const bool dra = g->d.variant == GM_DRA;
+  if (dra) {
+    // interpolated rows (region 2) around the real data
+    launch_pdl("moments_kernel", moments_kernel, c->num_sms * 2, 256, 0, s, g->Xall, B, X, XP, g->mom_part);
+    exchange_stats(g, g->mom_part, c->num_sms * 2, 2, 2, s);     // images.std() over the global batch
+    launch_pdl("moments_final_kernel", moments_final_kernel, 1, 256, 0, s, g->mom_part, c->num_sms * 2, float(double(B) * X * stat_world(g)), g->stats);
+    launch_pdl("xhat_kernel", xhat_kernel, c->num_sms * 8, 256, 0, s, g->Xall, g->Xall + size_t(2) * B * XP, B, X, XP,
+                                           aux, g->stats, seed, g->dev_step ? 0 : 2 * step, g->lc.dra_c, g->lo, dptr);
+    c->launches += 3;
   }
   if ((rc = launch_plan(c, sp->d1_d, s))) return rc;
-  if (g->wgp_linear) {
+  if (g->d.variant == GM_WGP) {
     // U = w2 * relu'(a_hat) and the logit part of s(x_hat) from the pre-activations of the real / fake rows
     launch_pdl("gp_hat_kernel", gp_hat_kernel, c->num_sms * 8, 256, 0, s, g->Aall, g->Aall + size_t(B) * HP, w2, g->DHall + size_t(2) * B * HP,
                g->slots + 2 * B, 2 * cdiv(H, 208), g->nreg * g->Bmax, B, H, HP, aux, seed, g->dev_step ? 0 : 2 * step, g->lo, dptr);
@@ -1356,12 +1332,12 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   }
   launch_loss(g, B, 0, inv_global_batch, s);
   launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall, g->ds, w2, g->DHall, g->dw2p, 2 * B, H, HP, g->dh_rows_per_iter, g->lo,
-             g->wgp_linear ? 1 : 0);
+             g->d.variant == GM_WGP ? 1 : 0);
   launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p, g->dh_blocks, HP, HP, g->dw2sum);
   c->launches += 2;
   if (gp) {
     const size_t rreg = size_t(g->nreg - 1) * B;
-    if (g->nreg != 3) {   // DRAGAN keeps a_hat (its penalty back-propagates through s(x_hat) too): U = 1[a_hat > 0] * w2 by a pass
+    if (dra) {   // DRAGAN keeps a_hat (its penalty back-propagates through s(x_hat) too): U = 1[a_hat > 0] * w2 by a pass
       launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, nullptr, w2, g->DHall + rreg * HP, nullptr,
                                                             B, H, HP, g->dh_rows_per_iter, g->lo, 0);
       c->launches++;
@@ -1385,7 +1361,7 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
     launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->DHg, nullptr, w2, static_cast<__nv_bfloat16*>(nullptr), g->dw2p2, B, H, HP, g->dh_rows_per_iter, g->lo, 0);
     launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p2, g->dh_blocks, HP, HP, g->dw2sum + HP);
     c->launches += 2;
-    if (g->nreg == 4) {   // DRAGAN: the penalty also back-propagates through s(xhat)
+    if (dra) {   // DRAGAN: the penalty also back-propagates through s(xhat)
       launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, g->ds + 2 * B, w2,
                                                             g->DHall + size_t(2) * B * HP, g->dw2p3, B, H, HP, g->dh_rows_per_iter, g->lo, 0);
       launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p3, g->dh_blocks, HP, HP, g->dw2sum + 2 * HP);

@@ -62,16 +62,13 @@ struct GemmParams {
   // AUX_L1 (BEGAN): out = sign(v - aux) * (row < row_split ? row_scale[0] : row_scale[1]), dot_out = sum |v - aux|
   const float* row_scale;
   int row_split;
-  // dot_mask: with the row-dot, store dot_w[n] * 1[v > 0] instead of v (the G step needs only
-  // M = w2 * relu'(a1) of D's hidden layer: dL/dx = ds * (M W1), src/ns_gan.py:57-60 backward)
+  // dot_mask, with the row-dot:
+  //   0: store v
+  //   1 (DOT_T 3): store dot_w[n] * 1[v > 0] instead of v (the G step needs only M = w2 * relu'(a1) of D's hidden
+  //      layer: dL/dx = ds * (M W1), src/ns_gan.py:57-60 backward)
+  //   3 (DOT_T 5; WGAN-GP's D forward, which never forms the x_hat rows): the row-dot runs on relu(v) but the
+  //      PRE-activation v is stored (the penalty's mask is 1[eps pre_real + (1-eps) pre_fake > 0], gp_hat_kernel)
   int dot_mask;
-  // dot_mask == 2 (DOT_T 4; WGAN-GP's D forward over [real; fake; x_hat] rows): rows >= mask_row0 store the mask form
-  // U = w2 * relu'(a1) (what the penalty's first gradient needs, SURVEY A.2) at out_alt + (row - mask_row0) * ldo,
-  // the rows below keep the activations at out + row * ldo
-  // dot_mask == 3 (DOT_T 5; WGAN-GP's D forward when the x_hat rows are never materialised): the row-dot runs on relu(v)
-  // but the PRE-activation v is stored (the penalty's mask is 1[eps pre_real + (1-eps) pre_fake > 0], gp_hat_kernel)
-  int mask_row0;
-  __nv_bfloat16* out_alt;
   // tma_store: full 32-column blocks of the bf16 output leave through the output tensor map
   // (cp.async.bulk.tensor store of the warp's swizzled staging tile) instead of LDS + STG
   int tma_store;
@@ -85,8 +82,6 @@ struct GemmParams {
   int ldp;
   int transpose;
   int f32_vec;          // set at launch: every row of every split starts on 16 bytes, so 16 columns leave as 4 float4
-  // optional phase timing (tools/time_phases.py): CTA 0 writes SM-clock stamps, see the kernel
-  long long* dbg;
   // ---- split-bf16 operands (SPLIT kernels, gm_prec GM_PREC_SPLIT): A = A_hi + A_lo, B = B_hi + B_lo as bf16 planes
   // lo_off elements apart; the contraction runs over nparts = 3 operand pairs (hi,hi), (hi,lo), (lo,hi) of kb_part
   // k-blocks each into the same accumulator (kblocks = 3 kb_part; the dropped lo*lo term is below fp32 resolution).
@@ -109,15 +104,6 @@ constexpr int kEpiVecBlocks = 8;                       // 32-column blocks of a 
 constexpr int kEpiVecBytes = kEpiVecBlocks * kEpiCols * 4 * 2;   // bias + row-dot weights
 static_assert(kEpiRows * kEpiPitch <= kEpiScratchBytes && 2 * kEpiRows * kEpiCols * 2 <= kEpiScratchBytes, "staging");
 __device__ __forceinline__ uint32_t frag_swz(int r) { return uint32_t(((r & 3) << 1) | ((r >> 2) & 1)); }
-
-// Phase timing (tools/time_phases.py) is compiled in only with -DGM_PHASE_TIMING.
-#ifdef GM_PHASE_TIMING
-__device__ __forceinline__ long long phase_clock() { return clock64(); }
-constexpr bool kPhaseTiming = true;
-#else
-__device__ __forceinline__ long long phase_clock() { return 0; }
-constexpr bool kPhaseTiming = false;
-#endif
 
 template <int BN_, bool STAGED_EPI = true>
 struct GemmCfg {
@@ -259,11 +245,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int act = ACT_T >= 0 ? ACT_T : p.act;
     const int aux_mode = AUX_T >= 0 ? AUX_T : p.aux_mode;
     const bool has_bias = BIAS_T >= 0 ? (BIAS_T != 0) : (p.bias != nullptr);
-    const bool has_dot = DOT_T >= 0 ? (DOT_T == 1 || DOT_T == 3 || DOT_T == 4 || DOT_T == 5) : (p.dot_w != nullptr);
+    const bool has_dot = DOT_T >= 0 ? (DOT_T == 1 || DOT_T == 3 || DOT_T == 5) : (p.dot_w != nullptr);
     const bool store_pre = DOT_T >= 0 ? (DOT_T == 5) : (p.dot_mask == 3);   // ReLU only inside the row-dot
-    constexpr bool kRowMask = DOT_T == 4 || DOT_T < 0;   // per-row choice between activation and mask output
     const bool mask_all = DOT_T >= 0 ? (DOT_T == 3) : (p.dot_mask == 1);
-    const bool mask_rows = DOT_T >= 0 ? (DOT_T == 4) : (p.dot_mask == 2);
     const bool has_sq = DOT_T >= 0 ? (DOT_T == 2) : (p.dot_sq != 0);
     // The bulk store serves the plain-activation epilogues only (launch_plan), so it is compiled out of the aux / row-dot
     // instances, and out of the universal 208-wide one, which those plain epilogues never reach.  Where the store path is
@@ -326,9 +310,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     };
     int stage = 0;
     uint32_t phase = 0;
-    int acc_iter = 0;
 #pragma unroll 1
-    for (int item = first; item < total; item += stride, ++acc_iter) {
+    for (int item = first; item < total; item += stride) {
       const int split = item / tiles;
       const int rem = item - split * tiles;
       const int n_tile = rem % p.n_tiles;
@@ -337,7 +320,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
       // ---------------- mainloop: one wgmma group in flight, the slot it read is released one k-block later
-      const long long tm0 = phase_clock();
       int prev = -1;
 #pragma unroll 1
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -368,16 +350,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       wgmma_pin(acc);
       if (prev >= 0) release(prev);
-      const long long tm1 = phase_clock();
-      if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && acc_iter < 16 && threadIdx.x == kProducerThreads) {
-        long long* d = p.dbg + acc_iter * 4;   // [tile][0, mainloop, 0, start stamp]
-        d[0] = 0; d[1] = tm1 - tm0; d[2] = 0; d[3] = tm0;
-      }
-      long long t_frag = 0, t_ld = 0;   // phase timing: fragment stores to the scratch tile, row reads from it
       const int wrow0 = m0 + wg * 64 + (cw & 3) * 16;   // first row of this warp
       const int row = wrow0 + er;
       const bool row_ok = row < p.M;
-      const bool mask_out = mask_all || (kRowMask && mask_rows && row >= p.mask_row0);
       constexpr bool kUniversal = ACT_T < 0;
       if (!A_MN && !(kUniversal && p.epi == EPI_F32)) {
         // ================= bf16 epilogue (K-major kernels) =================
@@ -468,17 +443,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const bool step_tma = tma_st && BN - cs >= kEpiStep && wrow0 < p.M;
           // accumulator fragments -> scratch -> this lane's row: both chunks in flight, one wait
           stage_acquire();
-          const long long tf0 = phase_clock();
           frag_to_scratch(s);
           __syncwarp();
-          const long long tl0 = phase_clock();
           uint32_t raw[2][16];
 #pragma unroll
           for (int q = 0; q < 2; ++q)
             if (q < nch && col0 + q * 16 < p.N) scratch_ld16(par * kEpiCols + q * 16, raw[q]);
           __syncwarp();
-          t_frag += tl0 - tf0;
-          t_ld += phase_clock() - tl0;
           uint4 ax[4];
           if (aux_mode != AUX_NONE) {   // prefetched aux (coalesced mapping) -> smem -> own row
             if constexpr (kAuxAsync) {
@@ -591,7 +562,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                       dot = fmaf(v[4 * k4 + 0], __uint_as_float(w.x), dot); dot = fmaf(v[4 * k4 + 1], __uint_as_float(w.y), dot);
                       dot = fmaf(v[4 * k4 + 2], __uint_as_float(w.z), dot); dot = fmaf(v[4 * k4 + 3], __uint_as_float(w.w), dot);
                     }
-                    if (mask_out) {
+                    if (mask_all) {
                       v[4 * k4 + 0] = v[4 * k4 + 0] > 0.f ? __uint_as_float(w.x) : 0.f;
                       v[4 * k4 + 1] = v[4 * k4 + 1] > 0.f ? __uint_as_float(w.y) : 0.f;
                       v[4 * k4 + 2] = v[4 * k4 + 2] > 0.f ? __uint_as_float(w.z) : 0.f;
@@ -609,8 +580,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const uint4 hi = make_uint4(pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
                 if constexpr (SPLIT) {   // residual plane of the output: v - bf16(v), straight from registers
                   if (p.lo_off != 0 && p.out != nullptr && row_ok && c0 < p.out_cols) {
-                    __nv_bfloat16* ob = (mask_rows && row >= p.mask_row0) ? p.out_alt + size_t(row - p.mask_row0) * p.ldo : p.out + size_t(row) * p.ldo;
-                    uint4* ol = reinterpret_cast<uint4*>(ob + p.lo_off + c0);
+                    uint4* ol = reinterpret_cast<uint4*>(p.out + size_t(row) * p.ldo + p.lo_off + c0);
                     ol[0] = make_uint4(pack_bf16x2_residual(v[0], v[1], lo.x), pack_bf16x2_residual(v[2], v[3], lo.y),
                                        pack_bf16x2_residual(v[4], v[5], lo.z), pack_bf16x2_residual(v[6], v[7], lo.w));
                     ol[1] = make_uint4(pack_bf16x2_residual(v[8], v[9], hi.x), pack_bf16x2_residual(v[10], v[11], hi.y),
@@ -648,9 +618,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const int rr = wrow0 + it * 4 + lr;
                 if (rr < p.M) {
                   __nv_bfloat16* dst = o + size_t(it * 4) * p.ldo;
-                  if constexpr (kRowMask) {
-                    if (mask_rows && rr >= p.mask_row0) dst = p.out_alt + size_t(rr - p.mask_row0) * p.ldo + oc;
-                  }
                   *reinterpret_cast<uint4*>(dst) = lds128(sa + it * 4 * kEpiPitch);
                 }
               }
@@ -660,10 +627,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         if ((has_dot || has_sq || aux_mode == AUX_VAE_OUT || aux_mode == AUX_L1) && p.dot_out != nullptr && row_ok)
           p.dot_out[size_t(n_tile * 2 + par) * p.dot_ld + row] = dot;
-        if (kPhaseTiming && p.dbg != nullptr && blockIdx.x == 0 && lane == 0 && cw == 0 && acc_iter < 16) {
-          long long* d = p.dbg + 64 + acc_iter * 4;   // [tile][fragment stores, rest of the epilogue, of which scratch reads, start stamp]
-          d[0] = t_frag; d[1] = phase_clock() - tm1 - t_frag; d[2] = t_ld; d[3] = tm1;
-        }
       } else {
         // ====== fp32 epilogue: split-K partials (MN-major kernels) or biased fp32 output ======
         float* base = p.part + size_t(split) * p.part_stride;

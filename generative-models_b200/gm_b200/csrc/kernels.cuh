@@ -469,29 +469,24 @@ __global__ void dh_kernel(const __nv_bfloat16* __restrict__ a, const float* __re
 }
 
 // ---------------------------------------------------------------- gradient penalty (WGAN-GP, DRAGAN)
-// xhat rows (bf16, ld, zero pad, NO ones column: the penalty has no bias gradient):
-//   mode 0 (src/w_gp_gan.py:197-201): xhat = eps*x + (1-eps)*fake,  eps ~ U[0,1) per row
-//   mode 1 (src/dra_gan.py:200-205):  xhat = delta*x + (1-delta)*(x + std*u), delta per row, u per element
-// rnd == nullptr: on-device Philox (row stream), else caller tensors: eps[rows] or
-// delta[rows] followed by u[rows*x].  stats: [0] sum x, [1] sum x^2 over the real rows.
-__global__ void xhat_kernel(const __nv_bfloat16* __restrict__ xr, const __nv_bfloat16* __restrict__ xf,
-                            __nv_bfloat16* __restrict__ out, int rows, int x, int ld, int mode,
+// DRAGAN's xhat rows (src/dra_gan.py:200-205, bf16, ld, zero pad, ones column at x: they carry a true backward path):
+//   xhat = delta*x + (1-delta)*(x + std*u), delta per row, u per element
+// rnd == nullptr: on-device Philox (row stream), else caller tensors: delta[rows] followed by u[rows*x].
+// stats: [0] sum x, [1] sum x^2, [2] count over the real rows.
+__global__ void xhat_kernel(const __nv_bfloat16* __restrict__ xr, __nv_bfloat16* __restrict__ out, int rows, int x, int ld,
                             const float* __restrict__ rnd, const float* __restrict__ stats,
                             unsigned long long seed, unsigned long long stream_id, float dra_c, long long lo_off,
                             const unsigned long long* __restrict__ step_ptr) {
   griddep_sync();
   if (step_ptr) stream_id += 2ull * (*step_ptr);
   // One warp per row, lanes walk the row's 16-byte groups (coalesced, unlike a thread-per-row
-  // mapping).  Philox: the row's eps / delta comes from subsequence r (lane-uniform),
-  // DRAGAN's per-element u from subsequence rows + r * groups + g.
+  // mapping).  Philox: the row's delta comes from subsequence r (lane-uniform), the per-element
+  // u from subsequence rows + r * groups + g.
   const int groups = ld / 8;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  float sd = 0.f;
-  if (mode == 1) {
-    const double n = stats[2], s1 = stats[0], s2 = stats[1];
-    sd = dra_c * float(sqrt(fmax((s2 - s1 * s1 / n) / (n - 1.0), 0.0)));   // C * images.std(): unbiased, global (src/dra_gan.py:204-205)
-  }
+  const double n = stats[2], s1 = stats[0], s2 = stats[1];
+  const float sd = dra_c * float(sqrt(fmax((s2 - s1 * s1 / n) / (n - 1.0), 0.0)));   // C * images.std(): unbiased, global (src/dra_gan.py:204-205)
   for (int r = w; r < rows; r += nwarps) {
     float e;
     if (rnd) e = rnd[r];
@@ -502,10 +497,9 @@ __global__ void xhat_kernel(const __nv_bfloat16* __restrict__ xr, const __nv_bfl
     }
     for (int g = lane; g < groups; g += 32) {
       const int c0 = g * 8;
-      float va[8], vb[8], v[8], u[8];
+      float va[8], v[8], u[8];
       load_bf16x8(xr + (long long)r * ld + c0, va, lo_off);
-      if (mode == 0) load_bf16x8(xf + (long long)r * ld + c0, vb, lo_off);
-      else if (rnd == nullptr && c0 < x) {
+      if (rnd == nullptr && c0 < x) {
         curandStatePhilox4_32_10_t su;
         curand_init(seed ^ 0x9E3779B97F4A7C15ull, (unsigned long long)rows + (unsigned long long)r * groups + g, stream_id * 256ull, &su);
         const float4 a = curand_uniform4(&su), b = curand_uniform4(&su);
@@ -514,13 +508,10 @@ __global__ void xhat_kernel(const __nv_bfloat16* __restrict__ xr, const __nv_bfl
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = c0 + j;
-        float o = (c == x && mode == 1) ? 1.f : 0.f;   // DRAGAN xhat rows carry a true backward path -> ones column
+        float o = c == x ? 1.f : 0.f;
         if (c < x) {
-          if (mode == 0) o = e * va[j] + (1.f - e) * vb[j];
-          else {
-            const float uu = rnd ? rnd[rows + (long long)r * x + c] : u[j];
-            o = e * va[j] + (1.f - e) * (va[j] + sd * uu);
-          }
+          const float uu = rnd ? rnd[rows + (long long)r * x + c] : u[j];
+          o = e * va[j] + (1.f - e) * (va[j] + sd * uu);
         }
         v[j] = o;
       }
@@ -534,7 +525,8 @@ __global__ void xhat_kernel(const __nv_bfloat16* __restrict__ xr, const __nv_bfl
 // their share of the D-layer GEMM are never formed.  From the stored pre-activations of the real and fake rows (bf16, or
 // hi + lo planes in split mode) one warp per row writes what the penalty needs (SURVEY A.2): U = w2 * relu'(a_hat) (the first
 // gradient's operand, bf16 [+ residual plane]) and the logit part s = sum_n w2[n] relu(a_hat[n]) into slot 0 of the row's
-// logit slots (the other slots are zeroed; b2 is added by the reader).  eps: rnd[r] or the same Philox draw as xhat_kernel.
+// logit slots (the other slots are zeroed; b2 is added by the reader).  eps: rnd[r], or curand_uniform from Philox
+// subsequence r of seed ^ 0x9E3779B97F4A7C15 at offset stream_id * 256.
 constexpr int kGpHatGroups = 2;    // 16-byte column groups per lane: ld <= 512 columns
 __global__ void gp_hat_kernel(const __nv_bfloat16* __restrict__ pre_r, const __nv_bfloat16* __restrict__ pre_f, const float* __restrict__ w2,
                               __nv_bfloat16* __restrict__ U, float* __restrict__ slots, int nslots, int slot_ld, int rows, int h, int ld,

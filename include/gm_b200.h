@@ -476,9 +476,6 @@ long long gm_launch_count(gm_ctx* ctx, int reset);
 int gm_prof_enable(gm_ctx* ctx, int on);   /* 0 off, 1 GEMM launches by kind (gm_prof_collect), 2 every launch by name (gm_prof_report) */
 /* level-2 report: synchronises and writes "name,launches,total_ms" lines (in first-launch order) into buf; returns bytes needed */
 int gm_prof_report(gm_ctx* ctx, char* buf, int buflen);
-/* debug aid: CTA 0 of following gm_gemm_bf16 launches writes per-tile phase durations
- * (SM clocks) into dbg_dev (128 int64); pass NULL to stop. */
-int gm_debug_phase_buffer(gm_ctx* ctx, long long* dbg_dev);
 int gm_prof_collect(gm_ctx* ctx, double* ms4, double* flops4, long long* count4);
 
 #ifdef __cplusplus
