@@ -145,11 +145,12 @@ static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 gri
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int BN, bool AMN, bool BMN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false>
+template <int BN, bool AMN, bool BMN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false,
+          bool PP = false>
 static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
-  using Cfg = GemmCfg<BN, !AMN>;
+  using Cfg = GemmCfg<BN, !AMN, PP>;
   constexpr int CL = kGemmCluster<BN, AMN, BMN>;
-  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, ACT_T, AUX_T, BIAS_T, DOT_T, SPLIT>;
+  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, ACT_T, AUX_T, BIAS_T, DOT_T, SPLIT, PP>;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3(pl.grid);
@@ -211,6 +212,8 @@ static cudaError_t launch_split(const GemmPlan& pl, cudaStream_t s) {
   return launch_inst<BN, AMN, BMN, -1, -1, -1, -1, true>(pl, s);
 }
 
+constexpr int kPingPongMaxKblocks = 7;   // K <= 448
+
 // K-major 128x208 kernel: pick the compile-time-specialised epilogue when the plan's
 // fused-epilogue combination is one of the train step's, else the universal variant.
 static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
@@ -219,8 +222,16 @@ static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
   const int aux = p.aux_mode;
   if (p.epi != EPI_BF16) return launch_inst<208, false, false>(pl, s);
   if (p.dot_sq && (bias || dot || aux != AUX_NONE || p.act != ACT_NONE)) return launch_inst<208, false, false>(pl, s);
-  if (bias && !dot && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0>(pl, s);
-  if (bias && !dot && aux == AUX_NONE && p.act == ACT_SIGMOID) return launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0>(pl, s);
+  // Short-K bias + activation GEMMs (G's two layers) are epilogue-bound: their consumer warpgroups run in ping-pong, so
+  // each half-tile's epilogue hides under the other warpgroup's wgmma.  Ping-pong loads the B tile once per 64-row half;
+  // from 8 k-blocks on, and with aux / row-dot epilogues, that extra feed cost more than it hid (DESIGN §5).
+  const bool pp = p.kblocks <= kPingPongMaxKblocks;
+  if (bias && !dot && aux == AUX_NONE && p.act == ACT_RELU)
+    return pp ? launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0, false, true>(pl, s)
+              : launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0>(pl, s);
+  if (bias && !dot && aux == AUX_NONE && p.act == ACT_SIGMOID)
+    return pp ? launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0, false, true>(pl, s)
+              : launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0>(pl, s);
   if (bias && dot && p.dot_mask == 1 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 3>(pl, s);
   if (bias && dot && p.dot_mask == 3 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 5>(pl, s);
   if (p.dot_mask) return launch_inst<208, false, false>(pl, s);
@@ -308,11 +319,13 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
                      int ldb, int ncover, int max_splits) {
   memset(pl, 0, sizeof *pl);
   if (M <= 0 || N <= 0 || K <= 0) return fail(c, GM_ERR_ARG, "gemm: bad extents %d %d %d", M, N, K);
-  int bn, boxn = 0;
+  int bn, boxn = 0, boxm = BM;
   if (mode == 0) {
     if (ncover <= 64) { pl->kind = PK_NT_64; bn = 64; boxn = 64; }
-    else { pl->kind = PK_NT_208; bn = 208; boxn = 208 / kGemmCluster<208, false, false>; }   // each CTA's share of the B tile
-    int rc = make_tmap(c, &pl->tmA, A, K, M, lda, BK, BM);
+    else {   // each CTA's share of the B tile; 64-row A boxes
+      pl->kind = PK_NT_208; bn = 208; boxn = 208 / kGemmCluster<208, false, false>; boxm = kGemmABoxRows<208, false>;
+    }
+    int rc = make_tmap(c, &pl->tmA, A, K, M, lda, BK, boxm);
     if (rc) return rc;
     rc = make_tmap(c, &pl->tmB, B, K, N, ldb, BK, boxn);
     if (rc) return rc;
@@ -339,7 +352,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     const __nv_bfloat16* B2 = static_cast<const __nv_bfloat16*>(B) + c->plan_lo;
     int rc;
     if (mode == 0) {
-      if ((rc = make_tmap(c, &pl->tmA2, A2, K, M, lda, BK, BM))) return rc;
+      if ((rc = make_tmap(c, &pl->tmA2, A2, K, M, lda, BK, boxm))) return rc;
       if ((rc = make_tmap(c, &pl->tmB2, B2, K, N, ldb, BK, boxn))) return rc;
     } else {
       if ((rc = make_tmap(c, &pl->tmA2, A2, M, K, lda, 64, BK))) return rc;

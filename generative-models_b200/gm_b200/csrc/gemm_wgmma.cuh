@@ -18,7 +18,10 @@
 // the per-row epilogue; the scratch is then reused as the bf16 staging of the store.  Meanwhile
 // the producer keeps filling the smem ring with the next tile's operands.  Pipelines: smem ring
 // full/empty mbarriers (TMA <-> wgmma), static round-robin tile scheduler (grid = #SMs).  The 128 x 208
-// K-major kernel runs as 2-CTA clusters that share the B tile (kGemmCluster).
+// K-major kernel runs as 2-CTA clusters that share the B tile (kGemmCluster).  Its PINGPONG instances, launched for
+// short-K GEMMs with a plain bias + activation epilogue, run the two consumer warpgroups in ping-pong: each runs its 64
+// rows of a tile as a half-item of its own, the mainloops take turns through two named barriers, and each warpgroup's
+// epilogue runs under the other one's wgmma.  A ring stage then holds one half-item's 64 A rows and the whole B tile.
 #pragma once
 #include "ptx.cuh"
 
@@ -30,6 +33,9 @@ constexpr int kMmaK = 16;
 constexpr int kProducerThreads = 128;                               // warpgroup 0: TMA producer
 constexpr int kConsumerWarps = 8;                                   // warpgroups 1..2: wgmma, then the epilogue
 constexpr int kGemmThreads = kProducerThreads + kConsumerWarps * 32;
+// named barriers of the ping-pong mainloop handoff (0 is __syncthreads'; the kernel uses no other)
+constexpr int kBarWg0Issued = 1;
+constexpr int kBarWg1Issued = 2;
 // setmaxnreg budget: 384 threads launch with 168 registers each; the producer drops to 40 so the consumers can hold a
 // 128 x 208 (or 256) fp32 accumulator next to the epilogue's registers
 constexpr int kProducerRegs = 40;
@@ -105,10 +111,18 @@ constexpr int kEpiVecBytes = kEpiVecBlocks * kEpiCols * 4 * 2;   // bias + row-d
 static_assert(kEpiRows * kEpiPitch <= kEpiScratchBytes && 2 * kEpiRows * kEpiCols * 2 <= kEpiScratchBytes, "staging");
 __device__ __forceinline__ uint32_t frag_swz(int r) { return uint32_t(((r & 3) << 1) | ((r >> 2) & 1)); }
 
-template <int BN_, bool STAGED_EPI = true>
+// K-major A tiles of the 128 x 208 kernel arrive as 64-row TMA boxes: one per stage in ping-pong, two otherwise
+template <int BN, bool A_MN>
+constexpr int kGemmABoxRows = (BN == 208 && !A_MN) ? BM / 2 : BM;
+
+template <int BN_, bool STAGED_EPI = true, bool PINGPONG_ = false>
 struct GemmCfg {
   static constexpr int BN = BN_;
-  static constexpr int A_BYTES = BM * BK * 2;
+  // ping-pong (128 x 208 K-major only): a stage holds the A rows of one 64-row half of the tile
+  static constexpr bool PINGPONG = PINGPONG_;
+  static_assert(!PINGPONG || (STAGED_EPI && BN == 208), "ping-pong: 128 x 208 K-major kernel only");
+  static constexpr int A_ROWS = PINGPONG ? BM / 2 : BM;
+  static constexpr int A_BYTES = A_ROWS * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // per-warp scratch / staging tile (+ per-warp copies of the tile's bias / row-dot weights in the K-major kernels)
@@ -122,6 +136,8 @@ struct GemmCfg {
   static_assert(BN % 16 == 0 && BN <= 256, "wgmma N constraint (and 16-column epilogue chunks)");
   static_assert(STAGES >= 2, "need a pipeline");
   static_assert(BN < 208 || STAGES >= 4, "the 208- and 256-wide kernels need a 4-stage ring to hide TMA latency");
+  // 5 x 34 816 + 50 688 = 224 768 B
+  static_assert(!PINGPONG || (STAGES == 5 && SMEM_BYTES <= kSmemBudget), "ping-pong ring");
 };
 
 // CTAs per cluster.  The 128 x 208 K-major kernel runs as 2-CTA clusters on adjacent m-tiles of one n-tile: both read
@@ -133,16 +149,21 @@ constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 2 : 1;
 // Epilogue specialisation: ACT_T / AUX_T / BIAS_T / DOT_T >= 0 fix the fused epilogue at
 // compile time (small code: the whole kernel must stay inside the instruction cache);
 // -1 selects the universal variant that reads the choice from GemmParams at run time.
-template <int BN, bool A_MN, bool B_MN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false>
+// PINGPONG: the consumer warpgroups run the 64-row halves of each tile as half-items of their own (see the consumer loop)
+template <int BN, bool A_MN, bool B_MN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false,
+          bool PINGPONG = false>
 // 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
   static_assert(!SPLIT || ACT_T < 0, "split operands: universal epilogue only");
-  using Cfg = GemmCfg<BN, !A_MN>;
+  using Cfg = GemmCfg<BN, !A_MN, PINGPONG>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int CL = kGemmCluster<BN, A_MN, B_MN>;
+  constexpr bool PP = PINGPONG;
+  constexpr int A_BOX = kGemmABoxRows<BN, A_MN>;
+  static_assert(Cfg::A_ROWS % A_BOX == 0, "A tile in whole boxes");
   static_assert(!B_MN || BN % 64 == 0, "MN-major B needs 64-wide atoms");
   // each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for one box
   static_assert(CL == 1 || (!B_MN && (BN / CL) % 8 == 0 && (Cfg::B_BYTES / CL) % 1024 == 0), "multicast B share");
@@ -165,8 +186,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (p.tma_store) tma_prefetch_desc(&tmC);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      // every consumer warp of every CTA in the cluster releases the slot: the peers' multicasts also write it
-      mbar_init(empty_bar(s), CL * kConsumerWarps);
+      // every consumer warp that reads the slot, in every CTA of the cluster, releases it: the peers' multicasts also
+      // write it.  In ping-pong one warpgroup per CTA reads a slot.
+      mbar_init(empty_bar(s), CL * (PP ? kConsumerWarps / 2 : kConsumerWarps));
     }
     fence_mbar_init();
   }
@@ -183,6 +205,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int tiles = (p.m_tiles + CL - 1) / CL * p.n_tiles;
   const int total = tiles * p.splits;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
+  // Ping-pong: an item is two half-items, rows [0, 64) for consumer warpgroup 0 and [64, 128) for warpgroup 1, whose
+  // k-blocks enter the ring one half after the other.  The second half is skipped in both CTAs of the cluster when rank
+  // 0's first row of it is past M (rank 1's rows are higher still), so the peers keep walking the same k-blocks.
+  auto halves_of = [&](int rem) -> int {
+    if constexpr (PP) return (rem / p.n_tiles) * CL * BM + Cfg::A_ROWS < p.M ? 2 : 1;
+    else return 1;
+  };
+  // A k-block's stage and phase follow from the running count `it` of k-blocks issued, in (item, half-item, k-block)
+  // order: stage it % STAGES, phase (it / STAGES) & 1.  Ping-pong consumers derive them from the count at each item,
+  // which they also advance past the other warpgroup's half; the cooperative consumers read every k-block and just carry
+  // stage and phase along.
+  auto stage_of = [](uint32_t it) { return int(it % STAGES); };
+  auto phase_of = [](uint32_t it) { return (it / STAGES) & 1u; };
 
   if (warp < kProducerThreads / 32) {
     // =========================== TMA producer ===========================
@@ -190,8 +225,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // uniform registers); one elected lane issues.  Warps 1..3 only release their registers.
     setmaxnreg_dec<kProducerRegs>();
     if (warp == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      uint32_t it = 0;
       const bool leader = elect_one();
       for (int item = first; item < total; item += stride) {
         const int split = item / tiles;
@@ -200,8 +234,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int n0 = (rem % p.n_tiles) * BN;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+        const int nh = halves_of(rem);
+        for (int h = 0; h < nh; ++h)
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const int stage = stage_of(it);
+          mbar_wait(empty_bar(stage), phase_of(it) ^ 1u);
           if (leader) {
             const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
             const uint32_t b_dst = a_dst + Cfg::A_BYTES;
@@ -212,7 +249,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const int k0 = kk * BK;
             mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
             if constexpr (!A_MN) {
-              tma_load_2d(a_dst, ta, full_bar(stage), k0, m0);
+#pragma unroll
+              for (int a = 0; a < Cfg::A_ROWS / A_BOX; ++a)
+                tma_load_2d(a_dst + a * (A_BOX * BK * 2), ta, full_bar(stage), k0, m0 + h * Cfg::A_ROWS + a * A_BOX);
             } else {
 #pragma unroll
               for (int a = 0; a < BM / 64; ++a)
@@ -229,7 +268,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
           }
           __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
@@ -310,6 +348,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     };
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t it = 0;   // ping-pong: the producer's running k-block count, advanced past the other warpgroup's halves too
 #pragma unroll 1
     for (int item = first; item < total; item += stride) {
       const int split = item / tiles;
@@ -319,12 +358,33 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int n0 = n_tile * BN;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
+      const int nh = halves_of(rem);
+      if constexpr (PP) {
+        // Warpgroup g runs half-item g of every item.  The mainloops take turns: warpgroup 1 issues its first wgmma of an
+        // item only after warpgroup 0 has issued all of its wgmmas of that item (named barrier kBarWg0Issued), and
+        // warpgroup 0 starts the next item only after warpgroup 1 has issued its half (kBarWg1Issued), so each
+        // warpgroup's epilogue runs while the other warpgroup's mainloop keeps the tensor pipe busy.  A skipped second
+        // half passes the turn straight back.  Every item's turn is handed over exactly once each way, except that
+        // warpgroup 0 waits for none before this CTA's first item and warpgroup 1 hands none back after its last.
+        if (wg == 1 || it != 0) named_bar_sync(wg == 1 ? kBarWg0Issued : kBarWg1Issued, kConsumerWarps * 32);
+        if (wg == 1 && nh == 1) {
+          it += uint32_t(kb1 - kb0);
+          if (item + stride < total) named_bar_arrive(kBarWg1Issued, kConsumerWarps * 32);
+          continue;
+        }
+      }
       // ---------------- mainloop: one wgmma group in flight, the slot it read is released one k-block later
       int prev = -1;
+      if constexpr (PP) {
+        const uint32_t it0 = it + (wg == 1 ? uint32_t(kb1 - kb0) : 0u);
+        stage = stage_of(it0);
+        phase = phase_of(it0);
+        it += uint32_t(nh * (kb1 - kb0));
+      }
 #pragma unroll 1
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(full_bar(stage), phase);
-        const uint32_t a_src = smem_base + stage * Cfg::STAGE_BYTES + wg * A_WG_OFF;
+        const uint32_t a_src = smem_base + stage * Cfg::STAGE_BYTES + (PP ? 0u : wg * A_WG_OFF);
         const uint32_t b_src = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
         const uint32_t a_lo = ((a_src >> 4) & 0x3FFFu) | ((A_LBO >> 4) << 16);
         const uint32_t b_lo = ((b_src >> 4) & 0x3FFFu) | ((B_LBO >> 4) << 16);
@@ -346,6 +406,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (prev >= 0) release(prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      if constexpr (PP) {
+        if (wg == 0 || item + stride < total) named_bar_arrive(wg == 0 ? kBarWg0Issued : kBarWg1Issued, kConsumerWarps * 32);
       }
       wgmma_wait<0>();
       wgmma_pin(acc);
