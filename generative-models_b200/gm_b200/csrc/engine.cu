@@ -145,12 +145,11 @@ static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 gri
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int BN, bool AMN, bool BMN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false,
-          bool PP = false>
+template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false>
 static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
   using Cfg = GemmCfg<BN, !AMN, PP>;
   constexpr int CL = kGemmCluster<BN, AMN, BMN>;
-  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, ACT_T, AUX_T, BIAS_T, DOT_T, SPLIT, PP>;
+  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP>;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3(pl.grid);
@@ -209,41 +208,39 @@ static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
 // split-operand plans (gm_prec GM_PREC_SPLIT): the universal epilogue with the residual-plane paths compiled in
 template <int BN, bool AMN, bool BMN>
 static cudaError_t launch_split(const GemmPlan& pl, cudaStream_t s) {
-  return launch_inst<BN, AMN, BMN, -1, -1, -1, -1, true>(pl, s);
+  return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(pl, s);
 }
 
 constexpr int kPingPongMaxKblocks = 7;   // K <= 448
 
-// K-major 128x208 kernel: pick the compile-time-specialised epilogue when the plan's
-// fused-epilogue combination is one of the train step's, else the universal variant.
+// K-major 128x208 kernel: the compile-time-specialised instance of the plan's epilogue signature when the train steps use
+// that signature, else the universal instance.
 static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
   const GemmParams& p = pl.p;
-  const bool bias = p.bias != nullptr, dot = p.dot_w != nullptr;
-  const int aux = p.aux_mode;
   if (p.epi != EPI_BF16) return launch_inst<208, false, false>(pl, s);
-  if (p.dot_sq && (bias || dot || aux != AUX_NONE || p.act != ACT_NONE)) return launch_inst<208, false, false>(pl, s);
   // Short-K bias + activation GEMMs (G's two layers) are epilogue-bound: their consumer warpgroups run in ping-pong, so
   // each half-tile's epilogue hides under the other warpgroup's wgmma.  Ping-pong loads the B tile once per 64-row half;
   // from 8 k-blocks on, and with aux / row-dot epilogues, that extra feed cost more than it hid (DESIGN §5).
   const bool pp = p.kblocks <= kPingPongMaxKblocks;
-  if (bias && !dot && aux == AUX_NONE && p.act == ACT_RELU)
-    return pp ? launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0, false, true>(pl, s)
-              : launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 0>(pl, s);
-  if (bias && !dot && aux == AUX_NONE && p.act == ACT_SIGMOID)
-    return pp ? launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0, false, true>(pl, s)
-              : launch_inst<208, false, false, ACT_SIGMOID, AUX_NONE, 1, 0>(pl, s);
-  if (bias && dot && p.dot_mask == 1 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 3>(pl, s);
-  if (bias && dot && p.dot_mask == 3 && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 5>(pl, s);
-  if (p.dot_mask) return launch_inst<208, false, false>(pl, s);
-  if (bias && dot && aux == AUX_NONE && p.act == ACT_RELU) return launch_inst<208, false, false, ACT_RELU, AUX_NONE, 1, 1>(pl, s);
-  if (!bias && !dot && aux == AUX_SIGMOID_GRAD && p.act == ACT_NONE) return launch_inst<208, false, false, ACT_NONE, AUX_SIGMOID_GRAD, 0, 0>(pl, s);
-  if (!bias && !dot && aux == AUX_RELU_MASK && p.act == ACT_NONE) return launch_inst<208, false, false, ACT_NONE, AUX_RELU_MASK, 0, 0>(pl, s);
-  if (!bias && !dot && aux == AUX_NONZERO_MASK && p.act == ACT_NONE) return launch_inst<208, false, false, ACT_NONE, AUX_NONZERO_MASK, 0, 0>(pl, s);
-  if (bias && !dot && aux == AUX_L1 && p.act == ACT_NONE) return launch_inst<208, false, false, ACT_NONE, AUX_L1, 1, 0>(pl, s);
-  if (bias && !dot && aux == AUX_VAE_OUT && p.act == ACT_SIGMOID) return launch_inst<208, false, false, ACT_SIGMOID, AUX_VAE_OUT, 1, 0>(pl, s);
-  if (!bias && !dot && aux == AUX_NONE && p.act == ACT_NONE && p.dot_sq) return launch_inst<208, false, false, ACT_NONE, AUX_NONE, 0, 2>(pl, s);
-  if (!bias && !dot && aux == AUX_NONE && p.act == ACT_NONE) return launch_inst<208, false, false, ACT_NONE, AUX_NONE, 0, 0>(pl, s);
-  return launch_inst<208, false, false>(pl, s);
+#define NT208(S) case S: return launch_inst<208, false, false, S>(pl, s)
+#define NT208_PINGPONG(S) case S: return pp ? launch_inst<208, false, false, S, false, true>(pl, s) : launch_inst<208, false, false, S>(pl, s)
+  switch (epi_sig(p)) {
+    NT208_PINGPONG(epi_sig(ACT_RELU, AUX_NONE, true, DOT_NONE));
+    NT208_PINGPONG(epi_sig(ACT_SIGMOID, AUX_NONE, true, DOT_NONE));
+    NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W));
+    NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W_MASK));
+    NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W_PRE));
+    NT208(epi_sig(ACT_NONE, AUX_NONE, false, DOT_NONE));
+    NT208(epi_sig(ACT_NONE, AUX_NONE, false, DOT_SQ));
+    NT208(epi_sig(ACT_NONE, AUX_SIGMOID_GRAD, false, DOT_NONE));
+    NT208(epi_sig(ACT_NONE, AUX_RELU_MASK, false, DOT_NONE));
+    NT208(epi_sig(ACT_NONE, AUX_NONZERO_MASK, false, DOT_NONE));
+    NT208(epi_sig(ACT_NONE, AUX_L1, true, DOT_NONE));
+    NT208(epi_sig(ACT_SIGMOID, AUX_VAE_OUT, true, DOT_NONE));
+    default: return launch_inst<208, false, false>(pl, s);
+  }
+#undef NT208
+#undef NT208_PINGPONG
 }
 
 static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
@@ -253,8 +250,7 @@ static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
     pl.tmc_state = 2;
     // the bulk store serves the pure activation epilogues only; the aux / row-dot epilogues keep LDS + STG
     // (a fence + wait for the bulk store would sit in their longer per-block dependency chain)
-    const bool plain = p.aux_mode == AUX_NONE && p.dot_w == nullptr && p.dot_sq == 0;
-    if (g_tma_store && nt && plain && p.nparts == 1 && p.epi == EPI_BF16 && p.out != nullptr && !(reinterpret_cast<uintptr_t>(p.out) & 15) &&
+    if (g_tma_store && nt && epi_plain(p.aux_mode, p.dot) && p.nparts == 1 && p.epi == EPI_BF16 && p.out != nullptr && !(reinterpret_cast<uintptr_t>(p.out) & 15) &&
         (p.ldo * 2) % 16 == 0 && p.out_cols > 0) {
       int rc = make_tmap(c, &pl.tmC, p.out, uint64_t(p.out_cols), uint64_t(p.M), uint64_t(p.ldo), kEpiCols, kEpiRows, CU_TENSOR_MAP_SWIZZLE_64B);
       if (rc) return rc;
@@ -266,15 +262,16 @@ static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   ProfAll pa;
   if (g_prof_all) {
     static const char* kKind[4] = {"gemm_nt208", "gemm_nt64", "gemm_tn256", "gemm_tn64"};
-    static std::map<int, std::string> names;   // interned: kind + epilogue signature
+    static std::map<int, std::string> names;   // interned: epilogue signature + kind, output type, K class, split
     const GemmParams& q = pl.p;
-    const int key = pl.kind | (q.act << 4) | (q.aux_mode << 8) | ((q.dot_w != nullptr) << 12) | (q.dot_sq << 14) |
-                    ((q.bias != nullptr) << 15) | ((q.epi == EPI_F32) << 16) | ((q.K >= 512) << 17) | ((q.nparts == 3) << 18) | (q.dot_mask << 19);
+    const bool f32 = q.epi == EPI_F32, klong = q.K >= 512, split = q.nparts == 3;
+    const int key = epi_sig(q) | (pl.kind | f32 << 2 | klong << 3 | split << 4) << kEpiSigBits;
     auto it = names.find(key);
     if (it == names.end()) {
       char buf[128];
-      snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kKind[pl.kind], q.act, q.aux_mode, q.bias ? " bias" : "", q.dot_w ? " dot" : "",
-               q.dot_mask == 3 ? " pre" : (q.dot_mask ? " mask" : ""), q.dot_sq ? " sq" : "", q.epi == EPI_F32 ? " f32" : "", q.K >= 512 ? "long" : "short", q.nparts == 3 ? " split" : "");
+      snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kKind[pl.kind], q.act, q.aux_mode, q.bias ? " bias" : "",
+               dot_has_w(q.dot) ? " dot" : "", q.dot == DOT_W_PRE ? " pre" : (q.dot == DOT_W_MASK ? " mask" : ""),
+               q.dot == DOT_SQ ? " sq" : "", f32 ? " f32" : "", klong ? "long" : "short", split ? " split" : "");
       it = names.emplace(key, buf).first;
     }
     pa.name = it->second.c_str();
@@ -539,6 +536,7 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
     p.aux = static_cast<const __nv_bfloat16*>(d->aux_dev);
     p.ld_aux = d->ld_aux;
     p.aux_mode = d->aux_mode;
+    p.dot = d->dot_w_dev ? DOT_W : DOT_NONE;
     p.dot_w = d->dot_w_dev;
     p.dot_out = d->dot_out_dev;
     p.dot_ld = d->dot_ld;
@@ -949,9 +947,15 @@ extern "C" int gm_gan_materialize_grads(gm_gan* g, gm_stream stream) {
   return GM_OK;
 }
 
+// epilogue setters for a plan fresh from plan_gemm (every other field zero)
 static void set_bf16_epi(GemmParams& p, __nv_bfloat16* out, int ldo, int out_cols, int pad_one, const float* bias, int act) {
   p.epi = EPI_BF16; p.out = out; p.ldo = ldo; p.out_cols = out_cols; p.pad_one = pad_one; p.bias = bias; p.act = act;
-  p.aux = nullptr; p.aux_mode = AUX_NONE; p.dot_w = nullptr; p.dot_out = nullptr; p.dot_sq = 0; p.row_scale = nullptr; p.row_split = 0; p.dot_mask = 0; p.row_vec = nullptr;
+}
+static void set_f32_epi(GemmParams& p, float* part, int ldp, long long part_stride, int transpose, const float* bias) {
+  p.epi = EPI_F32; p.part = part; p.ldp = ldp; p.part_stride = part_stride; p.transpose = transpose; p.bias = bias;
+}
+static void set_row_dot(GemmParams& p, int dot, const float* w, float* out, int ld) {
+  p.dot = dot; p.dot_w = w; p.dot_out = out; p.dot_ld = ld;
 }
 
 static int build_plans(gm_gan* g, int B, StepPlans** out) {
@@ -979,27 +983,23 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
   const int nfwd = g->d.variant == GM_DRA ? 3 : 2;      // DRAGAN also scores the interpolated rows
   if ((rc = plan_gemm(c, &sp.d1_d, 0, nfwd * B, H, X, g->Xall, XP, g->W1d_s, X, H, 1))) return rc;
   set_bf16_epi(sp.d1_d.p, g->Aall, HP, H, 0, pD + g->D.off_b1, ACT_RELU);
-  sp.d1_d.p.dot_w = pD + g->D.off_w2; sp.d1_d.p.dot_out = g->slots; sp.d1_d.p.dot_ld = slot_ld;
-  if (g->d.variant == GM_WGP) {
-    // WGAN-GP: the real / fake rows keep their PRE-activations (ReLU inside the row-dot and in dh_kernel): gp_hat_kernel
-    // forms a_hat = eps a(x) + (1-eps) a(G(z)) from them
-    sp.d1_d.p.dot_mask = 3;
-  }
+  // WGAN-GP: the real / fake rows keep their PRE-activations (ReLU inside the row-dot and in dh_kernel): gp_hat_kernel
+  // forms a_hat = eps a(x) + (1-eps) a(G(z)) from them
+  set_row_dot(sp.d1_d.p, g->d.variant == GM_WGP ? DOT_W_PRE : DOT_W, pD + g->D.off_w2, g->slots, slot_ld);
   if ((rc = plan_gemm(c, &sp.d1_g, 0, B, H, X, Xfake, XP, g->W1d_s, X, H, 1))) return rc;
   set_bf16_epi(sp.d1_g.p, Afake, HP, H, 0, pD + g->D.off_b1, ACT_RELU);
-  sp.d1_g.p.dot_w = pD + g->D.off_w2; sp.d1_g.p.dot_out = g->slots + B; sp.d1_g.p.dot_ld = slot_ld;
   // the G step does not update D: instead of the hidden activations it stores M = w2 * 1[a1 > 0]
   // (what dL/dfake = ds * (M W1d) needs) and so skips the dh pass over the fake rows
-  sp.d1_g.p.dot_mask = g->d.variant != GM_BEGAN;
+  set_row_dot(sp.d1_g.p, g->d.variant != GM_BEGAN ? DOT_W_MASK : DOT_W, pD + g->D.off_w2, g->slots + B, slot_ld);
   // D layer 1 on the real rows only (inference: gm_gan_discriminate)
   if ((rc = plan_gemm(c, &sp.d1_x, 0, B, H, X, g->Xall, XP, g->W1d_s, X, H, 1))) return rc;
   set_bf16_epi(sp.d1_x.p, g->Aall, HP, H, 0, pD + g->D.off_b1, ACT_RELU);
-  sp.d1_x.p.dot_w = pD + g->D.off_w2; sp.d1_x.p.dot_out = g->slots; sp.d1_x.p.dot_ld = slot_ld;
+  set_row_dot(sp.d1_x.p, DOT_W, pD + g->D.off_w2, g->slots, slot_ld);
   // dW1d^T (+ db1 row from the ones column): [X+1, H] = Xall^T DHall over 2B rows
   if ((rc = plan_gemm(c, &sp.dw1d, 1, X + 1, H, g->nreg * B, g->Xall, XP, g->DHall, HP, H, g->max_splits))) return rc;
   {
-    GemmParams& p = sp.dw1d.p;
-    p.epi = EPI_F32; p.part = g->PD; p.ldp = p.m_tiles * BM; p.part_stride = (long long)H * p.ldp; p.transpose = 1;
+    const int ldp = sp.dw1d.p.m_tiles * BM;
+    set_f32_epi(sp.dw1d.p, g->PD, ldp, (long long)H * ldp, 1, nullptr);
     sp.dw1d.flops = 2.0 * X * H * (double(g->nreg) * B);
   }
   if (g->nreg > 2) {
@@ -1008,7 +1008,7 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
     __nv_bfloat16* Rrows = g->Xall + rreg * XP;
     if ((rc = plan_gemm(c, &sp.gp_v, 0, B, X, H, g->DHall + rreg * HP, HP, g->W1d_t, H, X, 1))) return rc;
     set_bf16_epi(sp.gp_v.p, Rrows, XP, X, 0, nullptr, ACT_NONE);
-    sp.gp_v.p.dot_sq = 1; sp.gp_v.p.dot_out = g->slots_v; sp.gp_v.p.dot_ld = g->Bmax;
+    set_row_dot(sp.gp_v.p, DOT_SQ, nullptr, g->slots_v, g->Bmax);
     if ((rc = plan_gemm(c, &sp.gp_t, 0, B, H, X, Rrows, XP, g->W1d_s, X, H, 1))) return rc;
     set_bf16_epi(sp.gp_t.p, g->DHg, HP, H, 0, nullptr, ACT_NONE);
     // T = coef * (V W1^T) * relu'(a_hat): the per-row factor of R = coef V is applied in the epilogue (R itself is never
@@ -1023,22 +1023,16 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
   sp.dx.p.row_vec = g->ds + B;     // dL/ds of the fake rows (launch_loss, G step)
   // [dW2g | db2g] = DA2^T [Hg | 1]
   if ((rc = plan_gemm(c, &sp.dw2g, 1, X, H + 1, B, g->DA2, XP, g->Hg, HP, H + 1, g->max_splits))) return rc;
-  {
-    GemmParams& p = sp.dw2g.p;
-    p.epi = EPI_F32; p.part = g->PG2; p.ldp = rup(H + 1, 64); p.part_stride = (long long)X * p.ldp; p.transpose = 0;
-    sp.dw2g.flops = 2.0 * X * H * B;
-  }
+  set_f32_epi(sp.dw2g.p, g->PG2, rup(H + 1, 64), (long long)X * rup(H + 1, 64), 0, nullptr);
+  sp.dw2g.flops = 2.0 * X * H * B;
   // DHg = (DA2 W2g) * 1[Hg > 0]
   if ((rc = plan_gemm(c, &sp.dhg, 0, B, H, X, g->DA2, XP, g->W2g_t, X, H, 1))) return rc;
   set_bf16_epi(sp.dhg.p, g->DHg, HP, H, 0, nullptr, ACT_NONE);
   sp.dhg.p.aux = g->Hg; sp.dhg.p.ld_aux = HP; sp.dhg.p.aux_mode = AUX_RELU_MASK;
   // [dW1g | db1g] = DHg^T [Zb | 1]
   if ((rc = plan_gemm(c, &sp.dw1g, 1, H, Z + 1, B, g->DHg, HP, g->Zb, ZP, Z + 1, g->max_splits))) return rc;
-  {
-    GemmParams& p = sp.dw1g.p;
-    p.epi = EPI_F32; p.part = g->PG1; p.ldp = rup(Z + 1, 64); p.part_stride = (long long)H * p.ldp; p.transpose = 0;
-    sp.dw1g.flops = 2.0 * H * Z * B;
-  }
+  set_f32_epi(sp.dw1g.p, g->PG1, rup(Z + 1, 64), (long long)H * rup(Z + 1, 64), 0, nullptr);
+  sp.dw1g.flops = 2.0 * H * Z * B;
   if (g->d.variant == GM_BEGAN) {
     const int slr = 2 * g->Bmax;
     auto l1 = [&](GemmPlan& pl, const __nv_bfloat16* aux, float* slots, const float* rs, int split) {
@@ -1052,8 +1046,8 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
     set_bf16_epi(sp.be_dec_d.p, g->DR, XP, X, 0, pD + g->D.off_b2, ACT_NONE);
     l1(sp.be_dec_d, g->Xall, g->slots_r, g->be_state + 1, B);
     if ((rc = plan_gemm(c, &sp.be_gwd, 1, X, H + 1, 2 * B, g->DR, XP, g->Aall, HP, H + 1, g->max_splits))) return rc;
-    { GemmParams& p = sp.be_gwd.p; p.epi = EPI_F32; p.part = g->PWd; p.ldp = rup(H + 1, 64); p.part_stride = (long long)X * p.ldp; p.transpose = 0;
-      sp.be_gwd.flops = 2.0 * X * H * 2.0 * B; }
+    set_f32_epi(sp.be_gwd.p, g->PWd, rup(H + 1, 64), (long long)X * rup(H + 1, 64), 0, nullptr);
+    sp.be_gwd.flops = 2.0 * X * H * 2.0 * B;
     if ((rc = plan_gemm(c, &sp.be_de_d, 0, 2 * B, H, X, g->DR, XP, g->Wd_t, X, H, 1))) return rc;
     set_bf16_epi(sp.be_de_d.p, g->DHall, HP, H, 0, nullptr, ACT_NONE);
     sp.be_de_d.p.aux = g->Aall; sp.be_de_d.p.ld_aux = HP; sp.be_de_d.p.aux_mode = AUX_RELU_MASK;
@@ -1075,18 +1069,17 @@ static int build_plans(gm_gan* g, int B, StepPlans** out) {
     if ((rc = plan_gemm(c, &sp.q1, 0, B, H, X, Xfake, XP, g->Wq1_s, X, HP, 1))) return rc;
     set_bf16_epi(sp.q1.p, g->HQ, HP, HP, 1, pQ + g->Qn.off_b1, ACT_RELU);
     if ((rc = plan_gemm(c, &sp.q2, 0, B, QO, H, g->HQ, HP, g->Wq2_s, H, QO, 1))) return rc;
-    sp.q2.p.epi = EPI_F32; sp.q2.p.part = g->INF; sp.q2.p.ldp = 32; sp.q2.p.part_stride = 0; sp.q2.p.transpose = 0;
-    sp.q2.p.bias = pQ + g->Qn.off_b2;
+    set_f32_epi(sp.q2.p, g->INF, 32, 0, 0, pQ + g->Qn.off_b2);
     if ((rc = plan_gemm(c, &sp.gq2, 1, QO, H + 1, B, g->DINF, 64, g->HQ, HP, H + 1, g->max_splits))) return rc;
-    { GemmParams& p = sp.gq2.p; p.epi = EPI_F32; p.part = g->PQ2; p.ldp = 448; p.part_stride = (long long)64 * 448; p.transpose = 0;
-      sp.gq2.flops = 2.0 * QO * H * B; }
+    set_f32_epi(sp.gq2.p, g->PQ2, 448, (long long)64 * 448, 0, nullptr);
+    sp.gq2.flops = 2.0 * QO * H * B;
     if ((rc = plan_gemm(c, &sp.dhq, 0, B, H, rup(QO, 16), g->DINF, 64, g->Wq2_t, 64, H, 1))) return rc;
     set_bf16_epi(sp.dhq.p, g->DHQ, HP, H, 0, nullptr, ACT_NONE);
     sp.dhq.p.aux = g->HQ; sp.dhq.p.ld_aux = HP; sp.dhq.p.aux_mode = AUX_RELU_MASK;
     sp.dhq.flops = 2.0 * B * H * QO;
     if ((rc = plan_gemm(c, &sp.gq1, 1, H, X + 1, B, g->DHQ, HP, Xfake, XP, X + 1, g->max_splits))) return rc;
-    { GemmParams& p = sp.gq1.p; p.epi = EPI_F32; p.part = g->PQ1; p.ldp = rup(p.N, 64); p.part_stride = (long long)H * p.ldp; p.transpose = 0;
-      sp.gq1.flops = 2.0 * H * X * B; }
+    set_f32_epi(sp.gq1.p, g->PQ1, rup(X + 1, 64), (long long)H * rup(X + 1, 64), 0, nullptr);
+    sp.gq1.flops = 2.0 * H * X * B;
     if ((rc = plan_gemm(c, &sp.dfq, 0, B, X, H, g->DHQ, HP, g->Wq1_t, H, X, 1))) return rc;
     set_bf16_epi(sp.dfq.p, g->DA2, XP, X, 0, nullptr, ACT_NONE);
     sp.dfq.p.aux = Xfake; sp.dfq.p.ld_aux = XP; sp.dfq.p.aux_mode = AUX_SIGMOID_GRAD;

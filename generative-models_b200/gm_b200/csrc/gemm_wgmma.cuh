@@ -47,6 +47,25 @@ enum : int { EPI_BF16 = 0, EPI_F32 = 1 };
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2, ACT_LRELU = 3 };   // LeakyReLU(act_slope): universal epilogue only
 // AUX_NONZERO_MASK: like AUX_RELU_MASK for an aux that holds the SIGNED mask form w2 * relu'(a) (nonzero <=> active unit)
 enum : int { AUX_NONE = 0, AUX_SIGMOID_GRAD = 1, AUX_RELU_MASK = 2, AUX_VAE_OUT = 3, AUX_L1 = 4, AUX_NONZERO_MASK = 5 };
+// Row-dot of the stored values v into dot_out: DOT_W sum v * dot_w[n], DOT_SQ sum v * v.  DOT_W_MASK: as DOT_W, but
+// stores dot_w[n] * 1[v > 0] instead of v (the G step needs only M = w2 * relu'(a1) of D's hidden layer: dL/dx =
+// ds * (M W1), src/ns_gan.py:57-60 backward).  DOT_W_PRE: sum relu(v) * dot_w[n], and the PRE-activation v is stored
+// (WGAN-GP's D forward, which never forms the x_hat rows: the penalty's mask is 1[eps pre_real + (1-eps) pre_fake > 0])
+enum : int { DOT_NONE = 0, DOT_W = 1, DOT_SQ = 2, DOT_W_MASK = 3, DOT_W_PRE = 4 };
+__host__ __device__ constexpr bool dot_has_w(int dot) { return dot == DOT_W || dot == DOT_W_MASK || dot == DOT_W_PRE; }
+
+// Epilogue signature: (act, aux, bias, dot) packed into one int.  It is the kernel's EPI template argument, which fixes
+// the fused epilogue at compile time (small code: the whole kernel must stay inside the instruction cache);
+// kEpiUniversal selects the universal instance, which reads the epilogue from GemmParams at run time.
+constexpr int kEpiUniversal = -1;
+__host__ __device__ constexpr int epi_sig(int act, int aux, bool bias, int dot) { return act | aux << 2 | int(bias) << 5 | dot << 6; }
+constexpr int kEpiSigBits = 9;
+__host__ __device__ constexpr int epi_act(int sig) { return sig & 3; }
+__host__ __device__ constexpr int epi_aux(int sig) { return (sig >> 2) & 7; }
+__host__ __device__ constexpr bool epi_bias(int sig) { return (sig >> 5) & 1; }
+__host__ __device__ constexpr int epi_dot(int sig) { return sig >> 6; }
+// plain epilogues (no aux input, no row-dot) may store their bf16 output through the TMA-store path
+__host__ __device__ constexpr bool epi_plain(int aux, int dot) { return aux == AUX_NONE && dot == DOT_NONE; }
 
 struct GemmParams {
   int M, N, K;          // logical extents; K counts contraction elements
@@ -63,18 +82,11 @@ struct GemmParams {
   const __nv_bfloat16* aux;  // nullable, same [m, n] indexing, ld = ld_aux
   int ld_aux;
   int aux_mode;
-  const float* dot_w;   // nullable: row-dot of the *stored* values with dot_w[n]
-  int dot_sq;           // 1: dot_out = row sum of squares instead (dot_w unused)
   // AUX_L1 (BEGAN): out = sign(v - aux) * (row < row_split ? row_scale[0] : row_scale[1]), dot_out = sum |v - aux|
   const float* row_scale;
   int row_split;
-  // dot_mask, with the row-dot:
-  //   0: store v
-  //   1 (DOT_T 3): store dot_w[n] * 1[v > 0] instead of v (the G step needs only M = w2 * relu'(a1) of D's hidden
-  //      layer: dL/dx = ds * (M W1), src/ns_gan.py:57-60 backward)
-  //   3 (DOT_T 5; WGAN-GP's D forward, which never forms the x_hat rows): the row-dot runs on relu(v) but the
-  //      PRE-activation v is stored (the penalty's mask is 1[eps pre_real + (1-eps) pre_fake > 0], gp_hat_kernel)
-  int dot_mask;
+  int dot;              // DOT_*: row-dot of the stored values
+  const float* dot_w;   // its weights (DOT_W, DOT_W_MASK, DOT_W_PRE)
   // tma_store: full 32-column blocks of the bf16 output leave through the output tensor map
   // (cp.async.bulk.tensor store of the warp's swizzled staging tile) instead of LDS + STG
   int tma_store;
@@ -96,6 +108,8 @@ struct GemmParams {
   long long lo_off;
   float act_slope;      // ACT_LRELU
 };
+
+inline int epi_sig(const GemmParams& p) { return epi_sig(p.act, p.aux_mode, p.bias != nullptr, p.dot); }
 
 // Epilogue of one consumer warp: 16 rows (its fragments) x 64-column steps, one 32-column block per lane and step.
 // Its scratch tile holds a step's fp32 fragments (16-byte chunks of row r XOR-swizzled by frag_swz(r): conflict-free
@@ -146,18 +160,16 @@ struct GemmCfg {
 template <int BN, bool A_MN, bool B_MN>
 constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 2 : 1;
 
-// Epilogue specialisation: ACT_T / AUX_T / BIAS_T / DOT_T >= 0 fix the fused epilogue at
-// compile time (small code: the whole kernel must stay inside the instruction cache);
-// -1 selects the universal variant that reads the choice from GemmParams at run time.
+// EPI: the fused epilogue's signature (epi_sig), or kEpiUniversal.
 // PINGPONG: the consumer warpgroups run the 64-row halves of each tile as half-items of their own (see the consumer loop)
-template <int BN, bool A_MN, bool B_MN, int ACT_T = -1, int AUX_T = -1, int BIAS_T = -1, int DOT_T = -1, bool SPLIT = false,
-          bool PINGPONG = false>
+template <int BN, bool A_MN, bool B_MN, int EPI = kEpiUniversal, bool SPLIT = false, bool PINGPONG = false>
 // 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
-  static_assert(!SPLIT || ACT_T < 0, "split operands: universal epilogue only");
+  constexpr bool kUniversal = EPI == kEpiUniversal;
+  static_assert(!SPLIT || kUniversal, "split operands: universal epilogue only");
   using Cfg = GemmCfg<BN, !A_MN, PINGPONG>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int CL = kGemmCluster<BN, A_MN, B_MN>;
@@ -280,18 +292,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int par = lane >> 4;                     // epilogue: parity of this lane's 32-column block in a 64-column step
     const uint32_t scratch_s = epi_base + uint32_t(cw) * kEpiScratchBytes;
     const uint32_t vec_s = epi_base + kConsumerWarps * kEpiScratchBytes + uint32_t(cw) * kEpiVecBytes;   // K-major kernels
-    const int act = ACT_T >= 0 ? ACT_T : p.act;
-    const int aux_mode = AUX_T >= 0 ? AUX_T : p.aux_mode;
-    const bool has_bias = BIAS_T >= 0 ? (BIAS_T != 0) : (p.bias != nullptr);
-    const bool has_dot = DOT_T >= 0 ? (DOT_T == 1 || DOT_T == 3 || DOT_T == 5) : (p.dot_w != nullptr);
-    const bool store_pre = DOT_T >= 0 ? (DOT_T == 5) : (p.dot_mask == 3);   // ReLU only inside the row-dot
-    const bool mask_all = DOT_T >= 0 ? (DOT_T == 3) : (p.dot_mask == 1);
-    const bool has_sq = DOT_T >= 0 ? (DOT_T == 2) : (p.dot_sq != 0);
+    const int act = kUniversal ? p.act : epi_act(EPI);
+    const int aux_mode = kUniversal ? p.aux_mode : epi_aux(EPI);
+    const bool has_bias = kUniversal ? p.bias != nullptr : epi_bias(EPI);
+    const int dot_mode = kUniversal ? p.dot : epi_dot(EPI);
+    const bool has_dot = dot_has_w(dot_mode);
+    const bool store_pre = dot_mode == DOT_W_PRE;   // ReLU only inside the row-dot
+    const bool mask_all = dot_mode == DOT_W_MASK;
+    const bool has_sq = dot_mode == DOT_SQ;
     // The bulk store serves the plain-activation epilogues only (launch_plan), so it is compiled out of the aux / row-dot
     // instances, and out of the universal 208-wide one, which those plain epilogues never reach.  Where the store path is
     // compiled in, ptxas keeps the consumers at the launch register count (168) despite setmaxnreg: those instances spill
     // 300-370 bytes with it and none without it.
-    constexpr bool kTmaStore = !A_MN && !SPLIT && AUX_T <= 0 && DOT_T <= 0 && !(BN == 208 && ACT_T < 0);
+    constexpr bool kTmaStore = !A_MN && !SPLIT && (kUniversal ? BN != 208 : epi_plain(epi_aux(EPI), epi_dot(EPI)));
     const bool tma_st = kTmaStore && p.tma_store != 0;
     bool st_pending = false;   // a bulk store may still be reading this warp's scratch tile
     auto stage_acquire = [&]() {
@@ -416,7 +429,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int wrow0 = m0 + wg * 64 + (cw & 3) * 16;   // first row of this warp
       const int row = wrow0 + er;
       const bool row_ok = row < p.M;
-      constexpr bool kUniversal = ACT_T < 0;
       if (!A_MN && !(kUniversal && p.epi == EPI_F32)) {
         // ================= bf16 epilogue (K-major kernels) =================
         // coalesced lane mapping for aux reads / output writes: 8 lanes x 16 B = one 128-byte
@@ -429,7 +441,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         //    XOR-swizzled by row & 7 so that the row-per-lane reads are conflict-free.
         //    No registers held across the step, no STS;
         //  * otherwise: coalesced LDG into registers, transposed through the scratch tile.
-        constexpr bool kAuxAsync = (AUX_T > 0) && (DOT_T == 0) && (BIAS_T == 0);
+        constexpr bool kAuxAsync = !kUniversal && epi_aux(EPI) != AUX_NONE && epi_dot(EPI) == DOT_NONE && !epi_bias(EPI);
         const uint32_t auxt_s = vec_s;   // 16 rows x 128 B, chunks XOR-swizzled
         uint4 pre[kAuxAsync ? 1 : 4];
         auto aux_fetch = [&](int cs) {   // columns [cs, cs + 64) of the tile
@@ -565,7 +577,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
                     for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
                   }
-                } else if (ACT_T < 0 && act == ACT_LRELU) {
+                } else if (kUniversal && act == ACT_LRELU) {
 #pragma unroll
                   for (int j = 0; j < 16; ++j) v[j] = v[j] > 0.f ? v[j] : p.act_slope * v[j];
                 } else if (act == ACT_SIGMOID) {

@@ -407,7 +407,7 @@ __global__ void colsum_kernel(const float* __restrict__ part, int nparts, int ld
 __global__ void dh_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ ds,
                           const float* __restrict__ w2, __nv_bfloat16* __restrict__ dh, float* __restrict__ dw2p,
                           int rows, int h, int ld, int rows_per_iter, long long lo_off, int pre) {
-  // pre != 0: `a` holds PRE-activations (WGAN-GP's D forward, GemmParams.dot_mask == 3): relu is applied here
+  // pre != 0: `a` holds PRE-activations (WGAN-GP's D forward, GemmParams.dot == DOT_W_PRE): relu is applied here
   griddep_sync();
   extern __shared__ float sh_acc[];  // [rows_per_iter][ld]
   const int groups = ld / 8;
