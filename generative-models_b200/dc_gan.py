@@ -187,6 +187,18 @@ def pull_running_stats(eng, nets):
                     bn.running_var.copy_(run[1].cpu())
 
 
+def push_running_stats(eng, nets):
+    """the BatchNorm running statistics of the (state_dict prefix, module) pairs nets -> eng (the inverse of
+    pull_running_stats)"""
+    runs = {"G": eng.run_G, "D": eng.run_D}
+    with torch.no_grad():
+        for tag, mod in nets:
+            for i, r in runs[tag].items():
+                bn = getattr(mod, "bn%d" % (i + 1))
+                r[0].copy_(bn.running_mean)
+                r[1].copy_(bn.running_var)
+
+
 class EngineSync:
     """Parameter sync between a trainer's DcganEngine (self._engine) and its model's modules (self._nets(): (state_dict
     prefix, module) pairs); self._dirty marks module parameters newer than the engine's"""
@@ -274,7 +286,7 @@ class DCGANTrainer(EngineSync):
         if self._has_custom_step():
             return self._train_custom(num_epochs, G_lr, D_lr, D_steps)
         eng = self._engine_synced()
-        hpG, hpD = AdamHP.make(G_lr), AdamHP.make(D_lr)
+        hpG, hpD = AdamHP.make(G_lr), AdamHP.make(D_lr, clamp=self._d_clamp())
         for net in (eng.G, eng.D):                                  # fresh optimizers per train() call (src/ns_gan.py:107-110)
             net.exp_avg.zero_(); net.exp_avg_sq.zero_(); net.step = 0
         world, rank = par.world_size(), par.rank_of()
@@ -338,7 +350,7 @@ class DCGANTrainer(EngineSync):
         def after_step():
             self._dirty = True                      # the module parameters are newer than the engine's
         G_optimizer = FusedAdam(self.model.G.parameters(), lr=G_lr)
-        D_optimizer = FusedAdam(self.model.D.parameters(), lr=D_lr)
+        D_optimizer = FusedAdam(self.model.D.parameters(), lr=D_lr, clamp=self._d_clamp())
         reference_loop(self, num_epochs, G_optimizer, D_optimizer, D_steps, after_step)
         pull_running_stats(eng, self._nets())
 
@@ -351,6 +363,11 @@ class DCGANTrainer(EngineSync):
 
     def _pre_train(self, eng):
         """per-train() state of a subclass (e.g. Fisher GAN's multiplier), after the optimizers are reset"""
+
+    def _d_clamp(self):
+        """the bound c of the clamp to [-c, c] that every D Adam step of train() applies to all D parameters (WGAN's weight
+        clipping, src/w_gan.py:158,241-243); 0 = none"""
+        return 0.0
 
     def _loss(self, net, loss_val):
         return self._fused_loss([("G", self.model.G)] if net == 0 else [("D", self.model.D)], loss_val)

@@ -35,7 +35,7 @@ from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
 from gm_b200.gan_api import to_cuda
-from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats
+from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats, push_running_stats
 
 
 def _parent_of(module, what):
@@ -107,19 +107,10 @@ def _module_names(tensors, z):
     return out
 
 
-def _push_running_stats(eng, nets):
-    """the BatchNorm running statistics of the (state_dict prefix, module) pairs nets -> eng (the inverse of
-    dc_gan.pull_running_stats)"""
-    with torch.no_grad():
-        for tag, mod in nets:
-            for i, r in (eng.run_G if tag == "G" else eng.run_D).items():
-                bn = getattr(mod, "bn%d" % (i + 1))
-                r[0].copy_(bn.running_mean)
-                r[1].copy_(bn.running_var)
-
-
 class DCVAE(nn.Module):
     """ VAE super class to reconstruct an image (as src/vae.py:80-106), with conv encoder and decoder """
+    variant = "vae"                                    # the DcganEngine variant that trains this model
+    _Encoder = Encoder
 
     def __init__(self, image_size=64 * 64 * 3, hidden_dim=64, z_dim=100, channels=3):
         super().__init__()
@@ -128,7 +119,7 @@ class DCVAE(nn.Module):
         if hidden_dim % 16 or hidden_dim <= 0 or z_dim <= 0:
             raise GmError("hidden_dim must be a positive multiple of 16 and z_dim positive")
         self.__dict__.update(dict(image_size=image_size, hidden_dim=hidden_dim, z_dim=z_dim, channels=channels))
-        self.encoder = Encoder(image_size, hidden_dim, z_dim, channels)
+        self.encoder = self._Encoder(image_size, hidden_dim, z_dim, channels)
         self.decoder = Decoder(z_dim, hidden_dim, image_size, channels)
         dcgan_init(self)
         self.shape = 64
@@ -141,6 +132,14 @@ class DCVAE(nn.Module):
         """(state_dict prefix, module) of the engine's two nets: G is the decoder, D the encoder"""
         return [("G", self.decoder), ("D", self.encoder)]
 
+    def _engine_names(self, named):
+        """{"G." / "D." + module parameter name: tensor} -> the engine's names (_engine_names)"""
+        return _engine_names(named)
+
+    def _module_names(self, tensors):
+        """the inverse of the method _engine_names"""
+        return _module_names(tensors, self.z_dim)
+
     def _engine(self):
         """the trainer's engine, or - for a model without one, such as DCVAETrainer.best_model - a private engine loaded
         from this module's parameters and running statistics"""
@@ -150,9 +149,9 @@ class DCVAE(nn.Module):
         if not torch.cuda.is_available():
             raise GmError("DCVAE is not attached to a CUDA engine: there is no eager / CPU path")
         if self._own_engine is None:
-            object.__setattr__(self, "_own_engine", DcganEngine(self.hidden_dim, self.z_dim, self.channels, variant="vae"))
-        self._own_engine.load_torch_weights(_engine_names(module_params(self._nets())))
-        _push_running_stats(self._own_engine, self._nets())
+            object.__setattr__(self, "_own_engine", DcganEngine(self.hidden_dim, self.z_dim, self.channels, variant=self.variant))
+        self._own_engine.load_torch_weights(self._engine_names(module_params(self._nets())))
+        push_running_stats(self._own_engine, self._nets())
         return self._own_engine
 
     def _after_forward(self, eng, train):
@@ -166,7 +165,7 @@ class DCVAE(nn.Module):
         parameters and statistics, no link to the trainer's engine.  The new module's initialisation draws are taken on a
         forked RNG, so that copying leaves torch's random stream (the eps of later forwards) where it was."""
         with torch.random.fork_rng(devices=[]):
-            new = DCVAE(self.image_size, self.hidden_dim, self.z_dim, self.channels)
+            new = type(self)(self.image_size, self.hidden_dim, self.z_dim, self.channels)
         new.load_state_dict({k: v.detach().clone() for k, v in self.state_dict().items()})
         new.train(self.training)
         return new
@@ -210,21 +209,21 @@ class DCVAETrainer(EngineSync):
         return self.model._nets()
 
     def _sd(self):
-        return _engine_names(super()._sd())
+        return self.model._engine_names(super()._sd())
 
     def _torch_tensors(self, grads=False):
-        return _module_names(super()._torch_tensors(grads), self.model.z_dim)
+        return self.model._module_names(super()._torch_tensors(grads))
 
     def _engine_synced(self):
         m = self.model
         if self._engine is None:
-            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant="vae")
+            self._engine = DcganEngine(m.hidden_dim, m.z_dim, m.channels, variant=m.variant)
             self._dirty = self._stats_dirty = True
         if self._dirty:
             self._engine.load_torch_weights(self._sd())
             self._dirty = False
         if self._stats_dirty:
-            _push_running_stats(self._engine, self._nets())
+            push_running_stats(self._engine, self._nets())
             self._stats_dirty = False
         return self._engine
 
@@ -248,28 +247,36 @@ class DCVAETrainer(EngineSync):
             self.model.train()
             per_step = []
             for rows, n in (self._pool_batches(eng, pool, seed) if pool is not None else self._host_batches(eng)):
-                per_step.append(eng.vae_grad(rows, n, seed=seed, step=self._step).clone())
+                per_step.append(self._grad_step(eng, rows, n, seed).clone())
                 par.sum_gradients(eng.G.grads)                      # NCCL SUM (no-op on one GPU): the losses are sums
                 par.sum_gradients(eng.D.grads)
                 eng.apply(hp)
                 self._step += 1
             vals = torch.stack(per_step).tolist()
-            epoch_recon, epoch_kl = [v[0] for v in vals], [v[1] for v in vals]
-            epoch_loss = [a + b for a, b in zip(epoch_recon, epoch_kl)]
-            self.kl_loss.extend(epoch_kl)
-            self.recon_loss.extend(epoch_recon)
             self.model.eval()
             val_loss = self.evaluate(self.val_iter)
             if val_loss < self.best_val_loss:
                 self._pull()
                 self.best_model = deepcopy(self.model)
                 self.best_val_loss = val_loss
-            print("Epoch[%d/%d], Total Loss: %.4f, Reconst Loss: %.4f, KL Div: %.7f, Val Loss: %.4f"
-                  % (epoch, num_epochs, np.mean(epoch_loss), np.mean(epoch_recon), np.mean(epoch_kl), val_loss))
+            print(self._log_epoch(epoch, num_epochs, vals, val_loss))
             self.num_epochs += 1
             if self.viz:
                 self.sample_images(epoch)
         self._pull()
+
+    def _grad_step(self, eng, rows, n, seed):
+        """one train step's gradients into eng.G.grads / eng.D.grads; returns its losses (this process's sums)"""
+        return eng.vae_grad(rows, n, seed=seed, step=self._step)
+
+    def _log_epoch(self, epoch, num_epochs, vals, val_loss):
+        """keeps an epoch's per-step losses vals and returns its progress line (src/vae.py:172-187)"""
+        epoch_recon, epoch_kl = [v[0] for v in vals], [v[1] for v in vals]
+        epoch_loss = [a + b for a, b in zip(epoch_recon, epoch_kl)]
+        self.kl_loss.extend(epoch_kl)
+        self.recon_loss.extend(epoch_recon)
+        return ("Epoch[%d/%d], Total Loss: %.4f, Reconst Loss: %.4f, KL Div: %.7f, Val Loss: %.4f"
+                % (epoch, num_epochs, np.mean(epoch_loss), np.mean(epoch_recon), np.mean(epoch_kl), val_loss))
 
     def _host_batches(self, eng):
         """one epoch of train_iter: (NHWC bf16 rows, n) per batch"""

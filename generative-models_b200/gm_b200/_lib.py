@@ -138,6 +138,7 @@ def lib():
     L.gm_rows_to_image.argtypes = [vp, vp, i, i, vp, vp]
     L.gm_noise_rows.argtypes = [vp, vp, vp, i, i, i, u64, u64, vp]
     L.gm_loss_rows.argtypes = [vp, i, i, vp, i, i, f, vp, vp, vp, vp]
+    L.gm_loss_rows_c.argtypes = [vp, i, i, vp, i, i, f, C.POINTER(LossConsts), vp, vp, vp, vp]
     L.gm_gp_interp_rows.argtypes = [vp, vp, i, vp, i, i, i, i, vp, vp, u64, u64, vp, i, vp]
     L.gm_gp_penalty.argtypes = [vp, vp, i, i, i, i, f, f, f, vp, i, vp, vp, vp]
     L.gm_im2col_k4s2_lrelu_mask.argtypes = [vp, vp, i, i, i, i, i, vp, i, f, vp, i, vp]
@@ -157,6 +158,8 @@ def lib():
     L.gm_vae_latent_rows.argtypes = [vp, vp, i, vp, vp, vp, i, i, i, u64, u64, vp, vp]
     L.gm_vae_dlatent_rows.argtypes = [vp, vp, i, vp, i, vp, vp, i, i, i, f, vp]
     L.gm_bn_forward_eval.argtypes = [vp, vp, ll, i, i, vp, vp, vp, f, i, f, vp, i, vp]
+    L.gm_ae_latent_rows.argtypes = [vp, vp, i, vp, i, i, i, vp]
+    L.gm_ae_dlatent_rows.argtypes = [vp, vp, i, vp, i, vp, i, i, i, vp]
     L.gm_gan_use_device_step.argtypes = [vp, i, vp, vp]
     L.gm_gan_device_steps.argtypes = [vp, vp, vp]
     L.gm_ctx_set_pdl.argtypes = [vp, i]

@@ -671,6 +671,42 @@ __global__ void __launch_bounds__(256) sse_sigmoid_rows_kernel(const __nv_bfloat
   if (threadIdx.x == 0) part[blockIdx.x] = acc;
 }
 
+// ---- The autoencoder's ReLU code (src/ae.py:38-39) between the encoder head's fp32 rows h [rows, ldm] and the decoder.
+// One thread per (row, 8-column group of the output row), one 16-byte store; columns past z are the constant part of the
+// layout: the ones column at z and zeros (ae_latent_kernel), zeros only (ae_dlatent_kernel).
+__global__ void __launch_bounds__(256) ae_latent_kernel(const float* __restrict__ h, int ldm, __nv_bfloat16* __restrict__ zb, int ldz,
+                                                        int rows, int z) {
+  griddep_sync();
+  const int groups = ldz / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)rows * groups) return;
+  const int r = int(t / groups), c0 = int(t % groups) * 8;
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    v[j] = c < z ? fmaxf(h[(long long)r * ldm + c], 0.f) : (c == z ? 1.f : 0.f);
+  }
+  store_bf16x8(zb + (long long)r * ldz + c0, v, 0);
+}
+
+// dh = dz 1[h > 0] (0 at h == 0 and for NaN h, as torch's threshold backward) -> bf16 [rows, ld], zeros past z
+__global__ void __launch_bounds__(256) ae_dlatent_kernel(const float* __restrict__ h, int ldm, const float* __restrict__ dz, int lddz,
+                                                         __nv_bfloat16* __restrict__ out, int ld, int rows, int z) {
+  griddep_sync();
+  const int groups = ld / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)rows * groups) return;
+  const int r = int(t / groups), c0 = int(t % groups) * 8;
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    v[j] = (c < z && h[(long long)r * ldm + c] > 0.f) ? dz[(long long)r * lddz + c] : 0.f;
+  }
+  store_bf16x8(out + (long long)r * ld + c0, v, 0);
+}
+
 // Inference-mode BatchNorm2d's (mean, invstd) from the running statistics: stats[c] = running[0][c], stats[C + c] =
 // 1 / sqrt(running[1][c] + eps), in bn_finalize_kernel's layout and precision, for bn_apply_kernel
 __global__ void bn_eval_stats_kernel(const float* __restrict__ running, int C, float eps, float* __restrict__ stats) {

@@ -27,6 +27,9 @@ of src/vae.py:47-212 with conv nets) makes D the encoder - the D trunk with a li
 and G the decoder; vae_grad runs compute_batch + (recon + kl).backward() with the reparameterisation and KL
 (gm_vae_latent_rows, gm_vae_dlatent_rows) and the sum of squared errors through the sigmoid output (gm_sse_sigmoid_rows) on
 the device, and train=False forwards (model.eval()) run every BatchNorm on its running statistics (gm_bn_forward_eval).
+variant="ae" (the autoencoder of src/ae.py:38-160) is that encoder with one linear head of z outputs and the code relu(h)
+in place of the reparameterisation (gm_ae_latent_rows, gm_ae_dlatent_rows), the same decoder and loss (ae_grad).  The row
+losses mm, w, ls and f_* take LSGAN's targets ls_a, ls_b, ls_c from the engine (gm_loss_rows_c).
 
 Everything on the device is NHWC bf16 as row-major matrices [B*H*W, C]: a convolution is gm_im2col_k4s2 + one wgmma
 GEMM (gm_gemm_bf16), a transposed convolution one GEMM + gm_col2im_k4s2, BatchNorm / activations are gm_bn_* over the
@@ -223,8 +226,8 @@ class DcganEngine:
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         if hidden_dim % 16 or hidden_dim <= 0:
             raise GmError("hidden_dim (the base channel width) must be a positive multiple of 16")
-        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be", "info", "vae") and not variant.startswith("f_"):
-            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra, be, info and vae")
+        if variant not in ("ns", "mm", "w", "ls", "wgp", "ra", "fisher", "dra", "be", "info", "vae", "ae") and not variant.startswith("f_"):
+            raise GmError("the conv path supports the row-wise losses (ns, mm, w, ls, f_*), ra, fisher, wgp, dra, be, info, vae and ae")
         if embed_dim is not None and (variant != "be" or embed_dim <= 0):
             raise GmError("embed_dim is the positive embedding width of BEGAN's autoencoder D (variant='be')")
         if variant == "info":
@@ -234,10 +237,11 @@ class DcganEngine:
                 raise GmError("InfoGAN needs disc_dim >= 1 and cont_dim >= 1")
         elif disc_dim is not None or cont_dim is not None:
             raise GmError("disc_dim and cont_dim are the code widths of InfoGAN (variant='info')")
-        if variant == "vae":
-            # the VAE's encoder ends in the linear mu / log_var heads (src/vae.py:55-61)
+        if variant in ("vae", "ae"):
+            # the VAE's encoder ends in the linear mu / log_var heads (src/vae.py:55-61), the autoencoder's in the linear layer
+            # that its ReLU code follows (src/ae.py:38-39)
             if d_out_act is not None:
-                raise GmError("the VAE's encoder heads are linear; d_out_act is a discriminator option")
+                raise GmError("the %s encoder's head is linear; d_out_act is a discriminator option" % variant.upper())
             d_out_act = "none"
         elif variant == "be":
             # BEGAN's D is an autoencoder whose reconstruction is linear (src/be_gan.py:73-76)
@@ -259,6 +263,7 @@ class DcganEngine:
         self.d_bn = variant not in ("wgp", "dra")                # BatchNorm in D's layers 2-4; the penalised critics have none
         self.gp_lambda = 10.0                                    # LAMBDA of src/w_gp_gan.py:177, src/dra_gan.py:174
         self.gp_k, self.dra_c = 1.0, 1.0                         # K, C of src/dra_gan.py:174
+        self.ls_a, self.ls_b, self.ls_c = 0.0, 1.0, 1.0          # LSGAN's targets a, b, c (src/ls_gan.py:173,197)
         self.fisher = torch.tensor([0.0, 1e-6], device=self.device)   # Fisher's (LAMBDA, RHO), src/fisher_gan.py:117-118
         # stats_reduce(buf): SUM a float64 statistic buffer over the data-parallel ranks in place (RaNS / Fisher loss
         # moments, DRAGAN's image std, BEGAN's L1 sums); None on one process.  stat_batch (d_grad) is then the global batch.
@@ -289,7 +294,8 @@ class DcganEngine:
 
         self.e = z_dim if embed_dim is None else int(embed_dim)  # BEGAN's embedding width (N_h = N_z in the BEGAN paper)
         self.ep = (self.e + 15) // 16 * 16                       # embedding rows: [e | 0 pad], N of a bf16-output GEMM
-        self.mp = (2 * z_dim + 15) // 16 * 16                    # VAE encoder head rows: [mu | log_var | 0 pad]
+        # encoder head rows, the N of the fp32 row-major head GEMM: VAE [mu | log_var | 0 pad], autoencoder [h | 0 pad]
+        self.mp = ((z_dim if variant == "ae" else 2 * z_dim) + 15) // 16 * 16
         if variant == "be":
             # D = encoder (the DCGAN D trunk, l5: e outputs, zero-padded to ep rows) + decoder (the generator stack with e
             # in place of z, l1's input columns zero-padded to ep); the torch views trim the padding (_TRIM)
@@ -299,6 +305,10 @@ class DcganEngine:
             # the VAE's encoder: l5 is the mu head (rows [0, z)) stacked on the log_var head (rows [z, 2z)), zero-padded to mp
             # rows (the N of the fp32 row-major head GEMM)
             self._trim = {"D.l5.weight": 2 * z_dim}
+            d_shapes = d_stack("", self.mp)
+        elif variant == "ae":
+            # the autoencoder's encoder: l5 is the linear head of z outputs, zero-padded to mp rows
+            self._trim = {"D.l5.weight": z_dim}
             d_shapes = d_stack("", self.mp)
         else:
             self._trim = {"D.l5.weight": 1}
@@ -327,6 +337,7 @@ class DcganEngine:
         if variant == "be":
             self.began_init(0.0, 1)
         self.vae_loss = torch.zeros(2, device=self.device)       # VAE: (recon, kl) of the last vae_grad, this process's sums
+        self.ae_loss = torch.zeros(1, device=self.device)        # autoencoder: recon of the last ae_grad, this process's sum
         self._bufs = {}
         self._calls = {"d": 0, "g": 0}                           # custom_d_forward / custom_g_forward calls so far
         self._slot_gen = {"d": [0] * self.D_SLOTS, "g": [0] * self.G_SLOTS}   # the call that holds each slot
@@ -526,7 +537,7 @@ class DcganEngine:
         # D: fp32 [16, ld] with row 0 = logits (transposed store); Q and the VAE encoder: fp32 rows [n, qp] / [n, mp]; BEGAN:
         # the bf16 embedding rows [n, ep]
         gemm_bf16(flat, net.bf[pfx + "l5.weight"], logits, "nt",
-                  transpose=logits.dtype == torch.float32 and net is not self.Q and self.variant != "vae")
+                  transpose=logits.dtype == torch.float32 and net is not self.Q and self.variant not in ("vae", "ae"))
         return sv
 
     def d_backward(self, sv, ds, grads, need_wgrad=True, need_dimg=False, tag="d", pfx="", dimg_mode=C2I_SIGMOID_GRAD, net=None):
@@ -647,8 +658,9 @@ class DcganEngine:
 
     def _loss_rows(self, logits, n, g_step, inv, ds, loss):
         variant = VARIANTS[self._ROW_LOSS.get(self.variant, self.variant)]
-        check(self.h, lib().gm_loss_rows(self.h, variant, OUT_ACTS[self.d_out_act], _ptr(logits), n, g_step, inv, _ptr(ds), None,
-                                         loss, _stream()))
+        lc = _lib.LossConsts(self.gp_lambda, self.gp_k, self.dra_c, self.ls_a, self.ls_b, self.ls_c)
+        check(self.h, lib().gm_loss_rows_c(self.h, variant, OUT_ACTS[self.d_out_act], _ptr(logits), n, g_step, inv, C.byref(lc), _ptr(ds),
+                                           None, loss, _stream()))
 
     def _reduce_stats(self, buf):
         if self.stats_reduce is not None:
@@ -687,8 +699,8 @@ class DcganEngine:
         WGAN-GP: eps [n] fp32 (None = on-device Philox keyed by (seed, step)).  DRAGAN: gp_k, dra_c (None = self.gp_k,
         self.dra_c), delta [n] and u [n, ch*64*64] (the reference's NCHW-flattened layout) or None for Philox.  RaNS, Fisher
         and DRAGAN: stat_batch = the batch the statistics run over (None = n; the global batch under stats_reduce)."""
-        if self.variant == "vae":
-            raise GmError("the VAE has no D step: its train step is vae_grad")
+        if self.variant in ("vae", "ae"):
+            raise GmError("the %s has no D step: its train step is %s_grad" % (self.variant.upper(), self.variant))
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         lam = self.gp_lambda if gp_lambda is None else float(gp_lambda)
         stat_batch = n if stat_batch is None else int(stat_batch)
@@ -830,8 +842,8 @@ class DcganEngine:
 
     def g_grad(self, n, noise=None, inv_global_batch=None, seed=0, step=0):
         """train_G + backward (src/ns_gan.py:196-216,155): G gradients only."""
-        if self.variant == "vae":
-            raise GmError("the VAE has no G step: its train step is vae_grad")
+        if self.variant in ("vae", "ae"):
+            raise GmError("the %s has no G step: its train step is %s_grad" % (self.variant.upper(), self.variant))
         inv = 1.0 / n if inv_global_batch is None else inv_global_batch
         fake, gsv = self.g_forward(n, noise, seed, 2 * step + 1)
         if self.variant == "be":
@@ -845,9 +857,10 @@ class DcganEngine:
         return self.loss_buf[1]
 
     def apply(self, net, hp=None):
-        """Adam on G (net 0) or D (net 1) with hp.  The VAE's apply(hp) steps both: its one optimizer over encoder and decoder
-        (src/vae.py:139-142) is elementwise, so an Adam step per net with the same step count is that optimizer exactly."""
-        if self.variant == "vae":
+        """Adam on G (net 0) or D (net 1) with hp.  The VAE's and the autoencoder's apply(hp) steps both: their one optimizer
+        over encoder and decoder (src/vae.py:139-142, src/ae.py:98-101) is elementwise, so an Adam step per net with the same
+        step count is that optimizer exactly."""
+        if self.variant in ("vae", "ae"):
             hp = net if hp is None else hp
             self.D.adam(hp)
             self.G.adam(hp)
@@ -967,19 +980,73 @@ class DcganEngine:
         return rec, mulv[:, :self.z].clone(), mulv[:, self.z:2 * self.z].clone(), sums.float()
 
     def encode(self, images, train=True):
-        """Encoder.forward (src/vae.py:58-61): flat [n, ch*64*64] (NCHW flattened) -> (mu, log_var) fp32 [n, z]"""
-        self._vae_only("encode")
+        """Encoder.forward (src/vae.py:58-61): flat [n, ch*64*64] (NCHW flattened) -> (mu, log_var) fp32 [n, z]; the
+        autoencoder's (src/ae.py:38-39): -> the code relu(h) fp32 [n, z], the values the decoder reads (bf16)"""
         n = images.shape[0]
+        if self.variant == "ae":
+            h = self._buf("aee_h", n, self.mp, torch.float32)
+            self.d_forward(self.stage_images(images), n, h, "aee", train=train)
+            return self._ae_latent(h, n, "aee_")[:, :self.z].float()
+        self._vae_only("encode")
         mulv = self._buf("vaee_mulv", n, self.mp, torch.float32)
         self.d_forward(self.stage_images(images), n, mulv, "vee", train=train)
         return mulv[:, :self.z].clone(), mulv[:, self.z:2 * self.z].clone()
 
     def decode(self, z, train=True):
-        """Decoder.forward (src/vae.py:74-77): z [n, z] -> images flat [n, ch*64*64] (NCHW flattened) fp32"""
-        self._vae_only("decode")
+        """Decoder.forward (src/vae.py:74-77, src/ae.py:51-52): z [n, z] -> images flat [n, ch*64*64] (NCHW flattened) fp32"""
+        if self.variant != "ae":
+            self._vae_only("decode")
         n = z.shape[0]
         img, _ = self.g_forward(n, z.to(self.device, torch.float32).contiguous(), tag="vdd", train=train)
         return self.rows_to_image(img, n)
+
+    # ------------------------------------------------------------------ autoencoder (src/ae.py:38-52,147-160)
+    def _ae_only(self, what):
+        if self.variant != "ae":
+            raise GmError("%s is the autoencoder's (variant='ae')" % what)
+
+    def _ae_latent(self, h, n, tag):
+        """gm_ae_latent_rows on the encoder head's rows h [n, mp]: the decoder's bf16 input rows [n, zp] = [relu(h) | 1 | 0]"""
+        zrows = self._buf(tag + "z", n, self.zp)
+        check(self.h, lib().gm_ae_latent_rows(self.h, _ptr(h), self.mp, _ptr(zrows), self.zp, n, self.z, _stream()))
+        return zrows
+
+    def ae_grad(self, img_rows, n):
+        """compute_batch + recon.backward() (src/ae.py:147-160) for n NHWC image rows (stage_images): the encoder forward with
+        the head as fp32 rows h, the code relu(h), the decoder, recon = sum (x - out)^2 and the backward through all of them.
+        The loss is a sum, so the gradients carry scale 1 and sum exactly over data-parallel ranks.  Writes G.grads (decoder),
+        D.grads (encoder) and ae_loss[0] = recon, this process's sum."""
+        self._ae_only("ae_grad")
+        sums = self._buf("ae_sums", 1, 1, torch.float64)[0]
+        h = self._buf("ae_h", n, self.mp, torch.float32)
+        sve = self.d_forward(img_rows, n, h, "ae")
+        zrows = self._ae_latent(h, n, "ae_")
+        out, svd = self.g_forward(n, tag="ad", x_rows=zrows)
+        dpre = self._buf("ae_dpre", n * 4096, self.ch)
+        self.sse_sigmoid_rows(out, img_rows, n, 1.0, dpre, sums)
+        dz = self.g_backward(svd, dpre, need_dx=True, tag="ad", dx_dtype=torch.float32)
+        dh = self._buf("ae_dh", n, self.mp)
+        check(self.h, lib().gm_ae_dlatent_rows(self.h, _ptr(h), self.mp, _ptr(dz), dz.stride(0), _ptr(dh), self.mp, n, self.z, _stream()))
+        self.d_backward(sve, dh, self.D.grads, tag="ae")
+        self.ae_loss.copy_(sums)
+        # the step's stored tensors: the head rows, the code rows, the reconstruction, dpre, dz, the head upstream, activations
+        self.ae_saved_ = dict(h=h, zrows=zrows, out=out, dpre=dpre, dz=dz, dh=dh, sve=sve, svd=svd)
+        return self.ae_loss
+
+    def ae_forward(self, img_rows, n, train=True):
+        """Autoencoder.forward + compute_batch's loss without a backward (src/ae.py:66-67,147-160) for n NHWC image rows: (the
+        reconstruction flat [n, ch*64*64] (NCHW flattened) fp32, the code [n, z] fp32, recon fp32 [1] = sum (x - out)^2).
+        train=False runs every BatchNorm in inference mode (model.eval()); train=True takes batch statistics and updates the
+        running statistics, as torch does."""
+        self._ae_only("ae_forward")
+        sums = self._buf("aef_sums", 1, 1, torch.float64)[0]
+        h = self._buf("aef_h", n, self.mp, torch.float32)
+        self.d_forward(img_rows, n, h, "afe", train=train)
+        zrows = self._ae_latent(h, n, "aef_")
+        out, _ = self.g_forward(n, tag="afd", x_rows=zrows, train=train)
+        dpre = self._buf("aef_dpre", n * 4096, self.ch)
+        self.sse_sigmoid_rows(out, img_rows, n, 1.0, dpre, sums)
+        return self.rows_to_image(out, n), zrows[:, :self.z].float(), sums.float()
 
     # ------------------------------------------------------------------ BEGAN (src/be_gan.py:212-258)
     def began_state(self, values=None):
@@ -1094,7 +1161,7 @@ class DcganEngine:
 
     @property
     def supports_custom_loss(self):
-        return self.variant not in ("be", "info", "vae")
+        return self.variant not in ("be", "info", "vae", "ae")
 
     def _take_slot(self, kind):
         if not self.supports_custom_loss:

@@ -382,6 +382,10 @@ int gm_noise_rows(gm_ctx* ctx, const float* noise_dev, void* out_dev, int rows, 
  * or out_act outside their enums and for batch outside 1..2^30.  loss_dev[0] = loss, [1] = sum of ds (a fixed-order sum). */
 int gm_loss_rows(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, int g_step, float inv_global_batch,
                  float* ds_dev, float* d_out_dev, float* loss_dev, gm_stream stream);
+/* gm_loss_rows with the loss constants of lc (the LS targets ls_a, ls_b, ls_c; the other fields are unused here); lc NULL
+ * means the reference's defaults a = 0, b = 1, c = 1 (src/ls_gan.py:173,197), which is what gm_loss_rows runs. */
+int gm_loss_rows_c(gm_ctx* ctx, int variant, int out_act, const float* logits_dev, int batch, int g_step, float inv_global_batch,
+                   const gm_loss_consts* lc, float* ds_dev, float* d_out_dev, float* loss_dev, gm_stream stream);
 /* WGAN-GP on the batch-norm-free conv critic (src/w_gp_gan.py:197-218; gm_b200/dcgan.py sequences it).
  * x_hat = eps x_real + (1 - eps) x_fake per image over NHWC rows [B*HW, C]; eps_dev [B] fp32, or NULL for Philox U(0,1]
  * keyed by (seed, stream_id); eps_out_dev [B] (nullable) receives the eps used. */
@@ -467,6 +471,15 @@ int gm_vae_dlatent_rows(gm_ctx* ctx, const float* mulv_dev, int ldm, const float
                         int ld, int rows, int z, float scale, gm_stream stream);
 int gm_bn_forward_eval(gm_ctx* ctx, const void* x_dev, long long rows, int C, int ld, const float* gamma_dev, const float* beta_dev,
                        const float* running_dev, float eps, int act, float slope, void* y_dev, int ldy, gm_stream stream);
+/* The autoencoder (src/ae.py:38-39,147-160) on the conv path: the code is relu of the encoder head's linear output.
+ * gm_ae_latent_rows: on the head's fp32 rows h_dev [rows, ldm], zrows_dev [rows, ldz] bf16 = [relu(h) | 1 | 0 ...] (the
+ * decoder's input rows, the layout of gm_vae_latent_rows).  gm_ae_dlatent_rows: from dz_dev [rows, lddz] fp32 = dL/dcode,
+ * out_dev [rows, ld] bf16 = [dz 1[h > 0] | 0 ...] (0 at h == 0, as torch's relu backward), the upstream of the head.  Both
+ * refuse, with nothing launched: rows or z not positive, ldm / lddz below z, ldz not above z or ld below z, ldz / ld not a
+ * multiple of 8, h / dz not 4-byte or zrows / out not 16-byte aligned; GM_ERR_UNSUPPORTED for 2^31 threads or more. */
+int gm_ae_latent_rows(gm_ctx* ctx, const float* h_dev, int ldm, void* zrows_dev, int ldz, int rows, int z, gm_stream stream);
+int gm_ae_dlatent_rows(gm_ctx* ctx, const float* h_dev, int ldm, const float* dz_dev, int lddz, void* out_dev, int ld, int rows, int z,
+                       gm_stream stream);
 
 /* number of this library's kernels launched since the last call with reset != 0 */
 long long gm_launch_count(gm_ctx* ctx, int reset);
