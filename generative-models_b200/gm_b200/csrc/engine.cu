@@ -99,12 +99,14 @@ enum PlanKind { PK_NT_208 = 0, PK_NT_64, PK_TN_256, PK_TN_64 };
 struct GemmPlan {
   CUtensorMap tmA, tmB;
   CUtensorMap tmA2, tmB2;   // residual (lo) planes of the operands in split mode, else copies of tmA / tmB
+  CUtensorMap tmBt, tmB2t;  // MN-major 208-wide plans: 16-column tail boxes of tmB / tmB2 (32-byte swizzle)
   // output map of the K-major bf16 kernels (16-row x 32-column box, 64-byte swizzle), encoded at the first
   // launch because the epilogue (output pointer / leading dimension) is set after plan_gemm
   mutable CUtensorMap tmC;
   mutable int tmc_state;   // 0: not encoded yet, 1: in use, 2: output not eligible (STG path)
   GemmParams p;
   int kind;
+  int bn;         // tile width: the TN kind (PK_TN_256) runs 208- or 256-wide tiles
   int grid;
   double flops;   // algorithmic 2*M*N*K of the logical problem (no padding)
 };
@@ -114,6 +116,7 @@ struct GemmPlan {
 // statement of every kernel, after the prologue in the GEMM) until the predecessor completed.
 static bool g_pdl = true;   // GM_NO_PDL=1 turns it off (gm_ctx_create)
 static bool g_tma_store = true;   // GM_NO_TMA_STORE=1: epilogue stores through LDS + STG only
+static bool g_tn208 = true;       // GM_TN208=0: every wide TN plan takes the 256-wide tile (the previous route)
 // GM_PROF_ALL / gm_prof_enable(ctx, 2): CUDA events around EVERY launch on its stream, aggregated per kernel name by
 // gm_prof_report (in-stream durations including the launch gaps ncu's serialised per-kernel times cannot show)
 struct ProfAll { const char* name; cudaEvent_t e0, e1; };
@@ -145,11 +148,11 @@ static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 gri
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false>
+template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false,
+          int CL = kGemmCluster<BN, AMN, BMN>>
 static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
   using Cfg = GemmCfg<BN, !AMN, PP>;
-  constexpr int CL = kGemmCluster<BN, AMN, BMN>;
-  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP>;
+  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP, CL>;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3(pl.grid);
@@ -186,9 +189,10 @@ static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
     if (cached) { max_clusters[dev] = mc; configured[dev] = true; }
   }
   if (CL > 1) {
-    // persistent: one cluster per item, up to the clusters the device holds at once (a GPC may hold an odd number of SMs)
+    // persistent: one cluster per item, up to the clusters the device holds at once (a GPC may hold an odd number of SMs).
+    // K-major clusters pair m-tiles, MN-major ones n-tiles (of an even count)
     const GemmParams& q = pl.p;
-    const int items = cdiv(q.m_tiles, CL) * q.n_tiles * q.splits;
+    const int items = (BMN ? q.m_tiles * (q.n_tiles / CL) : cdiv(q.m_tiles, CL) * q.n_tiles) * q.splits;
     cfg.gridDim = dim3(CL * (items < mc ? items : mc));
   }
   if (g_pdl) {
@@ -202,7 +206,14 @@ static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
   prm.tma_store = pl.tmc_state == 1 ? 1 : 0;
   // fp32 rows take float4 stores only where every row of every split starts on 16 bytes (ldc = 30: row 1 is at byte 120)
   prm.f32_vec = prm.epi == EPI_F32 && !(reinterpret_cast<uintptr_t>(prm.part) & 15) && prm.ldp % 4 == 0 && prm.part_stride % 4 == 0;
-  return cudaLaunchKernelEx(&cfg, kern, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2, prm);
+  return cudaLaunchKernelEx(&cfg, kern, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2, pl.tmBt, pl.tmB2t, prm);
+}
+
+// TN kind: the 256-wide tile, or the 208-wide one as 2-CTA clusters over n-tile pairs (an even n-tile count, plan_gemm)
+template <bool SPLIT>
+static cudaError_t launch_tn(const GemmPlan& pl, cudaStream_t s) {
+  if (pl.bn == 256) return launch_inst<256, true, true, kEpiUniversal, SPLIT>(pl, s);
+  return launch_inst<208, true, true, kEpiUniversal, SPLIT, false, 2>(pl, s);
 }
 
 // split-operand plans (gm_prec GM_PREC_SPLIT): the universal epilogue with the residual-plane paths compiled in
@@ -261,15 +272,17 @@ static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   gm_ctx::ProfRec rec;
   ProfAll pa;
   if (g_prof_all) {
-    static const char* kKind[4] = {"gemm_nt208", "gemm_nt64", "gemm_tn256", "gemm_tn64"};
+    static const char* kKind[4] = {"gemm_nt208", "gemm_nt64", "gemm_tn", "gemm_tn64"};
     static std::map<int, std::string> names;   // interned: epilogue signature + kind, output type, K class, split
     const GemmParams& q = pl.p;
     const bool f32 = q.epi == EPI_F32, klong = q.K >= 512, split = q.nparts == 3;
-    const int key = epi_sig(q) | (pl.kind | f32 << 2 | klong << 3 | split << 4) << kEpiSigBits;
+    const int key = epi_sig(q) | (pl.kind | f32 << 2 | klong << 3 | split << 4 | (pl.bn == 208) << 5) << kEpiSigBits;
     auto it = names.find(key);
     if (it == names.end()) {
       char buf[128];
-      snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kKind[pl.kind], q.act, q.aux_mode, q.bias ? " bias" : "",
+      char kind[32];
+      snprintf(kind, sizeof kind, pl.kind == PK_TN_256 ? "%s%d" : "%s", kKind[pl.kind], pl.bn);
+      snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kind, q.act, q.aux_mode, q.bias ? " bias" : "",
                dot_has_w(q.dot) ? " dot" : "", q.dot == DOT_W_PRE ? " pre" : (q.dot == DOT_W_MASK ? " mask" : ""),
                q.dot == DOT_SQ ? " sq" : "", f32 ? " f32" : "", klong ? "long" : "short", split ? " split" : "");
       it = names.emplace(key, buf).first;
@@ -289,14 +302,14 @@ static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
     switch (pl.kind) {
       case PK_NT_208: e = launch_split<208, false, false>(pl, s); break;
       case PK_NT_64: e = launch_split<64, false, false>(pl, s); break;
-      case PK_TN_256: e = launch_split<256, true, true>(pl, s); break;
+      case PK_TN_256: e = launch_tn<true>(pl, s); break;
       default: e = launch_split<64, true, true>(pl, s); break;
     }
   } else
   switch (pl.kind) {
     case PK_NT_208: e = launch_nt208(pl, s); break;
     case PK_NT_64: e = launch_inst<64, false, false>(pl, s); break;
-    case PK_TN_256: e = launch_inst<256, true, true>(pl, s); break;
+    case PK_TN_256: e = launch_tn<false>(pl, s); break;
     default: e = launch_inst<64, true, true>(pl, s); break;
   }
   c->launches++;
@@ -327,14 +340,21 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     rc = make_tmap(c, &pl->tmB, B, K, N, ldb, BK, boxn);
     if (rc) return rc;
   } else {
-    // K (batch rows) need not be a multiple of 64: rows past the extent are TMA zero-fill
+    // K (batch rows) need not be a multiple of 64: rows past the extent are TMA zero-fill.  Wide outputs take the 208-wide
+    // tile, run as 2-CTA clusters over n-tile pairs, wherever it needs an even number of n-tiles and no more than the
+    // 256-wide one (400 and 401 columns: 416 instead of 512 computed), so tile count, split count and each output's
+    // k-block order stay those of the 256-wide tile.  An odd count keeps the 256-wide tile: unclustered, the 208-wide
+    // one slowed the DCGAN step (DESIGN §5)
+    const int n208 = cdiv(ncover, 208);
     if (ncover <= 64) { pl->kind = PK_TN_64; bn = 64; }
-    else { pl->kind = PK_TN_256; bn = 256; }
+    else { pl->kind = PK_TN_256; bn = g_tn208 && n208 % 2 == 0 && n208 <= cdiv(ncover, 256) ? 208 : 256; }
     int rc = make_tmap(c, &pl->tmA, A, M, K, lda, 64, BK);
     if (rc) return rc;
     rc = make_tmap(c, &pl->tmB, B, N, K, ldb, 64, BK);
     if (rc) return rc;
+    if (bn == 208 && (rc = make_tmap(c, &pl->tmBt, B, N, K, ldb, kTnTail, BK, CU_TENSOR_MAP_SWIZZLE_32B))) return rc;
   }
+  pl->bn = bn;
   GemmParams& p = pl->p;
   pl->flops = 2.0 * M * N * K;
   p.M = M; p.N = N; p.K = K;
@@ -342,7 +362,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
   p.n_tiles = cdiv(ncover, bn);
   p.kblocks = cdiv(K, BK);
   p.nparts = 1; p.kb_part = p.kblocks; p.lo_off = 0;
-  pl->tmA2 = pl->tmA; pl->tmB2 = pl->tmB;
+  pl->tmA2 = pl->tmA; pl->tmB2 = pl->tmB; pl->tmB2t = pl->tmBt;
   if (c->plan_lo > 0) {
     // split operands: second tensor maps on the residual planes, contraction over (hi,hi), (hi,lo), (lo,hi)
     const __nv_bfloat16* A2 = static_cast<const __nv_bfloat16*>(A) + c->plan_lo;
@@ -354,6 +374,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     } else {
       if ((rc = make_tmap(c, &pl->tmA2, A2, M, K, lda, 64, BK))) return rc;
       if ((rc = make_tmap(c, &pl->tmB2, B2, N, K, ldb, 64, BK))) return rc;
+      if (bn == 208 && (rc = make_tmap(c, &pl->tmB2t, B2, N, K, ldb, kTnTail, BK, CU_TENSOR_MAP_SWIZZLE_32B))) return rc;
     }
     p.nparts = 3; p.kblocks = 3 * p.kb_part; p.lo_off = c->plan_lo;
   }
@@ -419,6 +440,8 @@ extern "C" int gm_ctx_create(int device, gm_ctx** out) {
   g_pdl = !(np && np[0] == '1');
   const char* nts = getenv("GM_NO_TMA_STORE");
   g_tma_store = !(nts && nts[0] == '1');
+  const char* tn = getenv("GM_TN208");
+  g_tn208 = !(tn && tn[0] == '0');
   return GM_OK;
 }
 extern "C" int gm_ctx_destroy(gm_ctx* c) {

@@ -22,6 +22,8 @@
 // short-K GEMMs with a plain bias + activation epilogue, run the two consumer warpgroups in ping-pong: each runs its 64
 // rows of a tile as a half-item of its own, the mainloops take turns through two named barriers, and each warpgroup's
 // epilogue runs under the other one's wgmma.  A ring stage then holds one half-item's 64 A rows and the whole B tile.
+// The 128 x 208 MN-major kernel (split-K weight gradients of the 400- and 401-wide layers) takes B as three 64-column
+// boxes and a 16-column tail box and runs as 2-CTA clusters over n-tile pairs that share the A tile.
 #pragma once
 #include "ptx.cuh"
 
@@ -154,31 +156,48 @@ struct GemmCfg {
   static_assert(!PINGPONG || (STAGES == 5 && SMEM_BYTES <= kSmemBudget), "ping-pong ring");
 };
 
-// CTAs per cluster.  The 128 x 208 K-major kernel runs as 2-CTA clusters on adjacent m-tiles of one n-tile: both read
-// the same B tile (a slice of the weight matrix), so each CTA loads BN / 2 of its rows and multicasts them into both
-// CTAs' stage.  That cuts the bytes L2 feeds each CTA per k-block from 43 008 to 29 696, which bound the long-K mainloop.
+// CTAs per cluster (the default of the kernel's CL).  The 128 x 208 K-major kernel runs as 2-CTA clusters on adjacent
+// m-tiles of one n-tile: both read the same B tile (a slice of the weight matrix), so each CTA loads BN / 2 of its rows
+// and multicasts them into both CTAs' stage.  That cuts the bytes L2 feeds each CTA per k-block from 43 008 to 29 696,
+// which bound the long-K mainloop.  The 128 x 208 MN-major kernel is launched with CL = 2 when its n-tile count is even:
+// the two n-tiles of one (split, m-tile) read the same A tile (128 columns of the same batch rows), so each CTA loads
+// one 64-column box of it and multicasts it into both CTAs' stage (49 152 -> 34 816 bytes per CTA and k-block with the
+// 208-wide B).
 template <int BN, bool A_MN, bool B_MN>
 constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 2 : 1;
+// MN-major 208-wide B tile: three 64-column boxes (128-byte swizzle) and the last 16 columns as a box of their own
+// (32-byte swizzle, tensor map tmBt) behind them, read by an m64n192 and an m64n16 wgmma
+constexpr int kTnTail = 16;
 
 // EPI: the fused epilogue's signature (epi_sig), or kEpiUniversal.
 // PINGPONG: the consumer warpgroups run the 64-row halves of each tile as half-items of their own (see the consumer loop)
-template <int BN, bool A_MN, bool B_MN, int EPI = kEpiUniversal, bool SPLIT = false, bool PINGPONG = false>
+// CL: CTAs per cluster; with MN-major operands the cluster's CTAs take adjacent n-tiles of one m-tile.
+// tmBt / tmB2t: the 16-column tail boxes of tmB / tmB2 (MN-major 208-wide kernel only)
+template <int BN, bool A_MN, bool B_MN, int EPI = kEpiUniversal, bool SPLIT = false, bool PINGPONG = false,
+          int CL = kGemmCluster<BN, A_MN, B_MN>>
 // 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA2,
-                  const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmB2, const __grid_constant__ CUtensorMap tmBt,
+                  const __grid_constant__ CUtensorMap tmB2t, const GemmParams p) {
   constexpr bool kUniversal = EPI == kEpiUniversal;
   static_assert(!SPLIT || kUniversal, "split operands: universal epilogue only");
   using Cfg = GemmCfg<BN, !A_MN, PINGPONG>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int CL = kGemmCluster<BN, A_MN, B_MN>;
   constexpr bool PP = PINGPONG;
   constexpr int A_BOX = kGemmABoxRows<BN, A_MN>;
   static_assert(Cfg::A_ROWS % A_BOX == 0, "A tile in whole boxes");
-  static_assert(!B_MN || BN % 64 == 0, "MN-major B needs 64-wide atoms");
-  // each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for one box
-  static_assert(CL == 1 || (!B_MN && (BN / CL) % 8 == 0 && (Cfg::B_BYTES / CL) % 1024 == 0), "multicast B share");
+  // MN-major B: whole 64-column atoms, or (208) three of them and the 16-column tail
+  constexpr bool kTail = B_MN && BN == 208;
+  constexpr int B_BOXES = BN / 64;   // 64-column B boxes
+  static_assert(!B_MN || BN % 64 == 0 || kTail, "MN-major B needs 64-wide atoms");
+  static_assert(A_MN == B_MN, "one operand form per kernel");
+  // K-major: each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for
+  // one box.  MN-major: each CTA's share of the A tile is one whole 64-column box, so the A descriptor is unchanged.
+  static_assert(CL == 1 || CL == 2, "cluster size");
+  static_assert(CL == 1 || (!B_MN && (BN / CL) % 8 == 0 && (Cfg::B_BYTES / CL) % 1024 == 0) || (B_MN && kTail && BM / CL == 64),
+                "multicast share");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -195,6 +214,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if constexpr (SPLIT) { tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB2); }
+    if constexpr (kTail) { tma_prefetch_desc(&tmBt); if constexpr (SPLIT) tma_prefetch_desc(&tmB2t); }
     if (p.tma_store) tma_prefetch_desc(&tmC);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
@@ -209,12 +229,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   else __syncthreads();
   griddep_wait();     // barrier init above overlapped the previous grid's tail
 
-  // Work items walk (split, m-group, n-tile) with one item per cluster; CTA rank r of a cluster takes m-tile CL * group + r.
-  // m-tiles are rounded up to whole groups: a CTA on a tile past M loads its share of B, computes on zero-filled A rows
-  // and stores nothing (every store is guarded by row < M or clipped at the tensor extent), so both CTAs walk the same
-  // k-blocks through the ring.
+  // Work items walk (split, m-group, n-group) with one item per cluster.  K-major: CTA rank r of a cluster takes m-tile
+  // CL * group + r of the item's n-tile; m-tiles are rounded up to whole groups: a CTA on a tile past M loads its share
+  // of B, computes on zero-filled A rows and stores nothing (every store is guarded by row < M or clipped at the tensor
+  // extent), so both CTAs walk the same k-blocks through the ring.  MN-major (n_tiles a multiple of CL): rank r takes
+  // n-tile CL * group + r of the item's m-tile; both CTAs share split and m-tile, so they walk the same k-blocks too.
+  constexpr bool kPairN = CL > 1 && B_MN;
   const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
-  const int tiles = (p.m_tiles + CL - 1) / CL * p.n_tiles;
+  const int n_groups = kPairN ? p.n_tiles / CL : p.n_tiles;
+  const int tiles = (kPairN ? p.m_tiles : (p.m_tiles + CL - 1) / CL) * n_groups;
+  auto m0_of = [&](int rem) { return ((rem / n_groups) * (kPairN ? 1 : CL) + (kPairN ? 0 : rank)) * BM; };
+  auto n_tile_of = [&](int rem) { return (rem % n_groups) * (kPairN ? CL : 1) + (kPairN ? rank : 0); };
   const int total = tiles * p.splits;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
   // Ping-pong: an item is two half-items, rows [0, 64) for consumer warpgroup 0 and [64, 128) for warpgroup 1, whose
@@ -242,8 +267,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       for (int item = first; item < total; item += stride) {
         const int split = item / tiles;
         const int rem = item - split * tiles;
-        const int m0 = ((rem / p.n_tiles) * CL + rank) * BM;
-        const int n0 = (rem % p.n_tiles) * BN;
+        const int m0 = m0_of(rem);
+        const int n0 = n_tile_of(rem) * BN;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
         const int nh = halves_of(rem);
@@ -264,19 +289,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
               for (int a = 0; a < Cfg::A_ROWS / A_BOX; ++a)
                 tma_load_2d(a_dst + a * (A_BOX * BK * 2), ta, full_bar(stage), k0, m0 + h * Cfg::A_ROWS + a * A_BOX);
+            } else if constexpr (CL > 1) {   // A box r into this and the peer CTA; the full barrier expects both boxes
+              tma_load_2d_multicast(a_dst + rank * (BK * 128), ta, full_bar(stage), m0 + rank * 64, k0, (1u << CL) - 1);
             } else {
 #pragma unroll
               for (int a = 0; a < BM / 64; ++a)
                 tma_load_2d(a_dst + a * (BK * 128), ta, full_bar(stage), m0 + a * 64, k0);
             }
-            if constexpr (CL > 1) {   // rows [n0 + r BN/CL, +BN/CL) into this and the peer CTA; the full barrier expects both shares
+            if constexpr (CL > 1 && !B_MN) {   // rows [n0 + r BN/CL, +BN/CL) into this and the peer CTA; the full barrier expects both shares
               tma_load_2d_multicast(b_dst + rank * (Cfg::B_BYTES / CL), tb, full_bar(stage), k0, n0 + rank * (BN / CL), (1u << CL) - 1);
             } else if constexpr (!B_MN) {
               tma_load_2d(b_dst, tb, full_bar(stage), k0, n0);
             } else {
 #pragma unroll
-              for (int b = 0; b < BN / 64; ++b)
+              for (int b = 0; b < B_BOXES; ++b)
                 tma_load_2d(b_dst + b * (BK * 128), tb, full_bar(stage), n0 + b * 64, k0);
+              if constexpr (kTail)
+                tma_load_2d(b_dst + B_BOXES * (BK * 128), (SPLIT && opart == 1) ? &tmB2t : &tmBt, full_bar(stage), n0 + B_BOXES * 64, k0);
             }
           }
           __syncwarp();
@@ -320,6 +349,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t B_LBO = B_MN ? BK * 128 : 16, B_KADV = B_MN ? kMmaK * 128 : kMmaK * 2;
     constexpr uint32_t A_WG_OFF = A_MN ? BK * 128 : 64 * 128;   // this warpgroup's 64 rows of the A tile
     constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 30);      // SBO, 128B swizzle
+    // MN-major 16-column tail box: 32-byte rows, 32B swizzle; SBO = 8 k-rows * 32 B, LBO (next 16-column atom) unused
+    constexpr uint32_t TAIL_LBO = BK * kTnTail * 2, TAIL_KADV = kMmaK * kTnTail * 2;
+    constexpr uint32_t TAIL_DESC_HI = ((8u * kTnTail * 2) >> 4) | (3u << 30);
     constexpr int kSteps = (BN + kEpiStep - 1) / kEpiStep;
     float acc[BN / 2];
     // step s's fragments (columns [64 s, 64 s + 64), rows (lane >> 2) + {0, 8}) -> the scratch tile.  The acc index must
@@ -366,8 +398,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int item = first; item < total; item += stride) {
       const int split = item / tiles;
       const int rem = item - split * tiles;
-      const int n_tile = rem % p.n_tiles;
-      const int m0 = ((rem / p.n_tiles) * CL + rank) * BM;
+      const int n_tile = n_tile_of(rem);
+      const int m0 = m0_of(rem);
       const int n0 = n_tile * BN;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(kb0 + p.kb_per_split, p.kblocks);
@@ -401,6 +433,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint32_t b_src = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
         const uint32_t a_lo = ((a_src >> 4) & 0x3FFFu) | ((A_LBO >> 4) << 16);
         const uint32_t b_lo = ((b_src >> 4) & 0x3FFFu) | ((B_LBO >> 4) << 16);
+        const uint32_t t_lo = (((b_src + B_BOXES * (BK * 128)) >> 4) & 0x3FFFu) | ((TAIL_LBO >> 4) << 16);
         wgmma_pin(acc);
         wgmma_fence();
         // all four k-steps, also in a ragged last k-block: TMA zero-fills the operands past K
@@ -410,7 +443,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const uint64_t db = (uint64_t(DESC_HI) << 32) | (b_lo + k * (B_KADV >> 4));
           const uint32_t sc = (kb > kb0 || k > 0) ? 1u : 0u;
           if constexpr (BN == 256) wgmma_bf16_n256<A_MN, B_MN>(acc, da, db, sc);
-          else if constexpr (BN == 208) wgmma_bf16_n208<A_MN, B_MN>(acc, da, db, sc);
+          else if constexpr (kTail) {   // columns [0, 192) from the three boxes, [192, 208) from the tail box
+            const uint64_t dt = (uint64_t(TAIL_DESC_HI) << 32) | (t_lo + k * (TAIL_KADV >> 4));
+            wgmma_bf16_n192<A_MN, B_MN, 0>(acc, da, db, sc);
+            wgmma_bf16_n16<A_MN, B_MN, 96>(acc, da, dt, sc);
+          } else if constexpr (BN == 208) wgmma_bf16_n208<A_MN, B_MN>(acc, da, db, sc);
           else wgmma_bf16_n64<A_MN, B_MN>(acc, da, db, sc);
         }
         wgmma_commit();
@@ -491,8 +528,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int nitem = item + stride;
           if (nitem < total) {
             const int nrem = nitem - (nitem / tiles) * tiles;
-            const int nm0 = ((nrem / p.n_tiles) * CL + rank) * BM + wg * 64 + (cw & 3) * 16;
-            const int nn0 = (nrem % p.n_tiles) * BN;
+            const int nm0 = m0_of(nrem) + wg * 64 + (cw & 3) * 16;
+            const int nn0 = n_tile_of(nrem) * BN;
             // 16 rows x 416 B: four 128-byte lines per row
             for (int t = lane; t < kEpiRows * 4; t += 32) {
               const int r = nm0 + (t >> 2), c = nn0 + (t & 3) * 64;

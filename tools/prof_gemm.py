@@ -2,6 +2,10 @@
   g1: [65536,32(64)] x [400,64]^T  -> relu, bias, ones column   (epilogue-bound)
   d1: [131072,784]   x [400,784]^T -> relu, bias, fused row-dot (mainloop + epilogue)
   dx: [65536,400]    x [784,400]^T -> * aux(1-aux)
+and the two split-K weight gradients of the step (MN-major; the time is the GEMM kernel's alone, without the partials'
+reduction that gm_gemm_bf16 runs after it):
+  dw1d: [131072,785]^T x [131072,400] -> fp32, transposed partials (D's first layer + bias column)
+  dw2g: [65536,784]^T  x [65536,401]  -> fp32 partials (G's output layer + bias row)
 Prints CUDA-event times."""
 import os
 import sys
@@ -64,3 +68,29 @@ if "dhg" in which:
     out = torch.zeros(B, 416, device=dev, dtype=torch.bfloat16)
     t = timeit(lambda: gm_b200.gemm_bf16(A, W, out, "nt", K=784, aux=aux, aux_mode=2))
     print("dhg %.1f us  %.0f TFLOP/s" % (t, 2 * B * 400 * 784 / t / 1e6))
+
+
+def gemm_only(fn, n=5):
+    """mean time of the GEMM kernel alone (level-1 profile: events around each GEMM launch), us"""
+    for _ in range(2):
+        fn()
+    torch.cuda.synchronize()
+    gm_b200.prof_collect()
+    gm_b200.prof_enable(1)
+    for _ in range(n):
+        fn()
+    gm_b200.prof_enable(0)
+    ms = sum(r[1] for r in gm_b200.prof_collect())
+    return ms / n * 1e3
+
+
+if "dw1d" in which:
+    A, G = bf(2 * B, 800), bf(2 * B, 416, scale=0.1)
+    out = torch.zeros(400, 788, device=dev)
+    t = gemm_only(lambda: gm_b200.gemm_bf16(A, G, out, "tn", M=785, N=400, transpose=True))
+    print("dw1d %.1f us  %.0f TFLOP/s" % (t, 2 * 2 * B * 785 * 400 / t / 1e6))
+if "dw2g" in which:
+    A, G = bf(B, 800), bf(B, 416, scale=0.1)
+    out = torch.zeros(784, 448, device=dev)
+    t = gemm_only(lambda: gm_b200.gemm_bf16(A, G, out, "tn", M=784, N=401))
+    print("dw2g %.1f us  %.0f TFLOP/s" % (t, 2 * B * 784 * 401 / t / 1e6))
