@@ -5,6 +5,7 @@ Autoencoder, AutoencoderTrainer with train / compute_batch / evaluate / reconstr
 load_model and the attributes recon_loss, best_val_loss, num_epochs.  The loss follows the reference code: the sum of
 squared errors (src/ae.py:158).  Forward, loss, backward and Adam run in the sm_90a kernels behind gm_b200.AeEngine.
 """
+import weakref
 from copy import deepcopy  # noqa: F401
 
 import numpy as np
@@ -12,8 +13,58 @@ import torch
 import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
+from torch.autograd.function import once_differentiable
+
 from gm_b200 import AdamHP, AeEngine, GmError
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate, SlotRing)
+
+
+def _ring(eng, what):
+    """the engine's SlotRing of per-call Encoder / Decoder slots"""
+    rings = eng.__dict__.setdefault("rings", {})
+    if what not in rings:
+        rings[what] = SlotRing(eng.SLOTS, what)
+    return rings[what]
+
+
+class _EncoderCall(torch.autograd.Function):
+    """Encoder.forward under grad mode: the code relu(linear(x)) and its backward on the CUDA kernels
+    (AeEngine.encoder_forward / encoder_backward); autograd routes dL/dcode in and the parameter gradients out"""
+
+    @staticmethod
+    def forward(ctx, x, eng, *params):
+        ctx.slot, ctx.gen = _ring(eng, "Encoder").take()
+        ctx.eng, ctx.n = eng, x.shape[0]
+        return eng.encoder_forward(ctx.slot, x)
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, dcode):
+        if ctx.needs_input_grad[0]:
+            raise RuntimeError("the gradient with respect to the encoder's input is not computed")
+        _ring(ctx.eng, "Encoder").check(ctx.slot, ctx.gen)
+        g = ctx.eng.encoder_backward(ctx.slot, ctx.n, dcode)
+        return None, None, g["encoder.linear.weight"], g["encoder.linear.bias"]
+
+
+class _DecoderCall(torch.autograd.Function):
+    """Decoder.forward under grad mode: sigmoid(linear(code)) and its backward, with dL/dcode when the code requires grad"""
+
+    @staticmethod
+    def forward(ctx, code, eng, *params):
+        ctx.slot, ctx.gen = _ring(eng, "Decoder").take()
+        ctx.eng, ctx.n = eng, code.shape[0]
+        return eng.decoder_forward(ctx.slot, code)
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, dimages):
+        _ring(ctx.eng, "Decoder").check(ctx.slot, ctx.gen)
+        g, dcode = ctx.eng.decoder_backward(ctx.slot, ctx.n, dimages)
+        return (dcode if ctx.needs_input_grad[0] else None), None, g["decoder.linear.weight"], g["decoder.linear.bias"]
 
 
 class Encoder(nn.Module):
@@ -24,7 +75,10 @@ class Encoder(nn.Module):
         self.linear = nn.Linear(image_size, hidden_dim)
 
     def forward(self, x):
-        return _trainer_of(self, "Encoder")._ensure_engine(x.shape[0]).encode(to_cuda(x).float())
+        eng, attached = _engine_of(self, "Encoder", x.shape[0])
+        if attached and torch.is_grad_enabled():
+            return _EncoderCall.apply(to_cuda(x).float(), eng, self.linear.weight, self.linear.bias)
+        return eng.encode(to_cuda(x).float())
 
 
 class Decoder(nn.Module):
@@ -35,14 +89,22 @@ class Decoder(nn.Module):
         self.linear = nn.Linear(hidden_dim, image_size)
 
     def forward(self, encoder_output):
-        return _trainer_of(self, "Decoder")._ensure_engine(encoder_output.shape[0]).decode(to_cuda(encoder_output).float())
+        eng, attached = _engine_of(self, "Decoder", encoder_output.shape[0])
+        if attached and torch.is_grad_enabled():
+            return _DecoderCall.apply(to_cuda(encoder_output).float(), eng, self.linear.weight, self.linear.bias)
+        return eng.decode(to_cuda(encoder_output).float())
 
 
-def _trainer_of(module, what):
+def _engine_of(module, what, batch):
+    """(the engine behind an Encoder / Decoder, whether it is a trainer's): the AutoencoderTrainer's (grown on demand), or -
+    for a detached copy such as the best_model of an overridden compute_batch - the copy's private inference engine"""
     tr = getattr(module, "_owner", None)
-    if tr is None:
+    if tr is not None:
+        return tr._ensure_engine(batch), True
+    copy = module._copy_of() if getattr(module, "_copy_of", None) is not None else None
+    if copy is None:
         raise GmError(what + " is not attached to a CUDA engine yet: construct the AutoencoderTrainer first (there is no eager/CPU path)")
-    return tr
+    return copy._private_engine(batch), False
 
 
 class Autoencoder(nn.Module):
@@ -55,9 +117,32 @@ class Autoencoder(nn.Module):
         self.decoder = Decoder(hidden_dim=hidden_dim, image_size=image_size)
 
     def forward(self, x):
-        tr = _trainer_of(self.encoder, "Autoencoder")
-        out, _ = tr._ensure_engine(x.shape[0]).forward(to_cuda(x).float())
+        eng, attached = _engine_of(self.encoder, "Autoencoder", x.shape[0])
+        if attached and torch.is_grad_enabled():                # src/ae.py:63-64 on the differentiable encoder / decoder
+            return self.decoder(self.encoder(x))
+        out, _ = eng.forward(to_cuda(x).float())
         return out
+
+    def _private_engine(self, batch):
+        """the inference engine of a detached copy, loaded from the copy's own parameters on every call"""
+        eng = getattr(self, "_own_engine", None)
+        if eng is None or batch > eng.max_batch:
+            eng = AeEngine(self.image_size, self.hidden_dim, max_batch=max(batch, 64))
+            object.__setattr__(self, "_own_engine", eng)
+        eng.load({k: v.data for k, v in self.named_parameters()})
+        return eng
+
+    def __deepcopy__(self, memo):
+        """A detached copy (the reference keeps best_model = deepcopy(model), src/ae.py:134): same class, cloned parameter
+        values, no link to the trainer's engine; its encoder / decoder / forward run the inference calls on a private engine"""
+        new = Autoencoder(self.image_size, self.hidden_dim)
+        with torch.no_grad():
+            for (_, a), (_, b) in zip(new.named_parameters(), self.named_parameters()):
+                a.copy_(b.detach().cpu())
+        for mod in (new.encoder, new.decoder):
+            object.__setattr__(mod, "_copy_of", weakref.ref(new))
+        new.train(self.training)
+        return new
 
 
 class _AeLoss(torch.autograd.Function):
@@ -104,11 +189,18 @@ class AutoencoderTrainer:
             eng.exp_avg.copy_(old.exp_avg)
             eng.exp_avg_sq.copy_(old.exp_avg_sq)
             eng.steps = old.steps
+            for ring in getattr(old, "rings", {}).values():
+                ring.retire()
         self._engine, self._max_batch = eng, batch
         return eng
 
     def train(self, num_epochs, lr=1e-3, weight_decay=1e-5):
-        """ Train the autoencoder (src/ae.py:84-145): a true epoch over train_iter, losses read back once per epoch """
+        """ Train the autoencoder (src/ae.py:84-145): a true epoch over train_iter, losses read back once per epoch.  A
+        subclass's own compute_batch (README.md:31) is trained by the reference loop over the differentiable encoder /
+        decoder instead (gan_api.compute_batch_loop). """
+        if has_custom_compute_batch(self):
+            refuse_multi_rank()
+            return compute_batch_loop(self, num_epochs, lr, weight_decay, two_losses=False)
         hp = AdamHP.make(lr, weight_decay=weight_decay)
         if self._engine is not None:
             self._engine.reset_optimizer()
@@ -134,6 +226,7 @@ class AutoencoderTrainer:
         images, _ = batch
         return to_cuda(images.view(images.shape[0], -1)).float().contiguous()
 
+    @builtin_step
     def compute_batch(self, batch):
         """ Compute loss for a batch of examples (src/ae.py:147-160): .backward() delivers the gradients """
         images = self._images(batch)
@@ -144,18 +237,22 @@ class AutoencoderTrainer:
         return _AeLoss.apply(loss.detach().requires_grad_(True), loss, lambda: [(named[k], gviews[k]) for k in named])
 
     def evaluate(self, iterator):
-        """ Evaluate on a given dataset (src/ae.py:162-164) """
+        """ Evaluate on a given dataset (src/ae.py:162-164), with an overriding compute_batch as the reference does """
+        if has_custom_compute_batch(self):
+            return compute_batch_evaluate(self, iterator, two_losses=False)
         vals = []
-        for batch in iterator:
-            images = self._images(batch)
-            _, loss = self._ensure_engine(images.shape[0]).forward(images, want_loss=True)
-            vals.append(loss)
+        with torch.no_grad():
+            for batch in iterator:
+                images = self._images(batch)
+                _, loss = self._ensure_engine(images.shape[0]).forward(images, want_loss=True)
+                vals.append(loss)
         return float(torch.stack(vals).mean().item())
 
     def reconstruct_images(self, images, epoch, save=True):
         """ Reconstruct a fixed input (src/ae.py:166-195 without the plotting) """
         batch = to_cuda(images.view(images.shape[0], -1))
-        return self.model(batch).view(images.shape).squeeze()
+        with torch.no_grad():
+            return self.model(batch).view(images.shape).squeeze()
 
     def viz_loss(self):
         print("viz_loss: matplotlib is not installed")

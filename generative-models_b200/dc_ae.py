@@ -22,9 +22,9 @@ import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError  # noqa: F401
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import to_cuda, builtin_step, has_custom_compute_batch, compute_batch_evaluate
 from dc_gan import pull_running_stats
-from dc_vae import DCVAE, DCVAETrainer, Decoder, _parent_of  # noqa: F401  (Decoder: src/ae.py's surface)
+from dc_vae import DCVAE, DCVAETrainer, Decoder, _encoder_forward  # noqa: F401  (Decoder: src/ae.py's surface)
 
 
 class Encoder(nn.Module):
@@ -41,12 +41,7 @@ class Encoder(nn.Module):
         self.bn2, self.bn3, self.bn4 = (nn.BatchNorm2d(k) for k in c[1:])
 
     def forward(self, x):
-        x = to_cuda(x).float()
-        parent = _parent_of(self, "Encoder")
-        eng = parent._engine()
-        out = eng.encode(x.reshape(x.shape[0], -1), train=self.training)
-        parent._after_forward(eng, self.training)
-        return out
+        return _encoder_forward(self, x)
 
 
 class DCAutoencoder(DCVAE):
@@ -66,6 +61,8 @@ class DCAutoencoder(DCVAE):
     def forward(self, x):
         x = to_cuda(x).float()
         n = x.shape[0]
+        if torch.is_grad_enabled() and self.training:               # src/ae.py:63-64 on the differentiable encoder / decoder
+            return self.decoder(self.encoder(x))
         eng = self._engine()
         out, _, _ = eng.ae_forward(eng.stage_images(x.reshape(n, -1)), n, train=self.training)
         self._after_forward(eng, self.training)
@@ -74,6 +71,7 @@ class DCAutoencoder(DCVAE):
 
 class DCAutoencoderTrainer(DCVAETrainer):
     """ Object to hold data iterators, train the conv autoencoder (surface of src/ae.py:70-218) """
+    _two_losses = False                 # compute_batch returns one loss
 
     def _grad_step(self, eng, rows, n, seed):
         return eng.ae_grad(rows, n)
@@ -83,6 +81,7 @@ class DCAutoencoderTrainer(DCVAETrainer):
         self.recon_loss.extend(epoch_loss)
         return "Epoch[%d/%d], Train Loss: %.4f, Val Loss: %.4f" % (epoch, num_epochs, np.mean(epoch_loss), val_loss)
 
+    @builtin_step
     def compute_batch(self, batch):
         """ Compute loss for a batch of examples (src/ae.py:147-160): returns recon = sum (x - out)^2; .backward() delivers
         the engine's gradient to the module parameters """
@@ -94,7 +93,9 @@ class DCAutoencoderTrainer(DCVAETrainer):
 
     def evaluate(self, iterator):
         """ Evaluate on a given dataset (src/ae.py:162-164): the mean per-batch loss of the forward-only kernels, BatchNorm
-        in the model's mode """
+        in the model's mode; with an overriding compute_batch, its loss as the reference does """
+        if has_custom_compute_batch(self):
+            return compute_batch_evaluate(self, iterator, self._two_losses)
         eng = self._engine_synced()
         loss = []
         for batch in iterator:
@@ -108,7 +109,8 @@ class DCAutoencoderTrainer(DCVAETrainer):
     def reconstruct_images(self, images, epoch, save=True):
         """ src/ae.py:166-193 without the plotting: the reconstructions in the images' shape """
         batch = to_cuda(images.view(images.shape[0], -1))
-        return self.model(batch).view(images.shape).squeeze()
+        with torch.no_grad():
+            return self.model(batch).view(images.shape).squeeze()
 
     def viz_loss(self):
         try:

@@ -27,18 +27,8 @@ from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
-from gm_b200.gan_api import to_cuda, _FusedLoss, FusedAdam, builtin_step, reference_loop
+from gm_b200.gan_api import to_cuda, _FusedLoss, FusedAdam, builtin_step, reference_loop, first_order as _first_order
 from torch.autograd.function import once_differentiable
-
-
-def _first_order(backward):
-    """a create_graph=True backward through a conv node raises here, before the kernels run, instead of returning
-    gradients that a second differentiation would see as constants"""
-    def wrapper(ctx, *grads):
-        if torch.is_grad_enabled():
-            raise RuntimeError("the conv Generator / Discriminator nodes have no double backward (create_graph=True)")
-        return backward(ctx, *grads)
-    return wrapper
 
 
 def _grads_for(grads, tag, mod, names):

@@ -34,8 +34,10 @@ from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
-from gm_b200.gan_api import to_cuda
-from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats, push_running_stats
+from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate)
+from torch.autograd.function import once_differentiable
+from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats, push_running_stats, _grads_for, _node_args
 
 
 def _parent_of(module, what):
@@ -43,6 +45,56 @@ def _parent_of(module, what):
     if parent is None:
         raise GmError(what + " is not part of a DCVAE: construct it through DCVAE(...)")
     return parent
+
+
+class _EncoderCall(torch.autograd.Function):
+    """Encoder.forward in training mode under grad mode: the VAE's (mu, log_var) or the autoencoder's code and their
+    backward on the conv kernels (DcganEngine.custom_d_forward / custom_d_backward); autograd routes the upstream in and
+    the encoder's parameter gradients out"""
+
+    @staticmethod
+    def forward(ctx, x, parent, eng, mod, names, *params):
+        out, ctx.handle = eng.custom_d_forward(x)
+        ctx.parent, ctx.eng, ctx.mod, ctx.names = parent, eng, mod, names
+        return out
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, *dout):
+        grads, _ = ctx.eng.custom_d_backward(ctx.handle, dout if len(dout) == 2 else dout[0], ctx.needs_input_grad[0])
+        return (None, None, None, None, None, *_grads_for(ctx.parent._module_names(grads), "D", ctx.mod, ctx.names))
+
+
+class _DecoderCall(torch.autograd.Function):
+    """Decoder.forward in training mode under grad mode: the images and their backward, with dL/dz when z requires grad"""
+
+    @staticmethod
+    def forward(ctx, z, eng, mod, names, *params):
+        out, ctx.handle = eng.custom_g_forward(z)
+        ctx.eng, ctx.mod, ctx.names = eng, mod, names
+        return out
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, dimages):
+        grads, dz = ctx.eng.custom_g_backward(ctx.handle, dimages.float().contiguous(), need_dz=True)
+        return ((dz if ctx.needs_input_grad[0] else None), None, None, None, *_grads_for(grads, "G", ctx.mod, ctx.names))
+
+
+def _encoder_forward(mod, x):
+    """Encoder.forward of the VAE and the autoencoder: per-call kernels with a backward in training mode under grad mode,
+    the inference calls otherwise"""
+    x = to_cuda(x).float()
+    parent = _parent_of(mod, "Encoder")
+    eng = parent._engine()
+    if torch.is_grad_enabled() and mod.training:
+        out = _EncoderCall.apply(x.reshape(x.shape[0], -1), parent, eng, *_node_args(mod))
+    else:
+        out = eng.encode(x.reshape(x.shape[0], -1), train=mod.training)
+    parent._after_forward(eng, mod.training)
+    return out
 
 
 class Encoder(nn.Module):
@@ -60,12 +112,7 @@ class Encoder(nn.Module):
         self.log_var = nn.Conv2d(c[3], z_dim, 4, 1, 0, bias=False)
 
     def forward(self, x):
-        x = to_cuda(x).float()
-        parent = _parent_of(self, "Encoder")
-        eng = parent._engine()
-        out = eng.encode(x.reshape(x.shape[0], -1), train=self.training)
-        parent._after_forward(eng, self.training)
-        return out
+        return _encoder_forward(self, x)
 
 
 class Decoder(nn.Module):
@@ -87,7 +134,10 @@ class Decoder(nn.Module):
             z = z.view(1, -1)
         parent = _parent_of(self, "Decoder")
         eng = parent._engine()
-        out = eng.decode(z, train=self.training)
+        if torch.is_grad_enabled() and self.training:
+            out = _DecoderCall.apply(z, eng, *_node_args(self))
+        else:
+            out = eng.decode(z, train=self.training)
         parent._after_forward(eng, self.training)
         return out
 
@@ -173,6 +223,10 @@ class DCVAE(nn.Module):
     def forward(self, x):
         x = to_cuda(x).float()
         n = x.shape[0]
+        if torch.is_grad_enabled() and self.training:               # src/vae.py:94-98 on the differentiable encoder / decoder
+            mu, log_var = self.encoder(x)
+            z = self.reparameterize(mu, log_var)
+            return self.decoder(z), mu, log_var
         eng = self._engine()
         eps = torch.randn(n, self.z_dim, device=eng.device)                                # src/vae.py:104
         out, mu, lv, _ = eng.vae_forward(eng.stage_images(x.reshape(n, -1)), n, eps=eps, train=self.training)
@@ -187,6 +241,7 @@ class DCVAE(nn.Module):
 
 class DCVAETrainer(EngineSync):
     """ Object to hold data iterators, train the conv VAE (surface of src/vae.py:109-374) """
+    _two_losses = True                  # compute_batch returns (recon, kl)
 
     def __init__(self, model, train_iter, val_iter, test_iter, viz=False):
         self.model = model
@@ -230,8 +285,12 @@ class DCVAETrainer(EngineSync):
     # ------------------------------------------------------------------ reference surface
     def train(self, num_epochs, lr=1e-3, weight_decay=1e-5):
         """ Train a Variational Autoencoder (src/vae.py:127-191): a true epoch over train_iter with eps drawn on the device,
-        losses read back once per epoch, model.eval() validation, best model kept as a detached copy """
+        losses read back once per epoch, model.eval() validation, best model kept as a detached copy.  A subclass's own
+        compute_batch (README.md:31) is trained by the reference loop over the differentiable encoder / decoder instead
+        (gan_api.compute_batch_loop; train_iter is read on the host, device_dataset does not apply). """
         import torch.distributed as dist
+        if has_custom_compute_batch(self):
+            return self._train_custom(num_epochs, lr, weight_decay)
         eng = self._engine_synced()
         hp = AdamHP.make(lr, weight_decay=weight_decay)
         for net in eng.nets():                                      # a fresh optimizer per train() call (src/vae.py:139-142)
@@ -265,6 +324,15 @@ class DCVAETrainer(EngineSync):
                 self.sample_images(epoch)
         self._pull()
 
+    def _train_custom(self, num_epochs, lr, weight_decay):
+        refuse_multi_rank()
+        eng = self._engine_synced()
+        self.model.to(eng.device)                   # the reference's to_cuda(model): Adam runs on the device
+
+        def after_step():
+            self._dirty = True                      # the module parameters are newer than the engine's
+        compute_batch_loop(self, num_epochs, lr, weight_decay, self._two_losses, after_step)
+
     def _grad_step(self, eng, rows, n, seed):
         """one train step's gradients into eng.G.grads / eng.D.grads; returns its losses (this process's sums)"""
         return eng.vae_grad(rows, n, seed=seed, step=self._step)
@@ -296,6 +364,7 @@ class DCVAETrainer(EngineSync):
         images, _ = batch
         return to_cuda(images.view(images.shape[0], -1)).float().contiguous()
 
+    @builtin_step
     def compute_batch(self, batch):
         """ Compute loss for a batch of examples (src/vae.py:193-208): returns (recon, kl); (recon + kl).backward() delivers
         the engine's gradient of their sum to the module parameters (it rides on recon; kl carries none) """
@@ -314,7 +383,9 @@ class DCVAETrainer(EngineSync):
 
     def evaluate(self, iterator):
         """ Evaluate on a given dataset (src/vae.py:214-223): recon + kl per batch with the forward-only kernels, BatchNorm
-        in the model's mode """
+        in the model's mode; with an overriding compute_batch, its losses as the reference does """
+        if has_custom_compute_batch(self):
+            return compute_batch_evaluate(self, iterator, self._two_losses)
         eng = self._engine_synced()
         loss = []
         for batch in iterator:
@@ -329,13 +400,15 @@ class DCVAETrainer(EngineSync):
     def reconstruct_images(self, images, epoch, save=True):
         """ src/vae.py:225-252 without the plotting: the reconstructions in the images' shape """
         batch = to_cuda(images.view(images.shape[0], -1))
-        reconst_images, _, _ = self.model(batch)
+        with torch.no_grad():
+            reconst_images, _, _ = self.model(batch)
         return reconst_images.view(images.shape).squeeze()
 
     def sample_images(self, epoch=-100, num_images=36, save=True):
         """ Viz method 1 (src/vae.py:254-276): z ~ p(z), x ~ p(x|z) """
         z = to_cuda(torch.randn(num_images, self.model.z_dim))
-        sample = self.model.decoder(z)
+        with torch.no_grad():
+            sample = self.model.decoder(z)
         return sample.view(num_images, self.model.channels, self.model.shape, self.model.shape)
 
     def sample_interpolated_images(self):
@@ -346,7 +419,8 @@ class DCVAETrainer(EngineSync):
         out = []
         for alpha in np.linspace(0, 1, self.model.z_dim):
             z = to_cuda(float(alpha) * z1 + (1 - float(alpha)) * z2)
-            out.append(self.model.decoder(z).view(-1, self.model.channels, self.model.shape, self.model.shape))
+            with torch.no_grad():
+                out.append(self.model.decoder(z).view(-1, self.model.channels, self.model.shape, self.model.shape))
         return out
 
     def explore_latent_space(self, num_epochs=3):

@@ -125,6 +125,12 @@ def lib():
     L.gm_vae_apply.argtypes = [vp, C.POINTER(AdamHP), i, vp]
     L.gm_vae_forward.argtypes = [vp, vp, i, i, vp, u64, u64, vp, vp, vp, vp]
     L.gm_vae_decode.argtypes = [vp, vp, i, vp, vp]
+    L.gm_vae_num_slots.argtypes = [vp]
+    L.gm_vae_encoder_forward.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_vae_encoder_backward.argtypes = [vp, i, i, vp, vp, vp]
+    L.gm_vae_decoder_forward.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_vae_decoder_backward.argtypes = [vp, i, i, vp, vp, vp, vp]
+    L.gm_sigmoid_upstream_rows.argtypes = [vp, vp, vp, i, i, i, vp]
     ll = C.c_longlong
     L.gm_im2col_k4s2.argtypes = [vp, vp, i, i, i, i, i, vp, i, vp]
     L.gm_col2im_k4s2.argtypes = [vp, vp, i, i, i, i, i, vp, i, i, vp, i, f, vp]

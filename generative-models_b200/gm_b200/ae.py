@@ -130,6 +130,76 @@ class AeEngine:
         self._encode(n)
         return self.e[:n, :self.H].float()
 
+    # ------------------------------------------------------------------ per-call encoder / decoder (user-written losses)
+    # SLOTS encoder and SLOTS decoder calls keep their activations in their own buffers (allocated on first use) until their
+    # backward ran.  A backward only reads them, so a call may be back-propagated more than once (retain_graph); its scratch
+    # (da, de, gw1, gw2) is the fused step's (calls on one stream never overlap).
+    SLOTS = 2
+
+    def _slot(self, kind, slot):
+        bufs = getattr(self, "_slots_" + kind, None)
+        if bufs is None:
+            bf = dict(device=self.device, dtype=torch.bfloat16)
+            B = self.max_batch
+            if kind == "enc":       # [x | 1], [relu(h) | 1], the code relu(h) fp32
+                bufs = [(torch.zeros(B, self.XP, **bf), torch.zeros(B, self.HP, **bf),
+                         torch.zeros(B, self.H, device=self.device)) for _ in range(self.SLOTS)]
+            else:                   # [code | 1], the sigmoid output (its upstream after the backward)
+                bufs = [(torch.zeros(B, self.HP, **bf), torch.zeros(B, self.XP, **bf)) for _ in range(self.SLOTS)]
+            setattr(self, "_slots_" + kind, bufs)
+        return bufs[slot]
+
+    def slot_bytes(self):
+        """device bytes one encoder slot and one decoder slot hold"""
+        B = self.max_batch
+        return B * (2 * self.XP + 2 * self.HP + 4 * self.H), B * (2 * self.HP + 2 * self.XP)
+
+    def encoder_forward(self, slot, images):
+        """Encoder.forward (src/ae.py:36-38): images [n, x] fp32 -> the code relu(W1 x + b1) [n, h] fp32 (the bf16 values the
+        decoder reads, as encode)"""
+        n = images.shape[0]
+        if n > self.max_batch:
+            raise GmError("batch (%d) exceeds max_batch (%d)" % (n, self.max_batch))
+        xb, e, code = self._slot("enc", slot)
+        check(self.h, lib().gm_stage_images(self.h, _ptr(images.contiguous()), IMG_FMTS["f32"], None, _ptr(xb), n, self.X, self.XP, _stream()))
+        gemm_bf16(xb[:n], self.W1s, e[:n], "nt", K=self.X, bias=self.views()[NAMES[1]], act=1, pad_one=True, out_cols=self.HP)
+        code[:n].copy_(e[:n, :self.H])
+        return code[:n].clone()
+
+    def encoder_backward(self, slot, n, dcode):
+        """dcode [n, h] fp32 = dL/dcode of encoder_forward's call -> {encoder parameter name: gradient}: dh = dcode 1[h > 0]
+        (gm_ae_dlatent_rows), [dW1 | db1] = dh^T [x | 1]"""
+        xb, _, code = self._slot("enc", slot)
+        X, H = self.X, self.H
+        check(self.h, lib().gm_ae_dlatent_rows(self.h, _ptr(code), H, _ptr(dcode.float().contiguous()), H, _ptr(self.de), self.HP, n, H,
+                                               _stream()))
+        gemm_bf16(self.de[:n], xb[:n], self.gw1, "tn", M=H, N=X + 1)
+        return {NAMES[0]: self.gw1[:, :X].clone(), NAMES[1]: self.gw1[:, X].clone()}
+
+    def decoder_forward(self, slot, codes):
+        """Decoder.forward (src/ae.py:49-50): codes [n, h] fp32 -> images sigmoid(W2 code + b2) [n, x] fp32 (as decode)"""
+        n = codes.shape[0]
+        if n > self.max_batch:
+            raise GmError("batch (%d) exceeds max_batch (%d)" % (n, self.max_batch))
+        e, out = self._slot("dec", slot)
+        check(self.h, lib().gm_noise_rows(self.h, _ptr(codes.float().contiguous()), _ptr(e), n, self.H, self.HP, 0, 0, _stream()))
+        gemm_bf16(e[:n], self.W2s, out[:n], "nt", K=self.H, bias=self.views()[NAMES[3]], act=2, out_cols=self.X)
+        return out[:n, :self.X].float()
+
+    def decoder_backward(self, slot, n, dimages):
+        """dimages [n, x] fp32 = dL/d(images) of decoder_forward's call -> ({decoder parameter name: gradient}, dL/dcode [n, h]
+        fp32): the sigmoid upstream da = dimages out (1 - out) formed in scratch from the slot's out (gm_sigmoid_upstream_rows),
+        [dW2 | db2] = da^T [code | 1], dcode = da W2"""
+        e, out = self._slot("dec", slot)
+        X, H = self.X, self.H
+        da = self.da[:n]
+        da.copy_(out[:n])
+        check(self.h, lib().gm_sigmoid_upstream_rows(self.h, _ptr(dimages.float().contiguous()), _ptr(da), n, X, self.XP, _stream()))
+        gemm_bf16(da, e[:n], self.gw2, "tn", M=X, N=H + 1)
+        dcode = torch.empty(n, H, device=self.device)
+        gemm_bf16(da, self.W2t, dcode, "nt", K=X)
+        return {NAMES[2]: self.gw2[:, :H].clone(), NAMES[3]: self.gw2[:, H].clone()}, dcode
+
     def decode(self, codes):
         n = codes.shape[0]
         e = torch.zeros(n, self.HP, device=self.device, dtype=torch.bfloat16)

@@ -1156,12 +1156,13 @@ class DcganEngine:
     # drop-ins' autograd nodes (dc_gan._DcDForward / _DcGForward).  Each call keeps its saved activations in a slot of a ring,
     # D_SLOTS discriminator and G_SLOTS generator calls, allocated on first use; a backward whose slot a later call has taken
     # raises instead of reading that call's tensors.  The losses that need these are the ones whose D returns one score per
-    # image; BEGAN's autoencoder D, InfoGAN's coded input and Q and the VAE have none.
+    # image, and the VAE's and autoencoder's compute_batch, whose encoder is D's trunk and head and whose decoder is G;
+    # BEGAN's autoencoder D and InfoGAN's coded input and Q have none.
     D_SLOTS, G_SLOTS = 4, 2
 
     @property
     def supports_custom_loss(self):
-        return self.variant not in ("be", "info", "vae", "ae")
+        return self.variant not in ("be", "info")
 
     def _take_slot(self, kind):
         if not self.supports_custom_loss:
@@ -1181,19 +1182,32 @@ class DcganEngine:
     def custom_d_forward(self, images):
         """D(images) in training mode (batch statistics; the running statistics move per call, as nn.BatchNorm2d.train()):
         images [n, ch*64*64] (NCHW flattened) -> (scores [n, 1] fp32 = out_act(logits), the handle for custom_d_backward:
-        slot, generation, saved activations sv)"""
+        slot, generation, saved activations sv).  The VAE's encoder returns ((mu, log_var) [n, z] fp32, handle), the
+        autoencoder's (the code relu(h) [n, z] fp32, the bf16 values the decoder reads, handle), as encode does."""
         x = self._image_arg(images)
         n = x.shape[0]
         h = self._take_slot("d")
         tag = "cd%d" % h["slot"]
         rows = self.image_to_rows(x, dst=self._buf(tag + "x", n * 4096, self.ch))
+        if self.variant in ("vae", "ae"):
+            head = self._buf(tag + "head", n, self.mp, torch.float32)
+            h.update(n=n, sv=self.d_forward(rows, n, head, tag), head=head)
+            if self.variant == "ae":
+                return self._ae_latent(head, n, tag)[:, :self.z].float(), h
+            return (head[:, :self.z].clone(), head[:, self.z:2 * self.z].clone()), h
         logits = self._buf(tag + "logits", 16, n, torch.float32)
         h.update(n=n, sv=self.d_forward(rows, n, logits, tag), s=logits[0, :n])
         return self._out_act(h["s"].view(n, 1)), h
 
     def custom_d_backward(self, handle, dscore, need_dx):
         """dscore [n] = dL/d(score) of custom_d_forward's call -> ({"D.<name>": weight / BatchNorm gradient in torch's layout},
-        dL/d(images) [n, ch*64*64] fp32 or None).  dL/dlogit = dscore act'(s) is formed on the n logits."""
+        dL/d(images) [n, ch*64*64] fp32 or None).  dL/dlogit = dscore act'(s) is formed on the n logits.  For the VAE's
+        encoder dscore is (dL/dmu, dL/dlog_var), each [n, z], for the autoencoder's dL/dcode [n, z]; they have no dL/dx."""
+        if self.variant in ("vae", "ae"):
+            self._check_live(handle, "Encoder")
+            if need_dx:
+                raise GmError("the gradient with respect to the encoder's input is not computed")
+            return self._torch_views({"D": self._encoder_backward(handle, dscore)}), None
         self._check_live(handle, "Discriminator")
         n, s = handle["n"], handle["s"]
         d = dscore.reshape(n).to(self.device, torch.float32)
@@ -1206,6 +1220,25 @@ class DcganEngine:
         dimg = self.d_backward(handle["sv"], d.contiguous(), grads, need_dimg=need_dx, tag="cdb", dimg_mode=C2I_NONE)
         return self._torch_views({"D": grads}), (self.rows_to_image(dimg, n) if need_dx else None)
 
+    def _encoder_backward(self, handle, dhead):
+        """the head's bf16 upstream rows [n, mp] (the VAE's [dmu | dlog_var | 0] by gm_cast_bf16 into zeroed padding, the
+        autoencoder's dcode 1[h > 0] by gm_ae_dlatent_rows), then the trunk's backward -> flat D gradient"""
+        n, z, mp = handle["n"], self.z, self.mp
+        key = "cdhead%d" % handle["slot"]
+        if key not in self._bufs or self._bufs[key].shape[0] < n:
+            self._bufs[key] = torch.zeros(n, mp, device=self.device, dtype=torch.bfloat16)   # columns [2z, mp) stay zero
+        up = self._bufs[key][:n]
+        if self.variant == "ae":
+            dz = dhead.to(self.device, torch.float32).contiguous()
+            check(self.h, lib().gm_ae_dlatent_rows(self.h, _ptr(handle["head"]), mp, _ptr(dz), z, _ptr(up), mp, n, z, _stream()))
+        else:
+            for k, d in enumerate(dhead):
+                d = d.to(self.device, torch.float32).contiguous()
+                check(self.h, lib().gm_cast_bf16(self.h, _ptr(d), n, z, C.c_void_p(up.data_ptr() + 2 * k * z), mp, None, 0, _stream()))
+        grads = torch.zeros(self.D.total, device=self.device)
+        self.d_backward(handle["sv"], up, grads, tag="cdb")
+        return grads
+
     def custom_g_forward(self, noise):
         """G(noise) in training mode: noise [n, z] -> (images [n, ch*64*64] fp32, NCHW flattened; the handle for
         custom_g_backward)"""
@@ -1216,12 +1249,16 @@ class DcganEngine:
         h.update(n=n, sv=sv)
         return self.rows_to_image(img, n), h
 
-    def custom_g_backward(self, handle, dimages):
-        """dimages [n, ch*64*64] = dL/dG(z) of custom_g_forward's call -> {"G.<name>": gradient in torch's layout}.  The
-        upstream of the pre-sigmoid output, dimages G(z) (1 - G(z)), is rounded to bf16 once (gm_image_to_rows)."""
-        self._check_live(handle, "Generator")
+    def custom_g_backward(self, handle, dimages, need_dz=False):
+        """dimages [n, ch*64*64] = dL/dG(z) of custom_g_forward's call -> {"G.<name>": gradient in torch's layout}, and with
+        need_dz (the VAE's / autoencoder's decoder) also dL/dz [n, z] fp32.  The upstream of the pre-sigmoid output,
+        dimages G(z) (1 - G(z)), is rounded to bf16 once (gm_image_to_rows)."""
+        self._check_live(handle, "Decoder" if self.variant in ("vae", "ae") else "Generator")
         sv, n = handle["sv"], handle["n"]
         dpre = self.image_to_rows(dimages, sv["img"], self._buf("cgdpre", n * 4096, self.ch))
         grads = torch.zeros(self.G.total, device=self.device)
-        self.g_backward(sv, dpre, grads=grads)
-        return self._torch_views({"G": grads})
+        if not need_dz:
+            self.g_backward(sv, dpre, grads=grads)
+            return self._torch_views({"G": grads})
+        dz = self.g_backward(sv, dpre, grads=grads, need_dx=True, tag="cg", dx_dtype=torch.float32)
+        return self._torch_views({"G": grads}), dz[:, :self.zin].clone()

@@ -482,3 +482,41 @@ class VaeEngine:
         out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
         check(self.h, lib().gm_vae_decode(self.g, _ptr(z.contiguous().float()), n, _ptr(out), _stream()))
         return out
+
+    # ------------------------------------------------------------------ per-call encoder / decoder (user-written losses)
+    def num_slots(self):
+        return lib().gm_vae_num_slots(self.g)
+
+    def encoder_forward(self, slot, x):
+        """Encoder.forward on slot's buffers: x [n, image_size] fp32 -> (mu, log_var) [n, z] fp32"""
+        n = x.shape[0]
+        ml = torch.empty(n, 2 * self.z_dim, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_vae_encoder_forward(self.g, slot, _ptr(x.contiguous()), n, _ptr(ml), _stream()))
+        return ml[:, :self.z_dim], ml[:, self.z_dim:]
+
+    def encoder_backward(self, slot, n, dmu, dlog_var):
+        """-> {encoder parameter name: gradient} of encoder_forward's call on slot"""
+        grads = torch.empty_like(self.params)
+        dml = torch.cat([dmu.float(), dlog_var.float()], dim=1).contiguous()
+        check(self.h, lib().gm_vae_encoder_backward(self.g, slot, n, _ptr(dml), _ptr(grads), _stream()))
+        return {k: v for k, v in self.views(grads).items() if k.startswith("encoder.")}
+
+    def decoder_forward(self, slot, z):
+        """Decoder.forward on slot's buffers: z [n, z] fp32 -> images [n, image_size] fp32"""
+        n = z.shape[0]
+        out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_vae_decoder_forward(self.g, slot, _ptr(z.contiguous()), n, _ptr(out), _stream()))
+        return out
+
+    def decoder_backward(self, slot, n, dimages, need_dz):
+        """-> ({decoder parameter name: gradient}, dL/dz [n, z] fp32 or None) of decoder_forward's call on slot"""
+        grads = torch.empty_like(self.params)
+        dz = torch.empty(n, self.z_dim, device=self.device, dtype=torch.float32) if need_dz else None
+        check(self.h, lib().gm_vae_decoder_backward(self.g, slot, n, _ptr(dimages.float().contiguous()), _ptr(grads), _ptr(dz),
+                                                    _stream()))
+        return {k: v for k, v in self.views(grads).items() if k.startswith("decoder.")}, dz
+
+    def slot_bytes(self):
+        """device bytes one encoder slot and one decoder slot hold (allocated on the first per-call use)"""
+        XP, HP, ZP, B = (self.image_size + 16) // 16 * 16, (self.hidden_dim + 16) // 16 * 16, (self.z_dim + 64) // 64 * 64, self.max_batch
+        return 2 * B * (XP + HP) + 4 * B * 64, 2 * B * (ZP + HP + XP)

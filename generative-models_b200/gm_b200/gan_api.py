@@ -11,6 +11,7 @@ Adam is a hand-written sm_90a kernel behind the C ABI.  No autograd on the hot p
 """
 import os
 import weakref
+from copy import deepcopy
 
 import numpy as np
 import torch
@@ -182,6 +183,16 @@ def builtin_step(fn):
     return fn
 
 
+def first_order(backward):
+    """a create_graph=True backward through a CUDA node raises here, before the kernels run, instead of returning
+    gradients that a second differentiation would see as constants"""
+    def wrapper(ctx, *grads):
+        if torch.is_grad_enabled():
+            raise RuntimeError("the CUDA forward / backward nodes have no double backward (create_graph=True)")
+        return backward(ctx, *grads)
+    return wrapper
+
+
 def _split_like(flat, params):
     out, off = [], 0
     for p in params:
@@ -209,6 +220,11 @@ class _GForward(torch.autograd.Function):
         if eng.g_generation != ctx.generation:
             raise RuntimeError("Generator activations were overwritten by a later Generator.forward: "
                                "back-propagate a G output before calling G again")
+        if getattr(ctx, "consumed", False):
+            # gm_gan_g_backward turns the saved output into its upstream in place: a second pass would read that instead
+            raise RuntimeError("Generator activations were consumed by this call's first backward: a G output can be "
+                               "back-propagated once (retain_graph=True does not keep them)")
+        ctx.consumed = True
         flat = eng.g_backward(dimages.float().contiguous())
         return (None, None, *_split_like(flat, ctx.params))
 
@@ -294,6 +310,101 @@ def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step
         tr.num_epochs += 1
         if tr.viz:
             tr.generate_images(epoch)
+
+
+def has_custom_compute_batch(tr):
+    """True when tr's class overrides compute_batch (README.md:31) with a method not marked @builtin_step"""
+    return not getattr(type(tr).compute_batch, "_gm_builtin", False)
+
+
+def refuse_multi_rank():
+    """an overridden compute_batch trains on one process: refused under a process group of more than one rank"""
+    from . import parallel as par
+    if par.world_size() > 1:
+        raise GmError("an overridden compute_batch trains on one process; data-parallel training runs the built-in step")
+
+
+def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=None):
+    """The reference's train loop verbatim (src/vae.py:127-191 when compute_batch returns (recon, kl), src/ae.py:84-145 when
+    it returns one loss) for a VAE-family trainer tr whose compute_batch was overridden: the override's torch loss drives the
+    CUDA forward / backward kernels through the model's encoder / decoder autograd nodes, FusedAdam (coupled weight decay,
+    as torch.optim.Adam) steps the module parameters, validation runs tr.evaluate (which calls the override) in eval mode.
+    train_iter is read on the host.  after_step(), when given, runs after every optimizer step.  best_model is
+    deepcopy(tr.model), a detached copy with its own inference engine."""
+    optimizer = FusedAdam([p for p in tr.model.parameters() if p.requires_grad], lr=lr, weight_decay=weight_decay)
+    for epoch in range(1, num_epochs + 1):
+        tr.model.train()
+        epoch_loss, epoch_recon, epoch_kl = [], [], []
+        for batch in tr.train_iter:
+            optimizer.zero_grad()
+            if two_losses:
+                recon_loss, kl_diverge = tr.compute_batch(batch)
+                batch_loss = recon_loss + kl_diverge
+            else:
+                batch_loss = tr.compute_batch(batch)
+            batch_loss.backward()
+            optimizer.step()
+            if after_step is not None:
+                after_step()
+            epoch_loss.append(batch_loss.item())
+            if two_losses:
+                epoch_recon.append(recon_loss.item())
+                epoch_kl.append(kl_diverge.item())
+        if two_losses:
+            tr.kl_loss.extend(epoch_kl)
+            tr.recon_loss.extend(epoch_recon)
+        else:
+            tr.recon_loss.extend(epoch_loss)
+        tr.model.eval()
+        val_loss = tr.evaluate(tr.val_iter)
+        if val_loss < tr.best_val_loss:
+            tr.best_model = deepcopy(tr.model)
+            tr.best_val_loss = val_loss
+        if two_losses:
+            print("Epoch[%d/%d], Total Loss: %.4f, Reconst Loss: %.4f, KL Div: %.7f, Val Loss: %.4f"
+                  % (epoch, num_epochs, np.mean(epoch_loss), np.mean(epoch_recon), np.mean(epoch_kl), val_loss))
+        else:
+            print("Epoch[%d/%d], Train Loss: %.4f, Val Loss: %.4f" % (epoch, num_epochs, np.mean(epoch_loss), val_loss))
+        tr.num_epochs += 1
+        if tr.viz:
+            if two_losses:
+                tr.sample_images(epoch)
+            else:
+                tr.reconstruct_images(tr.debugging_image, epoch)
+
+
+def compute_batch_evaluate(tr, iterator, two_losses):
+    """evaluate (src/vae.py:214-223, src/ae.py:162-164) over the overridden compute_batch: the mean per-batch loss"""
+    loss = []
+    for batch in iterator:
+        out = tr.compute_batch(batch)
+        loss.append((out[0] + out[1]).item() if two_losses else out.item())
+    return float(np.mean(loss))
+
+
+class SlotRing:
+    """The per-call slots of one engine's encoder or decoder: take() hands them out round robin, numbering the calls; a
+    backward whose slot a later call took, or whose engine was replaced (retire(): a larger batch), raises"""
+
+    def __init__(self, n, what):
+        self.n, self.what, self.calls, self.gen, self.retired = n, what, 0, [0] * n, False
+
+    def take(self):
+        self.calls += 1
+        slot = (self.calls - 1) % self.n
+        self.gen[slot] = self.calls
+        return slot, self.calls
+
+    def check(self, slot, gen):
+        if self.retired:
+            raise RuntimeError("%s activations were overwritten: the engine was rebuilt for a larger batch since this call"
+                               % self.what)
+        if self.gen[slot] != gen:
+            raise RuntimeError("%s activations were overwritten: at most %d %s.forward results can await their backward"
+                               % (self.what, self.n, self.what))
+
+    def retire(self):
+        self.retired = True
 
 
 class _FusedLoss(torch.autograd.Function):

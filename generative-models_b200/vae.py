@@ -13,8 +13,11 @@ import torch
 import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
+from torch.autograd.function import once_differentiable
+
 from gm_b200 import AdamHP, GmError, VaeEngine
-from gm_b200.gan_api import to_cuda
+from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate, SlotRing)
 
 
 def _engine_of(module, what, batch):
@@ -24,6 +27,63 @@ def _engine_of(module, what, batch):
     if parent is None:
         raise GmError(what + " is not part of a VAE: construct it through VAE(...)")
     return parent._engine_for(batch, what)
+
+
+def _ring(eng, what):
+    """the engine's SlotRing of per-call Encoder / Decoder slots"""
+    rings = eng.__dict__.setdefault("rings", {})
+    if what not in rings:
+        rings[what] = SlotRing(eng.num_slots(), what)
+    return rings[what]
+
+
+def _check_no_dx(ctx):
+    if ctx.needs_input_grad[0]:
+        raise RuntimeError("the gradient with respect to the encoder's input is not computed")
+
+
+class _EncoderCall(torch.autograd.Function):
+    """Encoder.forward under grad mode: (mu, log_var) and their backward on the CUDA kernels (gm_vae_encoder_forward /
+    _backward); autograd routes dL/dmu, dL/dlog_var in and the encoder's parameter gradients out"""
+
+    @staticmethod
+    def forward(ctx, x, eng, names, *params):
+        ctx.slot, ctx.gen = _ring(eng, "Encoder").take()
+        ctx.eng, ctx.names, ctx.n = eng, names, x.shape[0]
+        return eng.encoder_forward(ctx.slot, x)
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, dmu, dlog_var):
+        _check_no_dx(ctx)
+        _ring(ctx.eng, "Encoder").check(ctx.slot, ctx.gen)
+        g = ctx.eng.encoder_backward(ctx.slot, ctx.n, dmu, dlog_var)
+        return (None, None, None, *[g["encoder." + k] for k in ctx.names])
+
+
+class _DecoderCall(torch.autograd.Function):
+    """Decoder.forward under grad mode: the images and their backward (gm_vae_decoder_forward / _backward), with dL/dz
+    when z requires grad (z = reparameterize(mu, log_var))"""
+
+    @staticmethod
+    def forward(ctx, z, eng, names, *params):
+        ctx.slot, ctx.gen = _ring(eng, "Decoder").take()
+        ctx.eng, ctx.names, ctx.n = eng, names, z.shape[0]
+        return eng.decoder_forward(ctx.slot, z)
+
+    @staticmethod
+    @first_order
+    @once_differentiable
+    def backward(ctx, dimages):
+        _ring(ctx.eng, "Decoder").check(ctx.slot, ctx.gen)
+        g, dz = ctx.eng.decoder_backward(ctx.slot, ctx.n, dimages, ctx.needs_input_grad[0])
+        return (dz, None, None, *[g["decoder." + k] for k in ctx.names])
+
+
+def _node_args(mod):
+    names, params = zip(*mod.named_parameters())
+    return (names,) + params
 
 
 class Encoder(nn.Module):
@@ -38,6 +98,8 @@ class Encoder(nn.Module):
     def forward(self, x):
         x = to_cuda(x).float()
         eng = _engine_of(self, "Encoder", x.shape[0])
+        if torch.is_grad_enabled():
+            return _EncoderCall.apply(x, eng, *_node_args(self))
         _, mu, lv, _ = eng.forward(x, want_images=False)
         return mu, lv
 
@@ -54,7 +116,10 @@ class Decoder(nn.Module):
         z = to_cuda(z)
         if z.dim() == 1:                       # the reference decodes single latent vectors too (src/vae.py:289-290)
             z = z.view(1, -1)
-        return _engine_of(self, "Decoder", z.shape[0]).decode(z)
+        eng = _engine_of(self, "Decoder", z.shape[0])
+        if torch.is_grad_enabled():
+            return _DecoderCall.apply(z.float(), eng, *_node_args(self))
+        return eng.decode(z)
 
 
 class VAE(nn.Module):
@@ -100,6 +165,10 @@ class VAE(nn.Module):
 
     def forward(self, x):
         x = to_cuda(x).float()
+        if torch.is_grad_enabled():                                  # src/vae.py:94-98 on the differentiable encoder / decoder
+            mu, log_var = self.encoder(x)
+            z = self.reparameterize(mu, log_var)
+            return self.decoder(z), mu, log_var
         eng = self._engine_for(x.shape[0])
         eps = to_cuda(torch.randn(x.shape[0], self.z_dim))          # src/vae.py:104
         out, mu, lv, _ = eng.forward(x, eps=eps)
@@ -160,12 +229,19 @@ class VAETrainer:
             eng.exp_avg.copy_(old.exp_avg)
             eng.exp_avg_sq.copy_(old.exp_avg_sq)
             eng.steps = old.steps
+            for ring in getattr(old, "rings", {}).values():
+                ring.retire()
         self._engine, self._max_batch = eng, batch
         return eng
 
     def train(self, num_epochs, lr=1e-3, weight_decay=1e-5):
         """ Train a Variational Autoencoder (src/vae.py:127-191): a true epoch over train_iter,
-        losses read back once per epoch, validation with the forward-only kernels, best model kept. """
+        losses read back once per epoch, validation with the forward-only kernels, best model kept.  A subclass's own
+        compute_batch (README.md:31) is trained by the reference loop over the differentiable encoder / decoder instead
+        (gan_api.compute_batch_loop; train_iter is read on the host, device_noise does not apply). """
+        if has_custom_compute_batch(self):
+            refuse_multi_rank()
+            return compute_batch_loop(self, num_epochs, lr, weight_decay, two_losses=True)
         hp = AdamHP.make(lr, weight_decay=weight_decay)
         if self._engine is not None:
             self._engine.reset_optimizer()
@@ -224,6 +300,7 @@ class VAETrainer:
         images, _ = batch
         return to_cuda(images.view(images.shape[0], -1)).float().contiguous()
 
+    @builtin_step
     def compute_batch(self, batch):
         """ Compute loss for a batch of examples (src/vae.py:193-208): returns (recon, kl); calling
         (recon + kl).backward() delivers the gradient of their sum, as in src/vae.py:158-161. """
@@ -244,26 +321,32 @@ class VAETrainer:
         return torch.sum(0.5 * (mu ** 2 + torch.exp(log_var) - log_var - 1))
 
     def evaluate(self, iterator):
-        """ Evaluate on a given dataset (src/vae.py:214-223) with the forward-only kernels """
+        """ Evaluate on a given dataset (src/vae.py:214-223) with the forward-only kernels, or with an overriding
+        compute_batch as the reference does """
+        if has_custom_compute_batch(self):
+            return compute_batch_evaluate(self, iterator, two_losses=True)
         loss = []
-        for batch in iterator:
-            images = self._images(batch)
-            eng = self._ensure_engine(images.shape[0])
-            eps = to_cuda(torch.randn(images.shape[0], self.model.z_dim))
-            _, _, _, ls = eng.forward(images, eps=eps, want_images=False, want_latent=False, want_losses=True)
-            loss.append(ls.sum())
+        with torch.no_grad():
+            for batch in iterator:
+                images = self._images(batch)
+                eng = self._ensure_engine(images.shape[0])
+                eps = to_cuda(torch.randn(images.shape[0], self.model.z_dim))
+                _, _, _, ls = eng.forward(images, eps=eps, want_images=False, want_latent=False, want_losses=True)
+                loss.append(ls.sum())
         return float(torch.stack(loss).mean().item())
 
     def reconstruct_images(self, images, epoch, save=True):
         """ src/vae.py:225-252 without the plotting """
         batch = to_cuda(images.view(images.shape[0], -1))
-        reconst_images, _, _ = self.model(batch)
+        with torch.no_grad():
+            reconst_images, _, _ = self.model(batch)
         return reconst_images.view(images.shape).squeeze()
 
     def sample_images(self, epoch=-100, num_images=36, save=True):
         """ Viz method 1 (src/vae.py:254-276): z ~ p(z), x ~ p(x|z) """
         z = to_cuda(torch.randn(num_images, self.model.z_dim))
-        sample = self.model.decoder(z)
+        with torch.no_grad():
+            sample = self.model.decoder(z)
         return sample.view(num_images, self.model.shape, self.model.shape)
 
     def sample_interpolated_images(self):
@@ -274,7 +357,8 @@ class VAETrainer:
         out = []
         for alpha in np.linspace(0, 1, self.model.z_dim):
             z = to_cuda(float(alpha) * z1 + (1 - float(alpha)) * z2)
-            out.append(self.model.decoder(z).view(-1, self.model.shape, self.model.shape))
+            with torch.no_grad():
+                out.append(self.model.decoder(z).view(-1, self.model.shape, self.model.shape))
         return out
 
     def explore_latent_space(self, num_epochs=3):

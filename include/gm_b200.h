@@ -314,6 +314,26 @@ int gm_vae_forward(gm_vae* vae, const void* images_dev, int img_fmt, int n, cons
                    uint64_t step, float* out_images_dev, float* mu_logvar_dev, float* losses_dev, gm_stream stream);
 /* Decoder.forward (src/vae.py:74-77) for sampling. */
 int gm_vae_decode(gm_vae* vae, const float* z_dev, int n, float* out_images_dev, gm_stream stream);
+/* ---- per-call encoder / decoder (a user-written compute_batch, README.md:31) -------------
+ * Encoder.forward and Decoder.forward (src/vae.py:58-61,74-77) and their backward halves as separate entry points; the
+ * host wraps them in torch.autograd.Function objects and composes VAE.forward from them (src/vae.py:94-106).  `slot` in
+ * [0, gm_vae_num_slots) picks the buffers that keep one encoder (decoder) call's activations alive until its backward.
+ * Gradients go to a caller-supplied flat gradient buffer in the engine's layout: an encoder backward writes its segments
+ * [enc.linear.W .. enc.log_var.b] only, a decoder backward its segments [dec.linear.W .. dec.recon.b] only.  dz_dev
+ * (nullable) [batch, z] = dL/dz.  Each call forms pending lazy gradients first.  All refuse null pointers, a slot outside
+ * [0, gm_vae_num_slots) and batch outside (0, max_batch] with GM_ERR_ARG, and a split-precision engine with
+ * GM_ERR_UNSUPPORTED, before anything is launched. */
+int gm_vae_num_slots(const gm_vae* vae);
+int gm_vae_encoder_forward(gm_vae* vae, int slot, const float* x_dev, int batch, float* mu_logvar_dev, gm_stream stream);
+int gm_vae_encoder_backward(gm_vae* vae, int slot, int batch, const float* dmu_logvar_dev, float* grads_dev, gm_stream stream);
+int gm_vae_decoder_forward(gm_vae* vae, int slot, const float* z_dev, int batch, float* images_dev, gm_stream stream);
+int gm_vae_decoder_backward(gm_vae* vae, int slot, int batch, const float* dimages_dev, float* grads_dev, float* dz_dev,
+                            gm_stream stream);
+/* dL/d(pre-sigmoid output) of a sigmoid layer (the kernel of gm_vae_decoder_backward): out_rows_dev [rows, ld] bf16 holds
+ * the sigmoid output out and is overwritten with dout_dev [rows, x] fp32 * out * (1 - out), 0 in columns [x, ld).
+ * Refuses, with nothing launched: rows or x not positive, ld below x or not a multiple of 8, dout not 4-byte or
+ * out_rows not 16-byte aligned; GM_ERR_UNSUPPORTED for 2^31 threads or more. */
+int gm_sigmoid_upstream_rows(gm_ctx* ctx, const float* dout_dev, void* out_rows_dev, int rows, int x, int ld, gm_stream stream);
 
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
