@@ -178,6 +178,7 @@ def lib():
     L.gm_vae_set_lazy_grads.argtypes = [vp, i, vp]
     L.gm_vae_materialize_grads.argtypes = [vp, vp]
     L.gm_vae_last_eps.argtypes = [vp, vp, i, vp]
+    L.gm_vae_debug_read.argtypes = [vp, i, i, i, i, vp, vp]
     L.gm_vae_set_sampler.argtypes = [vp, C.c_longlong, C.c_longlong, C.c_longlong, u64]
     L.gm_gan_fisher_state.argtypes = [vp, C.POINTER(C.c_float), i, vp]
     _lib = L

@@ -779,6 +779,8 @@ extern "C" int gm_gan_create(gm_ctx* c, const gm_gan_desc* d, gm_gan** out) {
                 d->image_size, d->hidden_dim, d->z_dim);
   if (d->max_batch <= 0) return fail(c, GM_ERR_ARG, "max_batch must be positive (got %d)", d->max_batch);
   if (d->dtype_mode != GM_PREC_BF16 && d->dtype_mode != GM_PREC_SPLIT) return fail(c, GM_ERR_ARG, "unknown dtype_mode %d", d->dtype_mode);
+  if (d->hidden_dim + 1 > 448 || d->z_dim + 1 > 448)
+    return fail(c, GM_ERR_UNSUPPORTED, "hidden_dim <= 447 and generator input width <= 447 in this build (got %d, %d)", d->hidden_dim, d->z_dim);
   gm_gan* g = new gm_gan();
   g->ctx = c;
   g->d = *d;
@@ -873,10 +875,6 @@ extern "C" int gm_gan_create(gm_ctx* c, const gm_gan_desc* d, gm_gan** out) {
     g->lo = g->arena.lo_off;
   }
 #undef TRY
-  if (g->H + 1 > 448 || g->Z + 1 > 448) {
-    gm_gan_destroy(g);
-    return fail(c, GM_ERR_UNSUPPORTED, "hidden_dim <= 447 and generator input width <= 447 in this build (got %d, %d)", d->hidden_dim, d->z_dim);
-  }
   *out = g;
   return GM_OK;
 }
@@ -1372,6 +1370,13 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
       c->launches++;
     }
     if ((rc = launch_plan(c, sp->gp_v, s))) return rc;          // V = U W1 -> R region of Xall, ||V||^2 -> slots_v
+    {
+      // dW1d's bias row sums DHall against Xall's ones column over all nreg regions, and the penalty has no b1 gradient:
+      // the R rows' ones column must be 0, but a larger earlier batch leaves its real rows' 1.0 there (V fills [0, X))
+      __nv_bfloat16* col = g->Xall + rreg * XP + X;
+      CU_OK(c, cudaMemset2DAsync(col, size_t(XP) * sizeof(__nv_bfloat16), 0, sizeof(__nv_bfloat16), B, s));
+      if (g->lo) CU_OK(c, cudaMemset2DAsync(col + g->lo, size_t(XP) * sizeof(__nv_bfloat16), 0, sizeof(__nv_bfloat16), B, s));
+    }
     GpParams gpp;
     gpp.slots_s = g->slots + 2 * B; gpp.nslots_s = 2 * cdiv(H, 208); gpp.slot_ld = g->nreg * g->Bmax;
     gpp.slots_v = g->slots_v; gpp.nslots_v = 2 * cdiv(X, 208); gpp.slotv_ld = g->Bmax;
@@ -1734,7 +1739,11 @@ extern "C" int gm_gan_debug_read(gm_gan* g, int which, int row0, int rows, int c
   which %= 16;
   const __nv_bfloat16* src[7] = {g->Zb, g->Hg, g->Xall, g->Aall, g->DHall, g->DA2, g->DHg};
   const int ld[7] = {g->ZP, g->HP, g->XP, g->HP, g->HP, g->XP, g->HP};
+  const long long nrow[7] = {g->Bmax, g->Bmax, (long long)g->nreg * g->Bmax, (long long)g->nreg * g->Bmax,
+                             (long long)g->nreg * g->Bmax, g->Bmax, g->Bmax};
   if (which < 0 || which > 6 || cols > ld[which]) return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: bad buffer / extent");
+  if ((long long)row0 + rows > nrow[which])
+    return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: rows [%d, %lld) run past the buffer's %lld rows", row0, (long long)row0 + rows, nrow[which]);
   const long long tot = (long long)rows * cols;
   launch_pdl("bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream),
              src[which] + size_t(row0) * ld[which] + (plane == 2 ? g->lo : 0), ld[which], out_dev, rows, cols, plane == 0 ? g->lo : 0ll);

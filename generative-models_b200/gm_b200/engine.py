@@ -461,6 +461,14 @@ class VaeEngine:
                                                     C.c_void_p(out.ctypes.data)))
         return torch.from_numpy(out).to(self.device)
 
+    BUFFERS = {"Xin": 0, "H1": 1, "Zb": 2, "H3": 3, "DA4": 4, "DA3": 5, "DML": 6, "DA1": 7}
+
+    def debug_read(self, which, row0, rows, cols):
+        """An internal bf16 buffer of the last grad() as fp32 [rows, cols] (hi + lo in split mode); tests only."""
+        out = torch.empty(rows, cols, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_vae_debug_read(self.g, self.BUFFERS[which], row0, rows, cols, _ptr(out), _stream()))
+        return out
+
     def apply(self, hp):
         self.steps += 1
         check(self.h, lib().gm_vae_apply(self.g, C.byref(hp), self.steps, _stream()))

@@ -306,6 +306,10 @@ int gm_vae_set_lazy_grads(gm_vae* vae, int on, gm_stream stream);
 int gm_vae_materialize_grads(gm_vae* vae, gm_stream stream);
 /* eps of the last gm_vae_grad / gm_vae_forward call (src/vae.py:104; the Philox draw when eps_dev was NULL) -> out_dev [batch, z] */
 int gm_vae_last_eps(gm_vae* vae, float* out_dev, int batch, gm_stream stream);
+/* test aid: an internal bf16 buffer of the last gm_vae_grad as fp32 (hi + lo planes summed in split mode) -> out_dev [rows, cols];
+ * which: 0 image rows, 1 encoder hidden, 2 latent z, 3 decoder hidden, 4 dL/d recon pre-sigmoid, 5 decoder hidden gradient,
+ * 6 [dmu | dlog_var], 7 encoder hidden gradient */
+int gm_vae_debug_read(gm_vae* vae, int which, int row0, int rows, int cols, float* out_dev, gm_stream stream);
 /* optimizer.step() with coupled weight decay (src/vae.py:139-142,162). */
 int gm_vae_apply(gm_vae* vae, const gm_adam_hp* hp, int step, gm_stream stream);
 /* VAE.forward (+ losses) without gradients: evaluate / reconstruct (src/vae.py:214-252).

@@ -392,41 +392,51 @@ def gan_train(P, variant, images, draws, steps, G_lr, D_lr, D_steps=1, clip=None
 
 
 # ---------------------------------------------------------------- VAE
-def vae_step(P, x, eps):
+def _relu(name, a):
+    return np.maximum(a, 0)
+
+
+def vae_step(P, x, eps, q=_exact, relu=_relu):
     """VAE.forward + compute_batch + backward (src/vae.py:94-106,193-212):
     recon = sum((x-out)^2), kl = sum(0.5(mu^2+exp(lv)-lv-1)); returns grads of
-    recon+kl for all ten tensors."""
-    W1, b1 = P["encoder.linear.weight"], P["encoder.linear.bias"]
-    Wm, bm = P["encoder.mu.weight"], P["encoder.mu.bias"]
-    Wv, bv = P["encoder.log_var.weight"], P["encoder.log_var.bias"]
-    W3, b3 = P["decoder.linear.weight"], P["decoder.linear.bias"]
-    W4, b4 = P["decoder.recon.weight"], P["decoder.recon.bias"]
-    a1 = linear(x, W1, b1)
-    h1 = np.maximum(a1, 0)
+    recon+kl for all ten tensors.
+    q: operand-quantisation hook at the points where the CUDA VAE stores bf16 GEMM operands (bf16_points models it):
+    the weights, x, the hidden rows, z, and the upstream gradients da4, da3, [dmu | dlv], da1; mu / log_var, dz, the
+    reconstruction and both losses stay fp32.
+    relu: relu(name, a) for the encoder ("h1") and decoder ("h3") hidden layers (tests give near-zero units a side);
+    the ReLU masks of the backward are taken from its output."""
+    W1, b1 = q("W", P["encoder.linear.weight"]), P["encoder.linear.bias"]
+    Wm, bm = q("W", P["encoder.mu.weight"]), P["encoder.mu.bias"]
+    Wv, bv = q("W", P["encoder.log_var.weight"]), P["encoder.log_var.bias"]
+    W3, b3 = q("W", P["decoder.linear.weight"]), P["decoder.linear.bias"]
+    W4, b4 = q("W", P["decoder.recon.weight"]), P["decoder.recon.bias"]
+    xq = q("x", x)
+    a1 = linear(xq, W1, b1)
+    h1 = q("h", relu("h1", a1))
     mu, lv = linear(h1, Wm, bm), linear(h1, Wv, bv)
     sd = np.exp(lv / 2)
-    z = mu + eps * sd                                      # src/vae.py:105
+    z = q("z", mu + eps * sd)                              # src/vae.py:105
     a3 = linear(z, W3, b3)
-    h3 = np.maximum(a3, 0)
+    h3 = q("h", relu("h3", a3))
     out = sigmoid(linear(h3, W4, b4))
-    recon = np.sum((x - out) ** 2)                         # src/vae.py:203
+    recon = np.sum((xq - out) ** 2)                        # src/vae.py:203
     kl = np.sum(0.5 * (mu ** 2 + np.exp(lv) - lv - 1))     # src/vae.py:212
     g = {}
-    da4 = -2 * (x - out) * out * (1 - out)
+    da4 = q("da4", -2 * (xq - out) * out * (1 - out))
     g["decoder.recon.weight"] = da4.T @ h3
     g["decoder.recon.bias"] = da4.sum(0)
-    da3 = (da4 @ W4) * (a3 > 0)
+    da3 = q("da3", (da4 @ W4) * (h3 > 0))
     g["decoder.linear.weight"] = da3.T @ z
     g["decoder.linear.bias"] = da3.sum(0)
     dz = da3 @ W3
-    dmu = mu + dz
-    dlv = 0.5 * (np.exp(lv) - 1) + dz * eps * sd * 0.5
+    dmu = q("dml", mu + dz)
+    dlv = q("dml", 0.5 * (np.exp(lv) - 1) + dz * eps * sd * 0.5)
     g["encoder.mu.weight"] = dmu.T @ h1
     g["encoder.mu.bias"] = dmu.sum(0)
     g["encoder.log_var.weight"] = dlv.T @ h1
     g["encoder.log_var.bias"] = dlv.sum(0)
-    da1 = (dmu @ Wm + dlv @ Wv) * (a1 > 0)
-    g["encoder.linear.weight"] = da1.T @ x
+    da1 = q("da1", (dmu @ Wm + dlv @ Wv) * (h1 > 0))
+    g["encoder.linear.weight"] = da1.T @ xq
     g["encoder.linear.bias"] = da1.sum(0)
     return recon, kl, g, dict(out=out, mu=mu, lv=lv)
 

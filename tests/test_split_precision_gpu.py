@@ -15,6 +15,7 @@ import torch
 from inputs import (GAN_SHAPES, INFO_SHAPES, BEGAN_SHAPES, VAE_SHAPES, STEPS, B, gm_init_weights, params_dict, load_case,
                     unpack_draws, images_from_bits)
 from oracle import ref_math as R
+from mlp_harness import DeviceReluSides, aux_from as _aux_from, gan_engine, nrel as _nrel
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3          # north_star: "within 1e-3 relative fp32"
@@ -39,88 +40,8 @@ def _dump():
         json.dump(_REPORT, f, indent=1, sort_keys=True)
 
 
-def _nrel(a, b):
-    a, b = np.asarray(a, np.float64).ravel(), np.asarray(b, np.float64).ravel()
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
 def _engine(variant, batch=B):
-    import gm_b200
-    eng = gm_b200.GanEngine(784, 400, 20, max_batch=batch, variant=variant,
-                            d_out_act="relu" if variant == "wgp" else "sigmoid", precision="split")
-    W = gm_init_weights(GAN_SHAPES, 1234)
-    eng.load(0, [W["G.linear"][0], W["G.linear"][1], W["G.generate"][0], W["G.generate"][1]])
-    eng.load(1, [W["D.linear"][0], W["D.linear"][1], W["D.discriminate"][0], W["D.discriminate"][1]])
-    return eng
-
-
-# ReLU boundaries.  dReLU/da is discontinuous at a = 0: a hidden unit whose pre-activation is ~1e-6 (fp32 rounding
-# level of a 784-term dot product) lands on either side depending on the summation order - the reference itself flips
-# such units between BLAS thread counts (SURVEY.md 8c: 8 vs 1 thread differ at 3e-7) - and one flipped unit moves a
-# batch-64 gradient by ~1e-2.  For units with |a| < TOL_A the oracle therefore takes the side the device took (read
-# back from the engine's activation buffers); every other unit must agree by itself.  The number of such units is
-# reported (0 or 1 per step at these sizes).
-TOL_A = 2e-5
-
-
-class DeviceReluSides:
-    """Context manager: patches oracle.ref_math's forward functions so that near-boundary ReLU units take the
-    device's side.  d_regions: row offsets (in units of B) of the D-hidden rows for successive d_forward calls."""
-
-    def __init__(self, eng, d_regions, g_hidden=True):
-        self.eng, self.d_regions, self.g_hidden, self.count = eng, list(d_regions), g_hidden, 0
-
-    def __enter__(self):
-        self._d, self._g, self._calls = R.d_forward, R.g_forward, 0
-
-        def d_forward(P, x, *a, **k):
-            fw = self._d(P, x, *a, **k)
-            reg = self.d_regions[min(self._calls, len(self.d_regions) - 1)]
-            reg = reg if isinstance(reg, tuple) else ("Aall", reg)
-            buf, reg, positive = reg if len(reg) == 3 else (reg[0], reg[1], False)
-            self._calls += 1
-            near = np.abs(fw["a1"]) < TOL_A
-            if near.any():
-                n = fw["a1"].shape[0]
-                # the buffers hold activations or the signed mask form w2 * relu'(a) (nonzero <=> active); WGAN-GP's real /
-                # fake rows hold PRE-activations (positive <=> active; regions flagged `positive`)
-                v = self.eng.debug_read(buf, reg * n, n, fw["a1"].shape[1]).cpu().numpy()
-                act = (v > 0) if positive else (v != 0)
-                for key in ("h", "hq"):
-                    v = fw[key].copy()
-                    v[near] = np.where(act[near], 1e-30, 0.0)
-                    fw[key] = v
-                self.count += int(near.sum())
-            return fw
-
-        def g_forward(P, z, *a, **k):
-            fw = self._g(P, z, *a, **k)
-            near = np.abs(fw["a1"]) < TOL_A
-            if self.g_hidden and near.any():
-                n = fw["a1"].shape[0]
-                act = self.eng.debug_read("Hg", 0, n, fw["a1"].shape[1]).cpu().numpy() > 0
-                v = fw["h"].copy()
-                v[near] = np.where(act[near], 1e-30, 0.0)
-                fw["h"] = v
-                self.count += int(near.sum())
-            return fw
-        R.d_forward, R.g_forward = d_forward, g_forward
-        return self
-
-    def __exit__(self, *exc):
-        R.d_forward, R.g_forward = self._d, self._g
-        return False
-
-
-def _aux_from(draws_iter, case):
-    if case == "wgp":
-        eps = next(draws_iter)
-        return eps.astype(np.float64), torch.from_numpy(eps.reshape(-1).copy()).cuda()
-    if case == "dra":
-        delta, u = next(draws_iter), next(draws_iter)
-        dev = torch.from_numpy(np.concatenate([delta.reshape(-1), u.reshape(-1)])).cuda()
-        return (delta.astype(np.float64), u.astype(np.float64)), dev
-    return None, None
+    return gan_engine(variant, max_batch=batch, precision="split")
 
 
 @pytest.mark.parametrize("case", ROW_VARIANTS + GP_VARIANTS)
