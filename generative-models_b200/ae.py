@@ -13,58 +13,10 @@ import torch
 import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
-from torch.autograd.function import once_differentiable
 
 from gm_b200 import AdamHP, AeEngine, GmError
-from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
-                             compute_batch_evaluate, SlotRing)
-
-
-def _ring(eng, what):
-    """the engine's SlotRing of per-call Encoder / Decoder slots"""
-    rings = eng.__dict__.setdefault("rings", {})
-    if what not in rings:
-        rings[what] = SlotRing(eng.SLOTS, what)
-    return rings[what]
-
-
-class _EncoderCall(torch.autograd.Function):
-    """Encoder.forward under grad mode: the code relu(linear(x)) and its backward on the CUDA kernels
-    (AeEngine.encoder_forward / encoder_backward); autograd routes dL/dcode in and the parameter gradients out"""
-
-    @staticmethod
-    def forward(ctx, x, eng, *params):
-        ctx.slot, ctx.gen = _ring(eng, "Encoder").take()
-        ctx.eng, ctx.n = eng, x.shape[0]
-        return eng.encoder_forward(ctx.slot, x)
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, dcode):
-        if ctx.needs_input_grad[0]:
-            raise RuntimeError("the gradient with respect to the encoder's input is not computed")
-        _ring(ctx.eng, "Encoder").check(ctx.slot, ctx.gen)
-        g = ctx.eng.encoder_backward(ctx.slot, ctx.n, dcode)
-        return None, None, g["encoder.linear.weight"], g["encoder.linear.bias"]
-
-
-class _DecoderCall(torch.autograd.Function):
-    """Decoder.forward under grad mode: sigmoid(linear(code)) and its backward, with dL/dcode when the code requires grad"""
-
-    @staticmethod
-    def forward(ctx, code, eng, *params):
-        ctx.slot, ctx.gen = _ring(eng, "Decoder").take()
-        ctx.eng, ctx.n = eng, code.shape[0]
-        return eng.decoder_forward(ctx.slot, code)
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, dimages):
-        _ring(ctx.eng, "Decoder").check(ctx.slot, ctx.gen)
-        g, dcode = ctx.eng.decoder_backward(ctx.slot, ctx.n, dimages)
-        return (dcode if ctx.needs_input_grad[0] else None), None, g["decoder.linear.weight"], g["decoder.linear.bias"]
+from gm_b200.gan_api import (to_cuda, builtin_step, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate, slot_ring, EngineCall, GradHandoff, grow_engine)
 
 
 class Encoder(nn.Module):
@@ -76,8 +28,20 @@ class Encoder(nn.Module):
 
     def forward(self, x):
         eng, attached = _engine_of(self, "Encoder", x.shape[0])
-        if attached and torch.is_grad_enabled():
-            return _EncoderCall.apply(to_cuda(x).float(), eng, self.linear.weight, self.linear.bias)
+        if attached and torch.is_grad_enabled():   # the code relu(linear(x)) and its backward on the CUDA kernels
+            ring, n = slot_ring(eng, "Encoder", eng.SLOTS), x.shape[0]
+
+            def forward(x):
+                slot, gen = ring.take()
+                return eng.encoder_forward(slot, x), (slot, gen)
+
+            def backward(handle, grads, need_dx):
+                if need_dx:
+                    raise RuntimeError("the gradient with respect to the encoder's input is not computed")
+                ring.check(*handle)
+                g = eng.encoder_backward(handle[0], n, grads[0])
+                return None, [g["encoder.linear.weight"], g["encoder.linear.bias"]]
+            return EngineCall.apply(to_cuda(x).float(), forward, backward, self.linear.weight, self.linear.bias)
         return eng.encode(to_cuda(x).float())
 
 
@@ -90,8 +54,18 @@ class Decoder(nn.Module):
 
     def forward(self, encoder_output):
         eng, attached = _engine_of(self, "Decoder", encoder_output.shape[0])
-        if attached and torch.is_grad_enabled():
-            return _DecoderCall.apply(to_cuda(encoder_output).float(), eng, self.linear.weight, self.linear.bias)
+        if attached and torch.is_grad_enabled():   # sigmoid(linear(code)) and its backward, with dL/dcode when the code requires grad
+            ring, n = slot_ring(eng, "Decoder", eng.SLOTS), encoder_output.shape[0]
+
+            def forward(code):
+                slot, gen = ring.take()
+                return eng.decoder_forward(slot, code), (slot, gen)
+
+            def backward(handle, grads, need_dcode):
+                ring.check(*handle)
+                g, dcode = eng.decoder_backward(handle[0], n, grads[0])
+                return (dcode if need_dcode else None), [g["decoder.linear.weight"], g["decoder.linear.bias"]]
+            return EngineCall.apply(to_cuda(encoder_output).float(), forward, backward, self.linear.weight, self.linear.bias)
         return eng.decode(to_cuda(encoder_output).float())
 
 
@@ -145,19 +119,6 @@ class Autoencoder(nn.Module):
         return new
 
 
-class _AeLoss(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, anchor, val, holder):
-        ctx.holder = holder
-        return val.clone()
-
-    @staticmethod
-    def backward(ctx, gout):
-        for p, g in ctx.holder():
-            p.grad = g * gout if p.grad is None else p.grad + g * gout
-        return None, None, None
-
-
 class AutoencoderTrainer:
     def __init__(self, model, train_iter, val_iter, test_iter, viz=False):
         """ Object to hold data iterators, train the model (src/ae.py:67-82) """
@@ -177,22 +138,8 @@ class AutoencoderTrainer:
         if self._engine is not None and batch <= self._max_batch:
             self._engine.sync_all()
             return self._engine
-        m, old = self.model, self._engine
-        batch = max(batch, self._max_batch, 64)
-        eng = AeEngine(m.image_size, m.hidden_dim, max_batch=batch)
-        named = dict(m.named_parameters())
-        eng.load({k: v.data for k, v in named.items()})
-        views = eng.views()
-        for k, p in named.items():
-            p.data = views[k]                      # nn.Parameter storage == the engine's fp32 master weights
-        if old is not None:
-            eng.exp_avg.copy_(old.exp_avg)
-            eng.exp_avg_sq.copy_(old.exp_avg_sq)
-            eng.steps = old.steps
-            for ring in getattr(old, "rings", {}).values():
-                ring.retire()
-        self._engine, self._max_batch = eng, batch
-        return eng
+        m = self.model
+        return grow_engine(self, batch, lambda rows: AeEngine(m.image_size, m.hidden_dim, max_batch=rows))
 
     def train(self, num_epochs, lr=1e-3, weight_decay=1e-5):
         """ Train the autoencoder (src/ae.py:84-145): a true epoch over train_iter, losses read back once per epoch.  A
@@ -232,9 +179,9 @@ class AutoencoderTrainer:
         images = self._images(batch)
         eng = self._ensure_engine(images.shape[0])
         loss = eng.grad(images).clone()
-        named = dict(self.model.named_parameters())
         gviews = eng.views(eng.grads)
-        return _AeLoss.apply(loss.detach().requires_grad_(True), loss, lambda: [(named[k], gviews[k]) for k in named])
+        pairs = [(p, gviews[k]) for k, p in self.model.named_parameters()]
+        return GradHandoff.apply(loss.detach().requires_grad_(True), loss, pairs)
 
     def evaluate(self, iterator):
         """ Evaluate on a given dataset (src/ae.py:162-164), with an overriding compute_batch as the reference does """

@@ -27,54 +27,7 @@ from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
-from gm_b200.gan_api import to_cuda, _FusedLoss, FusedAdam, builtin_step, reference_loop, first_order as _first_order
-from torch.autograd.function import once_differentiable
-
-
-def _grads_for(grads, tag, mod, names):
-    """the node's gradients {"<tag>.<name>": tensor} in the order of names, on the module's parameters' device"""
-    params = dict(mod.named_parameters())
-    return [grads["%s.%s" % (tag, k)].contiguous().to(params[k].device) for k in names]
-
-
-class _DcGForward(torch.autograd.Function):
-    """Generator.forward under grad mode: G(z) and its backward on the conv kernels (DcganEngine.custom_g_forward /
-    custom_g_backward); autograd routes dL/dG(z) in and the parameter gradients out"""
-
-    @staticmethod
-    def forward(ctx, noise, eng, mod, names, *params):
-        out, ctx.handle = eng.custom_g_forward(noise)
-        ctx.eng, ctx.mod, ctx.names = eng, mod, names
-        return out
-
-    @staticmethod
-    @_first_order
-    @once_differentiable        # the backward is a kernel chain: create_graph=True gets an error, not a missing term
-    def backward(ctx, dimages):
-        grads = ctx.eng.custom_g_backward(ctx.handle, dimages.float().contiguous())
-        return (None, None, None, None, *_grads_for(grads, "G", ctx.mod, ctx.names))
-
-
-class _DcDForward(torch.autograd.Function):
-    """Discriminator.forward under grad mode: D(x) and its backward, with dL/dx when x requires grad (D(G(z)))"""
-
-    @staticmethod
-    def forward(ctx, x, eng, mod, names, *params):
-        scores, ctx.handle = eng.custom_d_forward(x)
-        ctx.eng, ctx.mod, ctx.names = eng, mod, names
-        return scores
-
-    @staticmethod
-    @_first_order
-    @once_differentiable
-    def backward(ctx, dscore):
-        grads, dx = ctx.eng.custom_d_backward(ctx.handle, dscore.float(), ctx.needs_input_grad[0])
-        return (dx, None, None, None, *_grads_for(grads, "D", ctx.mod, ctx.names))
-
-
-def _node_args(mod):
-    names, params = zip(*mod.named_parameters())
-    return (mod, names) + params
+from gm_b200.gan_api import to_cuda, EngineCall, GradHandoff, flat_pairs, FusedAdam, builtin_step, reference_loop
 
 
 class Generator(nn.Module):
@@ -96,8 +49,13 @@ class Generator(nn.Module):
         if tr is None:
             raise GmError("Generator is not attached to a CUDA engine yet: construct the DCGANTrainer first")
         eng = tr._engine_synced()
-        if torch.is_grad_enabled() and eng.supports_custom_loss:
-            return _DcGForward.apply(to_cuda(x).float(), eng, *_node_args(self))
+        if torch.is_grad_enabled() and eng.supports_custom_loss:   # G(z) and its backward on the conv kernels
+            named = list(self.named_parameters())
+
+            def backward(handle, grads, need_dx):
+                g = eng.custom_g_backward(handle, grads[0].float().contiguous())
+                return None, [g["G." + k].contiguous().to(p.device) for k, p in named]
+            return EngineCall.apply(to_cuda(x).float(), eng.custom_g_forward, backward, *(p for _, p in named))
         return eng.generate(to_cuda(x).float())
 
 
@@ -128,8 +86,14 @@ class Discriminator(nn.Module):
         if tr is None:
             raise GmError("Discriminator is not attached to a CUDA engine yet: construct its trainer first")
         eng = tr._engine_synced()
-        if torch.is_grad_enabled() and eng.supports_custom_loss:
-            return _DcDForward.apply(to_cuda(x).float().reshape(x.shape[0], -1), eng, *_node_args(self))
+        if torch.is_grad_enabled() and eng.supports_custom_loss:   # D(x) and its backward, with dL/dx when x requires grad
+            named = list(self.named_parameters())
+
+            def backward(handle, grads, need_dx):
+                g, dx = eng.custom_d_backward(handle, grads[0].float(), need_dx)
+                return dx, [g["D." + k].contiguous().to(p.device) for k, p in named]
+            return EngineCall.apply(to_cuda(x).float().reshape(x.shape[0], -1), eng.custom_d_forward, backward,
+                                    *(p for _, p in named))
         return eng.discriminate(to_cuda(x).float().reshape(x.shape[0], -1))
 
 
@@ -230,7 +194,7 @@ class EngineSync:
         params = [p for _, _, p in named]
         flat = torch.cat([tg["%s.%s" % (tag, k)].detach().reshape(-1).to(p.device) for tag, k, p in named])
         self._dirty = True                                            # the caller's optimizer will change the module parameters
-        return _FusedLoss.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat, params)
+        return GradHandoff.apply(flat.detach().requires_grad_(True), loss_val.detach().to(flat.device), flat_pairs(params, flat))
 
 
 class DCGANTrainer(EngineSync):

@@ -34,10 +34,9 @@ from utils import *  # noqa: F401,F403
 from gm_b200 import AdamHP, GmError, DcganEngine
 from gm_b200 import parallel as par
 from gm_b200.dcgan import DevicePool
-from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
-                             compute_batch_evaluate)
-from torch.autograd.function import once_differentiable
-from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats, push_running_stats, _grads_for, _node_args
+from gm_b200.gan_api import (to_cuda, builtin_step, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate, EngineCall)
+from dc_gan import EngineSync, dcgan_init, module_params, pull_running_stats, push_running_stats
 
 
 def _parent_of(module, what):
@@ -47,50 +46,20 @@ def _parent_of(module, what):
     return parent
 
 
-class _EncoderCall(torch.autograd.Function):
-    """Encoder.forward in training mode under grad mode: the VAE's (mu, log_var) or the autoencoder's code and their
-    backward on the conv kernels (DcganEngine.custom_d_forward / custom_d_backward); autograd routes the upstream in and
-    the encoder's parameter gradients out"""
-
-    @staticmethod
-    def forward(ctx, x, parent, eng, mod, names, *params):
-        out, ctx.handle = eng.custom_d_forward(x)
-        ctx.parent, ctx.eng, ctx.mod, ctx.names = parent, eng, mod, names
-        return out
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, *dout):
-        grads, _ = ctx.eng.custom_d_backward(ctx.handle, dout if len(dout) == 2 else dout[0], ctx.needs_input_grad[0])
-        return (None, None, None, None, None, *_grads_for(ctx.parent._module_names(grads), "D", ctx.mod, ctx.names))
-
-
-class _DecoderCall(torch.autograd.Function):
-    """Decoder.forward in training mode under grad mode: the images and their backward, with dL/dz when z requires grad"""
-
-    @staticmethod
-    def forward(ctx, z, eng, mod, names, *params):
-        out, ctx.handle = eng.custom_g_forward(z)
-        ctx.eng, ctx.mod, ctx.names = eng, mod, names
-        return out
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, dimages):
-        grads, dz = ctx.eng.custom_g_backward(ctx.handle, dimages.float().contiguous(), need_dz=True)
-        return ((dz if ctx.needs_input_grad[0] else None), None, None, None, *_grads_for(grads, "G", ctx.mod, ctx.names))
-
-
 def _encoder_forward(mod, x):
     """Encoder.forward of the VAE and the autoencoder: per-call kernels with a backward in training mode under grad mode,
     the inference calls otherwise"""
     x = to_cuda(x).float()
     parent = _parent_of(mod, "Encoder")
     eng = parent._engine()
-    if torch.is_grad_enabled() and mod.training:
-        out = _EncoderCall.apply(x.reshape(x.shape[0], -1), parent, eng, *_node_args(mod))
+    if torch.is_grad_enabled() and mod.training:      # (mu, log_var) or the code, and their backward on the conv kernels
+        named = list(mod.named_parameters())
+
+        def backward(handle, grads, need_dx):
+            g, _ = eng.custom_d_backward(handle, grads if len(grads) == 2 else grads[0], need_dx)
+            g = parent._module_names(g)
+            return None, [g["D." + k].contiguous().to(p.device) for k, p in named]
+        out = EngineCall.apply(x.reshape(x.shape[0], -1), eng.custom_d_forward, backward, *(p for _, p in named))
     else:
         out = eng.encode(x.reshape(x.shape[0], -1), train=mod.training)
     parent._after_forward(eng, mod.training)
@@ -134,8 +103,13 @@ class Decoder(nn.Module):
             z = z.view(1, -1)
         parent = _parent_of(self, "Decoder")
         eng = parent._engine()
-        if torch.is_grad_enabled() and self.training:
-            out = _DecoderCall.apply(z, eng, *_node_args(self))
+        if torch.is_grad_enabled() and self.training:     # the images and their backward, with dL/dz when z requires grad
+            named = list(self.named_parameters())
+
+            def backward(handle, grads, need_dz):
+                g, dz = eng.custom_g_backward(handle, grads[0].float().contiguous(), need_dz=True)
+                return (dz if need_dz else None), [g["G." + k].contiguous().to(p.device) for k, p in named]
+            out = EngineCall.apply(z, eng.custom_g_forward, backward, *(p for _, p in named))
         else:
             out = eng.decode(z, train=self.training)
         parent._after_forward(eng, self.training)

@@ -43,6 +43,7 @@ import ctypes as C
 import torch
 
 from . import _lib
+from .gan_api import SlotRing
 from ._lib import GmError, OUT_ACTS, VARIANTS, check, lib, _ptr, _stream, gemm_bf16, adam_step
 
 SLOPE = 0.2
@@ -339,8 +340,9 @@ class DcganEngine:
         self.vae_loss = torch.zeros(2, device=self.device)       # VAE: (recon, kl) of the last vae_grad, this process's sums
         self.ae_loss = torch.zeros(1, device=self.device)        # autoencoder: recon of the last ae_grad, this process's sum
         self._bufs = {}
-        self._calls = {"d": 0, "g": 0}                           # custom_d_forward / custom_g_forward calls so far
-        self._slot_gen = {"d": [0] * self.D_SLOTS, "g": [0] * self.G_SLOTS}   # the call that holds each slot
+        coder = variant in ("vae", "ae")
+        self._rings = {"d": SlotRing(self.D_SLOTS, "Encoder" if coder else "Discriminator"),      # custom_d_forward's slots
+                       "g": SlotRing(self.G_SLOTS, "Decoder" if coder else "Generator")}          # custom_g_forward's
         self.init_weights()
 
     # ------------------------------------------------------------------ parameters
@@ -1153,7 +1155,7 @@ class DcganEngine:
 
     # ------------------------------------------------------------------ per-call forward / backward (user-written losses)
     # A user's train_D / train_G (README.md:31) calls model.D / model.G as its loss needs and back-propagates through the
-    # drop-ins' autograd nodes (dc_gan._DcDForward / _DcGForward).  Each call keeps its saved activations in a slot of a ring,
+    # drop-ins' autograd nodes (gan_api.EngineCall).  Each call keeps its saved activations in a slot of a ring,
     # D_SLOTS discriminator and G_SLOTS generator calls, allocated on first use; a backward whose slot a later call has taken
     # raises instead of reading that call's tensors.  The losses that need these are the ones whose D returns one score per
     # image, and the VAE's and autoencoder's compute_batch, whose encoder is D's trunk and head and whose decoder is G;
@@ -1168,16 +1170,11 @@ class DcganEngine:
         if not self.supports_custom_loss:
             raise GmError("per-call forwards with a backward are built for the discriminators with one score per image "
                           "(not %s)" % self.variant)
-        gens = self._slot_gen[kind]
-        self._calls[kind] += 1
-        slot = (self._calls[kind] - 1) % len(gens)
-        gens[slot] = self._calls[kind]
-        return dict(kind=kind, slot=slot, gen=self._calls[kind])
+        slot, gen = self._rings[kind].take()
+        return dict(kind=kind, slot=slot, gen=gen)
 
-    def _check_live(self, handle, what):
-        if self._slot_gen[handle["kind"]][handle["slot"]] != handle["gen"]:
-            raise RuntimeError("%s activations were overwritten: at most %d %s.forward results can await their backward"
-                               % (what, len(self._slot_gen[handle["kind"]]), what))
+    def _check_live(self, handle):
+        self._rings[handle["kind"]].check(handle["slot"], handle["gen"])
 
     def custom_d_forward(self, images):
         """D(images) in training mode (batch statistics; the running statistics move per call, as nn.BatchNorm2d.train()):
@@ -1204,11 +1201,11 @@ class DcganEngine:
         dL/d(images) [n, ch*64*64] fp32 or None).  dL/dlogit = dscore act'(s) is formed on the n logits.  For the VAE's
         encoder dscore is (dL/dmu, dL/dlog_var), each [n, z], for the autoencoder's dL/dcode [n, z]; they have no dL/dx."""
         if self.variant in ("vae", "ae"):
-            self._check_live(handle, "Encoder")
+            self._check_live(handle)
             if need_dx:
                 raise GmError("the gradient with respect to the encoder's input is not computed")
             return self._torch_views({"D": self._encoder_backward(handle, dscore)}), None
-        self._check_live(handle, "Discriminator")
+        self._check_live(handle)
         n, s = handle["n"], handle["s"]
         d = dscore.reshape(n).to(self.device, torch.float32)
         if self.d_out_act == "sigmoid":
@@ -1253,7 +1250,7 @@ class DcganEngine:
         """dimages [n, ch*64*64] = dL/dG(z) of custom_g_forward's call -> {"G.<name>": gradient in torch's layout}, and with
         need_dz (the VAE's / autoencoder's decoder) also dL/dz [n, z] fp32.  The upstream of the pre-sigmoid output,
         dimages G(z) (1 - G(z)), is rounded to bf16 once (gm_image_to_rows)."""
-        self._check_live(handle, "Decoder" if self.variant in ("vae", "ae") else "Generator")
+        self._check_live(handle)
         sv, n = handle["sv"], handle["n"]
         dpre = self.image_to_rows(dimages, sv["img"], self._buf("cgdpre", n * 4096, self.ch))
         grads = torch.zeros(self.G.total, device=self.device)

@@ -228,18 +228,9 @@ class GanEngine:
         check(self.h, lib().gm_gan_materialize_grads(self.g, _stream()))
 
     # ---- custom-loss path (README.md:31): forward / backward halves as separate calls
-    g_generation = 0
-    d_calls = 0
-
     @property
     def supports_custom_loss(self):
         return self.variant not in ("began",)        # BEGAN's D is an autoencoder (src/be_gan.py:63-76)
-
-    @property
-    def d_generation(self):
-        if not hasattr(self, "_d_generation"):
-            self._d_generation = [0] * self.num_slots()
-        return self._d_generation
 
     def num_slots(self):
         return lib().gm_gan_num_slots(self.g)

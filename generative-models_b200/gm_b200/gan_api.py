@@ -209,15 +209,15 @@ class _GForward(torch.autograd.Function):
     @staticmethod
     def forward(ctx, noise, engine, *params):
         ctx.engine, ctx.params = engine, params
-        engine.g_generation += 1
-        ctx.generation = engine.g_generation
+        ctx.ring = slot_ring(engine, "Generator", 1)
+        ctx.slot, ctx.gen = ctx.ring.take()
         return engine.g_forward(noise)
 
     @staticmethod
     @once_differentiable        # the backward is a CUDA kernel chain: a create_graph=True caller gets an error, not a silently missing term
     def backward(ctx, dimages):
         eng = ctx.engine
-        if eng.g_generation != ctx.generation:
+        if not ctx.ring.live(ctx.slot, ctx.gen):
             raise RuntimeError("Generator activations were overwritten by a later Generator.forward: "
                                "back-propagate a G output before calling G again")
         if getattr(ctx, "consumed", False):
@@ -236,17 +236,15 @@ class _DForward(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, engine, *params):
         ctx.engine, ctx.params = engine, params
-        ctx.slot = engine.d_calls % engine.num_slots()
-        engine.d_calls += 1
-        engine.d_generation[ctx.slot] = engine.d_calls
-        ctx.generation = engine.d_calls
+        ctx.ring = slot_ring(engine, "Discriminator", engine.num_slots())
+        ctx.slot, ctx.gen = ctx.ring.take()
         return engine.d_forward(ctx.slot, x).view(-1, 1)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dscore):
         eng = ctx.engine
-        if eng.d_generation[ctx.slot] != ctx.generation:
+        if not ctx.ring.live(ctx.slot, ctx.gen):
             raise RuntimeError("Discriminator activations were overwritten: at most %d Discriminator.forward "
                                "results can await their backward (construct the engine with a gradient-penalty "
                                "variant for more)" % eng.num_slots())
@@ -382,9 +380,32 @@ def compute_batch_evaluate(tr, iterator, two_losses):
     return float(np.mean(loss))
 
 
+def grow_engine(tr, batch, make):
+    """A VAE-family trainer tr's engine rebuilt for batch rows (at least its current size and 64) by make(max_batch): the
+    model's parameters become views of the new engine's fp32 master weights, the Adam moments and steps carry over, and
+    the per-call slots of the old engine are retired"""
+    m, old = tr.model, tr._engine
+    batch = max(batch, tr._max_batch, 64)
+    eng = make(batch)
+    named = dict(m.named_parameters())
+    eng.load({k: v.data for k, v in named.items()})
+    views = eng.views()
+    for k, p in named.items():
+        p.data = views[k]                      # nn.Parameter storage == the engine's fp32 master weights
+    if old is not None:
+        eng.exp_avg.copy_(old.exp_avg)
+        eng.exp_avg_sq.copy_(old.exp_avg_sq)
+        eng.steps = old.steps
+        for ring in getattr(old, "rings", {}).values():
+            ring.retire()
+    tr._engine, tr._max_batch = eng, batch
+    return eng
+
+
 class SlotRing:
-    """The per-call slots of one engine's encoder or decoder: take() hands them out round robin, numbering the calls; a
-    backward whose slot a later call took, or whose engine was replaced (retire(): a larger batch), raises"""
+    """The per-call slots of one engine's generator, discriminator, encoder or decoder: take() hands them out round robin,
+    numbering the calls; a backward whose slot a later call took, or whose engine was replaced (retire(): a larger batch),
+    raises"""
 
     def __init__(self, n, what):
         self.n, self.what, self.calls, self.gen, self.retired = n, what, 0, [0] * n, False
@@ -394,6 +415,9 @@ class SlotRing:
         slot = (self.calls - 1) % self.n
         self.gen[slot] = self.calls
         return slot, self.calls
+
+    def live(self, slot, gen):
+        return not self.retired and self.gen[slot] == gen
 
     def check(self, slot, gen):
         if self.retired:
@@ -407,25 +431,54 @@ class SlotRing:
         self.retired = True
 
 
-class _FusedLoss(torch.autograd.Function):
-    """0-dim loss whose backward() hands the gradients the fused kernels already
-    computed to the parameters' .grad (the reference calls loss.backward() then
-    optimizer.step(), src/ns_gan.py:138-139)."""
+def slot_ring(eng, what, n):
+    """eng's SlotRing of per-call `what` slots, made with n slots on first use"""
+    rings = eng.__dict__.setdefault("rings", {})
+    if what not in rings:
+        rings[what] = SlotRing(n, what)
+    return rings[what]
+
+
+class EngineCall(torch.autograd.Function):
+    """One call of an engine-backed module under grad mode: fwd(x) -> (outputs, handle) runs the forward kernels,
+    bwd(handle, upstream gradients, need_dx) -> (dL/dx or None, the gradients of params in their order) the backward
+    ones; autograd only routes the upstream in and the gradients out"""
 
     @staticmethod
-    def forward(ctx, flat_params, loss_val, flat_grad, param_list):
-        ctx.flat_grad, ctx.param_list = flat_grad, param_list
+    def forward(ctx, x, fwd, bwd, *params):
+        out, ctx.handle = fwd(x)
+        ctx.bwd = bwd
+        return out
+
+    @staticmethod
+    @first_order
+    @once_differentiable        # the backward is a kernel chain: create_graph=True gets an error, not a missing term
+    def backward(ctx, *grads):
+        dx, param_grads = ctx.bwd(ctx.handle, grads, ctx.needs_input_grad[0])
+        return (dx, None, None, *param_grads)
+
+
+class GradHandoff(torch.autograd.Function):
+    """A loss whose backward() adds gradients the fused kernels already computed, times the upstream, to the parameters'
+    .grad (the reference calls loss.backward() then optimizer.step(), src/ns_gan.py:138-139).  pairs: (parameter, its
+    gradient) - a view of an engine buffer is read when backward() runs, a copy keeps the values of the call."""
+
+    @staticmethod
+    def forward(ctx, anchor, loss_val, pairs):
+        ctx.pairs = pairs
         return loss_val.clone()
 
     @staticmethod
     def backward(ctx, gout):
-        off = 0
-        for p in ctx.param_list:
-            n = p.numel()
-            g = ctx.flat_grad[off:off + n].view_as(p) * gout
+        for p, g in ctx.pairs:
+            g = g.view_as(p) * gout
             p.grad = g if p.grad is None else p.grad + g
-            off += n
-        return None, None, None, None
+        return None, None, None
+
+
+def flat_pairs(params, flat):
+    """(parameter, its slice of the flat gradient buffer flat, as a view) for GradHandoff"""
+    return list(zip(params, flat.split([p.numel() for p in params])))
 
 
 class _StepGraph:
@@ -554,7 +607,7 @@ class GANTrainerBase:
     def _loss_tensor(self, net, loss_val):
         eng = self._engine
         params = list((self.model.G if net == G_NET else self.model.D).parameters())
-        return _FusedLoss.apply(eng.params[net].detach().requires_grad_(True), loss_val, eng.grads[net], params)
+        return GradHandoff.apply(eng.params[net].detach().requires_grad_(True), loss_val, flat_pairs(params, eng.grads[net]))
 
     # ------------------------------------------------------------------ reference surface
     def train(self, num_epochs, G_lr=2e-4, D_lr=2e-4, D_steps=1, **extra):

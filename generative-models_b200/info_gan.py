@@ -12,7 +12,7 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import parallel as par
 from gm_b200 import AdamHP, GmError, InfoGanEngine
-from gm_b200.gan_api import builtin_step, Generator as _Generator, Discriminator as _Discriminator, GANTrainerBase, _FusedLoss, to_cuda, G_NET, D_NET
+from gm_b200.gan_api import builtin_step, Generator as _Generator, Discriminator as _Discriminator, GANTrainerBase, GradHandoff, flat_pairs, to_cuda, G_NET, D_NET
 
 
 class Generator(_Generator):
@@ -173,7 +173,7 @@ class InfoGANTrainer(GANTrainerBase):
         loss = eng.q_grad(images.shape[0], noise.float().contiguous())
         params = list(m.G.parameters()) + list(m.Q.parameters())
         flat = torch.cat([eng.grads[G_NET], eng.q_grads])
-        return _FusedLoss.apply(flat.detach().requires_grad_(True), loss, flat, params)
+        return GradHandoff.apply(flat.detach().requires_grad_(True), loss, flat_pairs(params, flat))
 
     def compute_noise(self, batch_size, z_dim, disc_dim=None, cont_dim=None, c=None):
         """ src/info_gan.py:306-325: z, a uniformly drawn one-hot code, a Gaussian code """

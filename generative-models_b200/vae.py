@@ -13,11 +13,10 @@ import torch
 import torch.nn as nn
 
 from utils import *  # noqa: F401,F403
-from torch.autograd.function import once_differentiable
 
 from gm_b200 import AdamHP, GmError, VaeEngine
-from gm_b200.gan_api import (to_cuda, builtin_step, first_order, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
-                             compute_batch_evaluate, SlotRing)
+from gm_b200.gan_api import (to_cuda, builtin_step, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
+                             compute_batch_evaluate, slot_ring, EngineCall, GradHandoff, grow_engine)
 
 
 def _engine_of(module, what, batch):
@@ -27,63 +26,6 @@ def _engine_of(module, what, batch):
     if parent is None:
         raise GmError(what + " is not part of a VAE: construct it through VAE(...)")
     return parent._engine_for(batch, what)
-
-
-def _ring(eng, what):
-    """the engine's SlotRing of per-call Encoder / Decoder slots"""
-    rings = eng.__dict__.setdefault("rings", {})
-    if what not in rings:
-        rings[what] = SlotRing(eng.num_slots(), what)
-    return rings[what]
-
-
-def _check_no_dx(ctx):
-    if ctx.needs_input_grad[0]:
-        raise RuntimeError("the gradient with respect to the encoder's input is not computed")
-
-
-class _EncoderCall(torch.autograd.Function):
-    """Encoder.forward under grad mode: (mu, log_var) and their backward on the CUDA kernels (gm_vae_encoder_forward /
-    _backward); autograd routes dL/dmu, dL/dlog_var in and the encoder's parameter gradients out"""
-
-    @staticmethod
-    def forward(ctx, x, eng, names, *params):
-        ctx.slot, ctx.gen = _ring(eng, "Encoder").take()
-        ctx.eng, ctx.names, ctx.n = eng, names, x.shape[0]
-        return eng.encoder_forward(ctx.slot, x)
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, dmu, dlog_var):
-        _check_no_dx(ctx)
-        _ring(ctx.eng, "Encoder").check(ctx.slot, ctx.gen)
-        g = ctx.eng.encoder_backward(ctx.slot, ctx.n, dmu, dlog_var)
-        return (None, None, None, *[g["encoder." + k] for k in ctx.names])
-
-
-class _DecoderCall(torch.autograd.Function):
-    """Decoder.forward under grad mode: the images and their backward (gm_vae_decoder_forward / _backward), with dL/dz
-    when z requires grad (z = reparameterize(mu, log_var))"""
-
-    @staticmethod
-    def forward(ctx, z, eng, names, *params):
-        ctx.slot, ctx.gen = _ring(eng, "Decoder").take()
-        ctx.eng, ctx.names, ctx.n = eng, names, z.shape[0]
-        return eng.decoder_forward(ctx.slot, z)
-
-    @staticmethod
-    @first_order
-    @once_differentiable
-    def backward(ctx, dimages):
-        _ring(ctx.eng, "Decoder").check(ctx.slot, ctx.gen)
-        g, dz = ctx.eng.decoder_backward(ctx.slot, ctx.n, dimages, ctx.needs_input_grad[0])
-        return (dz, None, None, *[g["decoder." + k] for k in ctx.names])
-
-
-def _node_args(mod):
-    names, params = zip(*mod.named_parameters())
-    return (names,) + params
 
 
 class Encoder(nn.Module):
@@ -98,8 +40,21 @@ class Encoder(nn.Module):
     def forward(self, x):
         x = to_cuda(x).float()
         eng = _engine_of(self, "Encoder", x.shape[0])
-        if torch.is_grad_enabled():
-            return _EncoderCall.apply(x, eng, *_node_args(self))
+        if torch.is_grad_enabled():                # (mu, log_var) and their backward: gm_vae_encoder_forward / _backward
+            ring, n = slot_ring(eng, "Encoder", eng.num_slots()), x.shape[0]
+            names, params = zip(*self.named_parameters())
+
+            def forward(x):
+                slot, gen = ring.take()
+                return eng.encoder_forward(slot, x), (slot, gen)
+
+            def backward(handle, grads, need_dx):
+                if need_dx:
+                    raise RuntimeError("the gradient with respect to the encoder's input is not computed")
+                ring.check(*handle)
+                g = eng.encoder_backward(handle[0], n, *grads)
+                return None, [g["encoder." + k] for k in names]
+            return EngineCall.apply(x, forward, backward, *params)
         _, mu, lv, _ = eng.forward(x, want_images=False)
         return mu, lv
 
@@ -117,8 +72,19 @@ class Decoder(nn.Module):
         if z.dim() == 1:                       # the reference decodes single latent vectors too (src/vae.py:289-290)
             z = z.view(1, -1)
         eng = _engine_of(self, "Decoder", z.shape[0])
-        if torch.is_grad_enabled():
-            return _DecoderCall.apply(z.float(), eng, *_node_args(self))
+        if torch.is_grad_enabled():                # the images and their backward, with dL/dz when z requires grad
+            ring, n = slot_ring(eng, "Decoder", eng.num_slots()), z.shape[0]
+            names, params = zip(*self.named_parameters())
+
+            def forward(z):
+                slot, gen = ring.take()
+                return eng.decoder_forward(slot, z), (slot, gen)
+
+            def backward(handle, grads, need_dz):
+                ring.check(*handle)
+                g, dz = eng.decoder_backward(handle[0], n, grads[0], need_dz)
+                return dz, [g["decoder." + k] for k in names]
+            return EngineCall.apply(z.float(), forward, backward, *params)
         return eng.decode(z)
 
 
@@ -180,22 +146,6 @@ class VAE(nn.Module):
         return mu + epsilon * torch.exp(log_var / 2)
 
 
-class _VaeLoss(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, anchor, val, which, holder):
-        ctx.which, ctx.holder = which, holder
-        return val.clone()
-
-    @staticmethod
-    def backward(ctx, gout):
-        # (recon + kl).backward(): the fused kernels produced d(recon + kl)/dtheta once; deliver
-        # it with the recon term and nothing with the kl term (the reference always sums them)
-        if ctx.which == 0:
-            for p, g in ctx.holder():
-                p.grad = g * gout if p.grad is None else p.grad + g * gout
-        return None, None, None, None
-
-
 class VAETrainer:
     device_noise = True        # in-kernel Philox eps + resident dataset in train(); False: the reference's host draws
 
@@ -217,22 +167,8 @@ class VAETrainer:
     def _ensure_engine(self, batch):
         if self._engine is not None and batch <= self._max_batch:
             return self._engine
-        m, old = self.model, self._engine
-        batch = max(batch, self._max_batch, 64)
-        eng = VaeEngine(m.image_size, m.hidden_dim, m.z_dim, max_batch=batch)
-        named = dict(m.named_parameters())
-        eng.load({k: v.data for k, v in named.items()})
-        views = eng.views()
-        for k, p in named.items():
-            p.data = views[k]
-        if old is not None:
-            eng.exp_avg.copy_(old.exp_avg)
-            eng.exp_avg_sq.copy_(old.exp_avg_sq)
-            eng.steps = old.steps
-            for ring in getattr(old, "rings", {}).values():
-                ring.retire()
-        self._engine, self._max_batch = eng, batch
-        return eng
+        m = self.model
+        return grow_engine(self, batch, lambda rows: VaeEngine(m.image_size, m.hidden_dim, m.z_dim, max_batch=rows))
 
     def train(self, num_epochs, lr=1e-3, weight_decay=1e-5):
         """ Train a Variational Autoencoder (src/vae.py:127-191): a true epoch over train_iter,
@@ -310,11 +246,12 @@ class VAETrainer:
         eps = to_cuda(torch.randn(images.shape[0], self.model.z_dim))
         losses = eng.grad(images, eps=eps, seed=self._seed, step=self._step).clone()
         self._step += 1
-        named = dict(self.model.named_parameters())
         gviews = eng.views(eng.grads)
-        holder = lambda: [(named[k], gviews[k]) for k in named]     # noqa: E731
+        pairs = [(p, gviews[k]) for k, p in self.model.named_parameters()]
         anchor = losses.detach().requires_grad_(True)
-        return _VaeLoss.apply(anchor, losses[0], 0, holder), _VaeLoss.apply(anchor, losses[1], 1, holder)
+        # the fused kernels produced d(recon + kl)/dtheta once: the recon term delivers it, the kl term nothing (the
+        # reference always back-propagates their sum)
+        return GradHandoff.apply(anchor, losses[0], pairs), GradHandoff.apply(anchor, losses[1], [])
 
     def kl_divergence(self, mu, log_var):
         """ src/vae.py:210-212 (torch, for direct use) """
