@@ -23,16 +23,21 @@ struct gm_ctx {
   int num_sms = 0;
   PFN_encodeTiled encode = nullptr;
   std::string err;
-  long long launches = 0;
+  long long launches = 0;     // kernels launched by this context (counted by launch() only; gm_launch_count)
+  // Run-time switches, read from the environment by gm_ctx_create:
+  bool pdl = true;            // programmatic stream serialisation on every launch (GM_NO_PDL=1 off; gm_ctx_set_pdl)
+  bool tma_store = true;      // GM_NO_TMA_STORE=1: epilogue stores through LDS + STG only
+  bool tn208 = true;          // GM_TN208=0: every wide TN plan takes the 256-wide tile (the previous route)
   float* scratch = nullptr;   // split-K partials for the generic gm_gemm_bf16
   size_t scratch_bytes = 0;
-  // optional per-launch GEMM timing (bench.py roofline): CUDA events on the launch stream
-  bool prof = false;
   void* red = nullptr;        // scratch of the conv building blocks' two-stage reductions (engine_conv.inl)
   size_t red_bytes = 0;
   void* loss_zero = nullptr;  // 64 zero bytes: bias / Fisher state / completion counter for gm_loss_rows
   long long plan_lo = 0;      // > 0 while an engine in split-operand mode builds its plans: element offset of the lo planes
-  struct ProfRec { cudaEvent_t e0, e1; int kind; double flops; };
+  // gm_prof_enable: 0 off, 1 CUDA events around every GEMM launch (gm_prof_collect sums them by plan kind), 2 around every
+  // launch (gm_prof_report sums them by kernel name: in-stream durations including the launch gaps)
+  int prof = 0;
+  struct ProfRec { const char* name; int kind; double flops; cudaEvent_t e0, e1; };   // name: level 2 only; kind -1: not a GEMM
   std::vector<ProfRec> prof_recs;
 };
 
@@ -111,130 +116,159 @@ struct GemmPlan {
   double flops;   // algorithmic 2*M*N*K of the logical problem (no padding)
 };
 
-// Every kernel of the library is launched with programmatic stream serialisation: the grid
-// may become resident while its predecessor drains, and blocks in griddepcontrol.wait (first
-// statement of every kernel, after the prologue in the GEMM) until the predecessor completed.
-static bool g_pdl = true;   // GM_NO_PDL=1 turns it off (gm_ctx_create)
-static bool g_tma_store = true;   // GM_NO_TMA_STORE=1: epilogue stores through LDS + STG only
-static bool g_tn208 = true;       // GM_TN208=0: every wide TN plan takes the 256-wide tile (the previous route)
-// GM_PROF_ALL / gm_prof_enable(ctx, 2): CUDA events around EVERY launch on its stream, aggregated per kernel name by
-// gm_prof_report (in-stream durations including the launch gaps ncu's serialised per-kernel times cannot show)
-struct ProfAll { const char* name; cudaEvent_t e0, e1; };
-static bool g_prof_all = false;
-static std::vector<ProfAll> g_prof_all_recs;
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
-  struct Scope {
-    cudaStream_t s; ProfAll r; bool on;
-    Scope(const char* n, cudaStream_t s_) : s(s_), on(g_prof_all) {
-      if (on) { r.name = n; cudaEventCreate(&r.e0); cudaEventCreate(&r.e1); cudaEventRecord(r.e0, s); }
-    }
-    ~Scope() { if (on) { cudaEventRecord(r.e1, s); g_prof_all_recs.push_back(r); } }
-  } scope(name, s);
-  // xhat_kernel never takes the attribute: launched early behind the generator's output GEMM its CTAs would pile up on
-  // the first SMs that GEMM frees instead of spreading over the whole chip
-  const bool pdl = g_pdl && strcmp(name, "xhat_kernel") != 0;
+// Profile name of a GEMM launch: plan kind and epilogue signature, output type, K class, split (interned)
+static const char* gemm_name(const GemmPlan& pl) {
+  static const char* kKind[4] = {"gemm_nt208", "gemm_nt64", "gemm_tn", "gemm_tn64"};
+  static std::map<int, std::string> names;
+  const GemmParams& q = pl.p;
+  const bool f32 = q.epi == EPI_F32, klong = q.K >= 512, split = q.nparts == 3;
+  const int key = epi_sig(q) | (pl.kind | f32 << 2 | klong << 3 | split << 4 | (pl.bn == 208) << 5) << kEpiSigBits;
+  auto it = names.find(key);
+  if (it == names.end()) {
+    char buf[128];
+    char kind[32];
+    snprintf(kind, sizeof kind, pl.kind == PK_TN_256 ? "%s%d" : "%s", kKind[pl.kind], pl.bn);
+    snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kind, q.act, q.aux_mode, q.bias ? " bias" : "",
+             dot_has_w(q.dot) ? " dot" : "", q.dot == DOT_W_PRE ? " pre" : (q.dot == DOT_W_MASK ? " mask" : ""),
+             q.dot == DOT_SQ ? " sq" : "", f32 ? " f32" : "", klong ? "long" : "short", split ? " split" : "");
+    it = names.emplace(key, buf).first;
+  }
+  return it->second.c_str();
+}
+
+// What launch() accounts a kernel as: its name (a GEMM is named by its plan), whether it takes programmatic stream
+// serialisation, and for a GEMM its plan (kind and FLOPs for gm_prof_collect) and cluster size.
+struct KernelTag {
+  const char* name;
+  bool pdl = true;
+  const GemmPlan* plan = nullptr;
+  int cluster = 1;
+  KernelTag(const char* n, bool pdl_ = true) : name(n), pdl(pdl_) {}
+  KernelTag(const GemmPlan& pl, int cl) : name(nullptr), plan(&pl), cluster(cl) {}
+};
+
+// Launch configuration; `at` receives its attributes.  With `pdl` the grid may become resident while its predecessor
+// drains, and blocks in griddepcontrol.wait (first statement of every kernel, after the prologue in the GEMM) until the
+// predecessor completed.
+static cudaLaunchConfig_t launch_cfg(dim3 grid, dim3 block, size_t smem, cudaStream_t s, int cluster, bool pdl,
+                                     cudaLaunchAttribute (&at)[2]) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+  if (cluster > 1) {
+    at[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+    at[cfg.numAttrs].val.clusterDim.x = cluster;
+    at[cfg.numAttrs].val.clusterDim.y = 1;
+    at[cfg.numAttrs].val.clusterDim.z = 1;
+    ++cfg.numAttrs;
+  }
+  if (pdl) {
+    at[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    ++cfg.numAttrs;
+  }
+  return cfg;
+}
+
+// Every kernel of the library is launched here: a failed launch ends the entry point with GM_ERR_CUDA (nothing after it
+// is enqueued), a successful one is counted (gm_launch_count) and, when the context's profiling level asks for it, timed.
+template <typename... KArgs, typename... Args>
+[[nodiscard]] static int launch(gm_ctx* c, const KernelTag& k, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                                cudaStream_t s, Args&&... args) {
+  cudaLaunchAttribute at[2];
+  const cudaLaunchConfig_t cfg = launch_cfg(grid, block, smem, s, k.cluster, k.pdl && c->pdl, at);
+  const bool timed = c->prof == 2 || (c->prof == 1 && k.plan);
+  gm_ctx::ProfRec r;
+  if (timed) {
+    r.name = c->prof == 2 ? (k.plan ? gemm_name(*k.plan) : k.name) : nullptr;
+    r.kind = k.plan ? k.plan->kind : -1;
+    r.flops = k.plan ? k.plan->flops : 0.0;
+    CU_OK(c, cudaEventCreate(&r.e0));
+    CU_OK(c, cudaEventCreate(&r.e1));
+    CU_OK(c, cudaEventRecord(r.e0, s));
+  }
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+  if (e != cudaSuccess) {
+    cudaGetLastError();   // a launch error is not sticky: leave no trace of it for the caller's next runtime call
+    if (timed) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
+    return fail(c, GM_ERR_CUDA, "%s launch failed: %s", k.plan ? gemm_name(*k.plan) : k.name, cudaGetErrorString(e));
+  }
+  c->launches++;
+  if (timed) {
+    c->prof_recs.push_back(r);
+    CU_OK(c, cudaEventRecord(r.e1, s));
+  }
+  return GM_OK;
 }
 
 template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false,
           int CL = kGemmCluster<BN, AMN, BMN>>
-static cudaError_t launch_inst(const GemmPlan& pl, cudaStream_t s) {
+static int launch_inst(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   using Cfg = GemmCfg<BN, !AMN, PP>;
   auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP, CL>;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof cfg);
-  cfg.gridDim = dim3(pl.grid);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = s;
-  cudaLaunchAttribute at[2];
-  int na = 0;
-  if (CL > 1) {
-    at[na].id = cudaLaunchAttributeClusterDimension;
-    at[na].val.clusterDim.x = CL;
-    at[na].val.clusterDim.y = 1;
-    at[na].val.clusterDim.z = 1;
-    ++na;
-  }
   // the opt-in to > 48 KB dynamic shared memory is per (function, device); so is the number of clusters that fit at once
   static bool configured[64] = {};
   static int max_clusters[64] = {};
   int dev = 0;
-  cudaGetDevice(&dev);
+  CU_OK(c, cudaGetDevice(&dev));
   const bool cached = dev >= 0 && dev < 64;
   int mc = cached ? max_clusters[dev] : 0;
   if (!cached || !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
+    CU_OK(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     if (CL > 1) {
-      cfg.gridDim = dim3(CL);
-      cfg.attrs = at;
-      cfg.numAttrs = na;
-      e = cudaOccupancyMaxActiveClusters(&mc, kern, &cfg);
-      if (e != cudaSuccess) return e;
-      if (mc < 1) return cudaErrorInvalidConfiguration;
+      cudaLaunchAttribute at[2];
+      const cudaLaunchConfig_t cfg = launch_cfg(dim3(CL), dim3(kGemmThreads), Cfg::SMEM_BYTES, s, CL, false, at);
+      CU_OK(c, cudaOccupancyMaxActiveClusters(&mc, kern, &cfg));
+      if (mc < 1) return fail(c, GM_ERR_CUDA, "%s: no %d-CTA cluster fits on device %d", gemm_name(pl), CL, dev);
     }
     if (cached) { max_clusters[dev] = mc; configured[dev] = true; }
   }
+  dim3 grid(pl.grid);
   if (CL > 1) {
     // persistent: one cluster per item, up to the clusters the device holds at once (a GPC may hold an odd number of SMs).
     // K-major clusters pair m-tiles, MN-major ones n-tiles (of an even count)
     const GemmParams& q = pl.p;
     const int items = (BMN ? q.m_tiles * (q.n_tiles / CL) : cdiv(q.m_tiles, CL) * q.n_tiles) * q.splits;
-    cfg.gridDim = dim3(CL * (items < mc ? items : mc));
+    grid = dim3(CL * (items < mc ? items : mc));
   }
-  if (g_pdl) {
-    at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = at;
-  cfg.numAttrs = na;
   GemmParams prm = pl.p;
   prm.tma_store = pl.tmc_state == 1 ? 1 : 0;
   // fp32 rows take float4 stores only where every row of every split starts on 16 bytes (ldc = 30: row 1 is at byte 120)
   prm.f32_vec = prm.epi == EPI_F32 && !(reinterpret_cast<uintptr_t>(prm.part) & 15) && prm.ldp % 4 == 0 && prm.part_stride % 4 == 0;
-  return cudaLaunchKernelEx(&cfg, kern, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2, pl.tmBt, pl.tmB2t, prm);
+  return launch(c, KernelTag(pl, CL), kern, grid, kGemmThreads, Cfg::SMEM_BYTES, s, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2,
+                pl.tmBt, pl.tmB2t, prm);
 }
 
 // TN kind: the 256-wide tile, or the 208-wide one as 2-CTA clusters over n-tile pairs (an even n-tile count, plan_gemm)
 template <bool SPLIT>
-static cudaError_t launch_tn(const GemmPlan& pl, cudaStream_t s) {
-  if (pl.bn == 256) return launch_inst<256, true, true, kEpiUniversal, SPLIT>(pl, s);
-  return launch_inst<208, true, true, kEpiUniversal, SPLIT, false, 2>(pl, s);
+static int launch_tn(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
+  if (pl.bn == 256) return launch_inst<256, true, true, kEpiUniversal, SPLIT>(c, pl, s);
+  return launch_inst<208, true, true, kEpiUniversal, SPLIT, false, 2>(c, pl, s);
 }
 
 // split-operand plans (gm_prec GM_PREC_SPLIT): the universal epilogue with the residual-plane paths compiled in
 template <int BN, bool AMN, bool BMN>
-static cudaError_t launch_split(const GemmPlan& pl, cudaStream_t s) {
-  return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(pl, s);
+static int launch_split(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
+  return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(c, pl, s);
 }
 
 constexpr int kPingPongMaxKblocks = 7;   // K <= 448
 
 // K-major 128x208 kernel: the compile-time-specialised instance of the plan's epilogue signature when the train steps use
 // that signature, else the universal instance.
-static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
+static int launch_nt208(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   const GemmParams& p = pl.p;
-  if (p.epi != EPI_BF16) return launch_inst<208, false, false>(pl, s);
+  if (p.epi != EPI_BF16) return launch_inst<208, false, false>(c, pl, s);
   // Short-K bias + activation GEMMs (G's two layers) are epilogue-bound: their consumer warpgroups run in ping-pong, so
   // each half-tile's epilogue hides under the other warpgroup's wgmma.  Ping-pong loads the B tile once per 64-row half;
   // from 8 k-blocks on, and with aux / row-dot epilogues, that extra feed cost more than it hid (DESIGN §5).
   const bool pp = p.kblocks <= kPingPongMaxKblocks;
-#define NT208(S) case S: return launch_inst<208, false, false, S>(pl, s)
-#define NT208_PINGPONG(S) case S: return pp ? launch_inst<208, false, false, S, false, true>(pl, s) : launch_inst<208, false, false, S>(pl, s)
+#define NT208(S) case S: return launch_inst<208, false, false, S>(c, pl, s)
+#define NT208_PINGPONG(S) case S: return pp ? launch_inst<208, false, false, S, false, true>(c, pl, s) : launch_inst<208, false, false, S>(c, pl, s)
   switch (epi_sig(p)) {
     NT208_PINGPONG(epi_sig(ACT_RELU, AUX_NONE, true, DOT_NONE));
     NT208_PINGPONG(epi_sig(ACT_SIGMOID, AUX_NONE, true, DOT_NONE));
@@ -248,78 +282,40 @@ static cudaError_t launch_nt208(const GemmPlan& pl, cudaStream_t s) {
     NT208(epi_sig(ACT_NONE, AUX_NONZERO_MASK, false, DOT_NONE));
     NT208(epi_sig(ACT_NONE, AUX_L1, true, DOT_NONE));
     NT208(epi_sig(ACT_SIGMOID, AUX_VAE_OUT, true, DOT_NONE));
-    default: return launch_inst<208, false, false>(pl, s);
+    default: return launch_inst<208, false, false>(c, pl, s);
   }
 #undef NT208
 #undef NT208_PINGPONG
 }
 
-static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
+[[nodiscard]] static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   if (pl.tmc_state == 0) {
     const GemmParams& p = pl.p;
     const bool nt = pl.kind == PK_NT_208 || pl.kind == PK_NT_64;
     pl.tmc_state = 2;
     // the bulk store serves the pure activation epilogues only; the aux / row-dot epilogues keep LDS + STG
     // (a fence + wait for the bulk store would sit in their longer per-block dependency chain)
-    if (g_tma_store && nt && epi_plain(p.aux_mode, p.dot) && p.nparts == 1 && p.epi == EPI_BF16 && p.out != nullptr && !(reinterpret_cast<uintptr_t>(p.out) & 15) &&
+    if (c->tma_store && nt && epi_plain(p.aux_mode, p.dot) && p.nparts == 1 && p.epi == EPI_BF16 && p.out != nullptr && !(reinterpret_cast<uintptr_t>(p.out) & 15) &&
         (p.ldo * 2) % 16 == 0 && p.out_cols > 0) {
       int rc = make_tmap(c, &pl.tmC, p.out, uint64_t(p.out_cols), uint64_t(p.M), uint64_t(p.ldo), kEpiCols, kEpiRows, CU_TENSOR_MAP_SWIZZLE_64B);
       if (rc) return rc;
       pl.tmc_state = 1;
     }
   }
-  cudaError_t e;
-  gm_ctx::ProfRec rec;
-  ProfAll pa;
-  if (g_prof_all) {
-    static const char* kKind[4] = {"gemm_nt208", "gemm_nt64", "gemm_tn", "gemm_tn64"};
-    static std::map<int, std::string> names;   // interned: epilogue signature + kind, output type, K class, split
-    const GemmParams& q = pl.p;
-    const bool f32 = q.epi == EPI_F32, klong = q.K >= 512, split = q.nparts == 3;
-    const int key = epi_sig(q) | (pl.kind | f32 << 2 | klong << 3 | split << 4 | (pl.bn == 208) << 5) << kEpiSigBits;
-    auto it = names.find(key);
-    if (it == names.end()) {
-      char buf[128];
-      char kind[32];
-      snprintf(kind, sizeof kind, pl.kind == PK_TN_256 ? "%s%d" : "%s", kKind[pl.kind], pl.bn);
-      snprintf(buf, sizeof buf, "%s[act%d aux%d%s%s%s%s%s K%s%s]", kind, q.act, q.aux_mode, q.bias ? " bias" : "",
-               dot_has_w(q.dot) ? " dot" : "", q.dot == DOT_W_PRE ? " pre" : (q.dot == DOT_W_MASK ? " mask" : ""),
-               q.dot == DOT_SQ ? " sq" : "", f32 ? " f32" : "", klong ? "long" : "short", split ? " split" : "");
-      it = names.emplace(key, buf).first;
-    }
-    pa.name = it->second.c_str();
-    cudaEventCreate(&pa.e0); cudaEventCreate(&pa.e1);
-    cudaEventRecord(pa.e0, s);
-  }
-  if (c->prof) {
-    cudaEventCreate(&rec.e0);
-    cudaEventCreate(&rec.e1);
-    rec.kind = pl.kind;
-    rec.flops = pl.flops;
-    cudaEventRecord(rec.e0, s);
-  }
   if (pl.p.nparts == 3) {
     switch (pl.kind) {
-      case PK_NT_208: e = launch_split<208, false, false>(pl, s); break;
-      case PK_NT_64: e = launch_split<64, false, false>(pl, s); break;
-      case PK_TN_256: e = launch_tn<true>(pl, s); break;
-      default: e = launch_split<64, true, true>(pl, s); break;
+      case PK_NT_208: return launch_split<208, false, false>(c, pl, s);
+      case PK_NT_64: return launch_split<64, false, false>(c, pl, s);
+      case PK_TN_256: return launch_tn<true>(c, pl, s);
+      default: return launch_split<64, true, true>(c, pl, s);
     }
-  } else
+  }
   switch (pl.kind) {
-    case PK_NT_208: e = launch_nt208(pl, s); break;
-    case PK_NT_64: e = launch_inst<64, false, false>(pl, s); break;
-    case PK_TN_256: e = launch_tn<false>(pl, s); break;
-    default: e = launch_inst<64, true, true>(pl, s); break;
+    case PK_NT_208: return launch_nt208(c, pl, s);
+    case PK_NT_64: return launch_inst<64, false, false>(c, pl, s);
+    case PK_TN_256: return launch_tn<false>(c, pl, s);
+    default: return launch_inst<64, true, true>(c, pl, s);
   }
-  c->launches++;
-  if (c->prof) {
-    cudaEventRecord(rec.e1, s);
-    c->prof_recs.push_back(rec);
-  }
-  if (g_prof_all) { cudaEventRecord(pa.e1, s); g_prof_all_recs.push_back(pa); }
-  if (e != cudaSuccess) return fail(c, GM_ERR_CUDA, "GEMM launch failed: %s", cudaGetErrorString(e));
-  return GM_OK;
 }
 
 // mode 0 (NT): A [M, lda] K-contiguous, B [N, ldb] K-contiguous.
@@ -347,7 +343,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     // one slowed the DCGAN step (DESIGN §5)
     const int n208 = cdiv(ncover, 208);
     if (ncover <= 64) { pl->kind = PK_TN_64; bn = 64; }
-    else { pl->kind = PK_TN_256; bn = g_tn208 && n208 % 2 == 0 && n208 <= cdiv(ncover, 256) ? 208 : 256; }
+    else { pl->kind = PK_TN_256; bn = c->tn208 && n208 % 2 == 0 && n208 <= cdiv(ncover, 256) ? 208 : 256; }
     int rc = make_tmap(c, &pl->tmA, A, M, K, lda, 64, BK);
     if (rc) return rc;
     rc = make_tmap(c, &pl->tmB, B, N, K, ldb, 64, BK);
@@ -437,11 +433,11 @@ extern "C" int gm_ctx_create(int device, gm_ctx** out) {
   if (!fn || q != cudaDriverEntryPointSuccess) return fail(c, GM_ERR_CUDA, "cuTensorMapEncodeTiled not available");
   c->encode = reinterpret_cast<PFN_encodeTiled>(fn);
   const char* np = getenv("GM_NO_PDL");
-  g_pdl = !(np && np[0] == '1');
+  c->pdl = !(np && np[0] == '1');
   const char* nts = getenv("GM_NO_TMA_STORE");
-  g_tma_store = !(nts && nts[0] == '1');
+  c->tma_store = !(nts && nts[0] == '1');
   const char* tn = getenv("GM_TN208");
-  g_tn208 = !(tn && tn[0] == '0');
+  c->tn208 = !(tn && tn[0] == '0');
   return GM_OK;
 }
 extern "C" int gm_ctx_destroy(gm_ctx* c) {
@@ -463,8 +459,7 @@ extern "C" long long gm_launch_count(gm_ctx* c, int reset) {
 
 extern "C" int gm_prof_enable(gm_ctx* c, int on) {
   if (!c) return GM_ERR_ARG;
-  c->prof = on == 1;
-  g_prof_all = on == 2;
+  c->prof = on == 1 || on == 2 ? on : 0;
   return GM_OK;
 }
 // level-2 profile (gm_prof_enable(ctx, 2)): synchronises, then writes "name,launches,total_ms\n" lines (one per kernel
@@ -474,15 +469,17 @@ extern "C" int gm_prof_report(gm_ctx* c, char* buf, int buflen) {
   CU_OK(c, cudaDeviceSynchronize());
   std::map<std::string, std::pair<long long, double>> agg;
   std::vector<std::string> order;
-  for (auto& r : g_prof_all_recs) {
-    float t = 0.f;
-    cudaEventElapsedTime(&t, r.e0, r.e1);
-    auto it = agg.find(r.name);
-    if (it == agg.end()) { order.push_back(r.name); it = agg.emplace(r.name, std::make_pair(0ll, 0.0)).first; }
-    it->second.first++; it->second.second += t;
+  for (auto& r : c->prof_recs) {
+    if (r.name) {   // recorded at level 2
+      float t = 0.f;
+      cudaEventElapsedTime(&t, r.e0, r.e1);
+      auto it = agg.find(r.name);
+      if (it == agg.end()) { order.push_back(r.name); it = agg.emplace(r.name, std::make_pair(0ll, 0.0)).first; }
+      it->second.first++; it->second.second += t;
+    }
     cudaEventDestroy(r.e0); cudaEventDestroy(r.e1);
   }
-  g_prof_all_recs.clear();
+  c->prof_recs.clear();
   std::string out;
   for (auto& n : order) {
     char line[256];
@@ -500,9 +497,11 @@ extern "C" int gm_prof_collect(gm_ctx* c, double* ms, double* flops, long long* 
   for (int i = 0; i < 4; ++i) { ms[i] = 0; flops[i] = 0; count[i] = 0; }
   CU_OK(c, cudaDeviceSynchronize());
   for (auto& r : c->prof_recs) {
-    float t = 0.f;
-    cudaEventElapsedTime(&t, r.e0, r.e1);
-    ms[r.kind] += t; flops[r.kind] += r.flops; count[r.kind]++;
+    if (r.kind >= 0) {
+      float t = 0.f;
+      cudaEventElapsedTime(&t, r.e0, r.e1);
+      ms[r.kind] += t; flops[r.kind] += r.flops; count[r.kind]++;
+    }
     cudaEventDestroy(r.e0);
     cudaEventDestroy(r.e1);
   }
@@ -588,11 +587,8 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
   if (rc) return rc;
   const long long rows = d->transpose ? d->N : d->M;
   const int cols = d->transpose ? d->M : d->N;
-  launch_pdl("reduce_partials_kernel", reduce_partials_kernel, unsigned((rows * cols + 255) / 256), 256, 0, s, c->scratch, p.splits, per,
+  return launch(c, "reduce_partials_kernel", reduce_partials_kernel, unsigned((rows * cols + 255) / 256), 256, 0, s, c->scratch, p.splits, per,
              rows, cols, d->ldc, static_cast<float*>(d->C_dev));
-  c->launches++;
-  CU_OK(c, cudaGetLastError());
-  return GM_OK;
 }
 
 static void fill_adam(AdamParams& a, const gm_adam_hp* hp, int step) {
@@ -610,10 +606,7 @@ extern "C" int gm_adam_step_lr(gm_ctx* c, float* p, const float* g, float* m, fl
   a.p = p; a.g = g; a.m = m; a.v = v; a.total = n; a.nseg = 0;
   fill_adam(a, hp, step);
   a.lr_scale = lr_scale_dev;
-  launch_pdl("adam_kernel", adam_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
-  c->launches++;
-  CU_OK(c, cudaGetLastError());
-  return GM_OK;
+  return launch(c, "adam_kernel", adam_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
 }
 
 extern "C" int gm_adam_step(gm_ctx* c, float* p, const float* g, float* m, float* v, int n, const gm_adam_hp* hp,
@@ -746,19 +739,22 @@ struct gm_gan {
   long long lo = 0;          // arena.lo_off: > 0 in split-operand mode
 };
 
-static int dev_alloc(gm_gan* g, __nv_bfloat16** p, size_t count) {   // bf16 buffers come from the arena (finalised at the end of create)
+// Zeroed device buffers of an engine (gm_gan, gm_vae), freed by its destroy.  bf16 buffers come from the engine's arena
+// (finalised at the end of create) unless T is given explicitly, as for the VAE's per-call slot buffers.
+template <typename E>
+static int dev_alloc(E* g, __nv_bfloat16** p, size_t count) {
   g->arena.request(p, count);
   return GM_OK;
 }
 
-template <typename T>
-static int dev_alloc(gm_gan* g, T** p, size_t count) {
+template <typename T, typename E>
+static int dev_alloc(E* g, T** p, size_t count) {
   void* q = nullptr;
   cudaError_t e = cudaMalloc(&q, count * sizeof(T));
   if (e != cudaSuccess) return fail(g->ctx, GM_ERR_CUDA, "cudaMalloc(%zu) failed: %s", count * sizeof(T), cudaGetErrorString(e));
+  g->allocs.push_back(q);
   e = cudaMemset(q, 0, count * sizeof(T));
   if (e != cudaSuccess) return fail(g->ctx, GM_ERR_CUDA, "cudaMemset failed: %s", cudaGetErrorString(e));
-  g->allocs.push_back(q);
   *p = static_cast<T*>(q);
   return GM_OK;
 }
@@ -921,17 +917,13 @@ extern "C" int gm_gan_sync_shadows(gm_gan* g, int net, gm_stream stream) {
   a.p = g->par[net];
   a.update = 0;
   adam_segs(g, net, a);
-  launch_pdl("adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
 }
 
-static void flush_pending(gm_gan* g, cudaStream_t s);
-static void bump_step(gm_gan* g, int which, cudaStream_t s) {
-  if (!g->dev_step) return;
-  launch_pdl("bump_step_kernel", bump_step_kernel, 1, 32, 0, s, g->dstep + which);
-  g->ctx->launches++;
+static int flush_pending(gm_gan* g, cudaStream_t s);
+static int bump_step(gm_gan* g, int which, cudaStream_t s) {
+  if (!g->dev_step) return GM_OK;
+  return launch(g->ctx, "bump_step_kernel", bump_step_kernel, 1, 32, 0, s, g->dstep + which);
 }
 
 
@@ -948,24 +940,20 @@ extern "C" int gm_gan_apply(gm_gan* g, int net, const gm_adam_hp* hp, int step, 
     g->pend[net] = false;
   }
   if (g->dev_step) a.step_ptr = g->dstep + net;   // bias corrections from the device counter (`step` is ignored)
-  launch_pdl("adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
-  g->ctx->launches++;
-  bump_step(g, net, static_cast<cudaStream_t>(stream));
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  const int rc = launch(g->ctx, "adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
+  return rc ? rc : bump_step(g, net, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int gm_gan_set_lazy_grads(gm_gan* g, int on, gm_stream stream) {
   if (!g) return GM_ERR_ARG;
-  if (!on) flush_pending(g, static_cast<cudaStream_t>(stream));
+  int rc;
+  if (!on && (rc = flush_pending(g, static_cast<cudaStream_t>(stream)))) return rc;
   g->lazy = on != 0;
   return GM_OK;
 }
 extern "C" int gm_gan_materialize_grads(gm_gan* g, gm_stream stream) {
   if (!g) return GM_ERR_ARG;
-  flush_pending(g, static_cast<cudaStream_t>(stream));
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return flush_pending(g, static_cast<cudaStream_t>(stream));
 }
 
 // epilogue setters for a plan fresh from plan_gemm (every other field zero)
@@ -1120,18 +1108,16 @@ static int check_step_args(gm_gan* g, int batch) {
 
 static int run_generator(gm_gan* g, StepPlans* sp, int B, const float* noise, uint64_t seed, uint64_t stream_id, cudaStream_t s,
                          const unsigned long long* step_ptr = nullptr) {
-  launch_pdl("stage_noise_kernel", stage_noise_kernel, cdiv(B * ((g->Z + 8) / 8), 256), 256, 0, s, noise, g->Zb, B, g->Z, g->ZP, seed, stream_id, g->lo, step_ptr);
-  g->ctx->launches++;
   int rc;
+  if ((rc = launch(g->ctx, "stage_noise_kernel", stage_noise_kernel, cdiv(B * ((g->Z + 8) / 8), 256), 256, 0, s, noise, g->Zb, B, g->Z, g->ZP, seed, stream_id, g->lo, step_ptr))) return rc;
   if ((rc = launch_plan(g->ctx, sp->g1, s))) return rc;
-  if ((rc = launch_plan(g->ctx, sp->g2, s))) return rc;
-  return GM_OK;
+  return launch_plan(g->ctx, sp->g2, s);
 }
 
 // replace per-block partial sums by their sum over all ranks (no-op without an attached communicator)
-static void exchange_stats(gm_gan* g, double* part, int nblk, int stride, int nvals, cudaStream_t s) {
+static int exchange_stats(gm_gan* g, double* part, int nblk, int stride, int nvals, cudaStream_t s) {
   gm_comm* m = g->comm;
-  if (!m || m->world <= 1) return;
+  if (!m || m->world <= 1) return GM_OK;
   CommStats cs;
   memset(&cs, 0, sizeof cs);
   for (int r = 0; r < m->world; ++r) {
@@ -1139,12 +1125,11 @@ static void exchange_stats(gm_gan* g, double* part, int nblk, int stride, int nv
     cs.f[r] = reinterpret_cast<unsigned long long*>(static_cast<char*>(m->peer[r]) + m->sflag_off);
   }
   cs.rank = m->rank; cs.world = m->world; cs.seq = ++m->seq_stats;
-  launch_pdl("stats_exchange_kernel", stats_exchange_kernel, 1, 256, 0, s, part, nblk, stride, nvals, cs);
-  g->ctx->launches++;
+  return launch(g->ctx, "stats_exchange_kernel", stats_exchange_kernel, 1, 256, 0, s, part, nblk, stride, nvals, cs);
 }
 static int stat_world(const gm_gan* g) { return (g->comm && g->comm->world > 1) ? g->comm->world : 1; }
 
-static void launch_loss(gm_gan* g, int B, int g_step, float inv_b, cudaStream_t s) {
+static int launch_loss(gm_gan* g, int B, int g_step, float inv_b, cudaStream_t s) {
   LossParams lp;
   lp.slots = g->slots + (g_step ? B : 0);
   lp.nslots = 2 * cdiv(g->H, 208);
@@ -1164,36 +1149,36 @@ static void launch_loss(gm_gan* g, int B, int g_step, float inv_b, cudaStream_t 
   lp.partB = g->loss_part + size_t(g->loss_blocks) * 4;
   lp.partR = g->loss_part + size_t(g->loss_blocks) * 8;
   const int v = g->d.variant;
+  int rc;
   if (!g_step && (v == V_RA || v == V_FISHER)) {
-    launch_pdl("loss_pass_kernel<0>", loss_pass_kernel<0>, lp.nblk, kLossThreads, 0, s, lp);
-    g->ctx->launches++;
-    exchange_stats(g, lp.partA, lp.nblk, 4, 4, s);       // sum d, d^2 per branch over all ranks
+    if ((rc = launch(g->ctx, "loss_pass_kernel<0>", loss_pass_kernel<0>, lp.nblk, kLossThreads, 0, s, lp))) return rc;
+    if ((rc = exchange_stats(g, lp.partA, lp.nblk, 4, 4, s))) return rc;       // sum d, d^2 per branch over all ranks
     if (v == V_RA) {
-      launch_pdl("loss_pass_kernel<1>", loss_pass_kernel<1>, lp.nblk, kLossThreads, 0, s, lp);
-      g->ctx->launches++;
-      exchange_stats(g, lp.partB, lp.nblk, 4, 1, s);     // sum q(1-q)/(q+eps) over all ranks' real rows
+      if ((rc = launch(g->ctx, "loss_pass_kernel<1>", loss_pass_kernel<1>, lp.nblk, kLossThreads, 0, s, lp))) return rc;
+      if ((rc = exchange_stats(g, lp.partB, lp.nblk, 4, 1, s))) return rc;     // sum q(1-q)/(q+eps) over all ranks' real rows
     }
   }
-  launch_pdl("loss_pass_kernel<2>", loss_pass_kernel<2>, lp.nblk, kLossThreads, 0, s, lp);   // its last block writes loss[0..1]
-  g->ctx->launches += 1;
+  return launch(g->ctx, "loss_pass_kernel<2>", loss_pass_kernel<2>, lp.nblk, kLossThreads, 0, s, lp);   // its last block writes loss[0..1]
 }
 
 // The flat gradient of `net` from its partials: now (finalize kernel), or - with lazy gradients -
 // inside the next gm_gan_apply(net).
-static void emit_grads(gm_gan* g, int net, const GradSegs& gs, cudaStream_t s, bool force_now = false) {
+static int emit_grads(gm_gan* g, int net, const GradSegs& gs, cudaStream_t s, bool force_now = false) {
   if (g->lazy && !force_now) {
     g->pend_segs[net] = gs;
     g->pend[net] = true;
-    return;
+    return GM_OK;
   }
-  launch_pdl("finalize_grads_kernel", finalize_grads_kernel, cdiv(gs.total, 256), 256, 0, s, gs, g->grd[net]);
-  g->ctx->launches++;
-  g->pend[net] = false;
+  const int rc = launch(g->ctx, "finalize_grads_kernel", finalize_grads_kernel, cdiv(gs.total, 256), 256, 0, s, gs, g->grd[net]);
+  if (!rc) g->pend[net] = false;
+  return rc;
 }
 // Partials are only valid until the next *_grad call reuses the buffers: form pending gradients first.
-static void flush_pending(gm_gan* g, cudaStream_t s) {
+static int flush_pending(gm_gan* g, cudaStream_t s) {
+  int rc;
   for (int net = 0; net < 2; ++net)
-    if (g->pend[net]) emit_grads(g, net, g->pend_segs[net], s, true);
+    if (g->pend[net] && (rc = emit_grads(g, net, g->pend_segs[net], s, true))) return rc;
+  return GM_OK;
 }
 
 // ---- BEGAN (src/be_gan.py:212-258): D = autoencoder, L1 reconstruction losses ----
@@ -1208,8 +1193,7 @@ static int began_finalize_g(gm_gan* g, StepPlans* sp, cudaStream_t s, bool force
   gs.s[1] = {g->G.off_b1, g->H, 2, 0, p1.ldp, g->Z, p1.splits, p1.part_stride, g->PG1};
   gs.s[2] = {g->G.off_w2, g->X * g->H, 0, g->H, p2.ldp, 0, p2.splits, p2.part_stride, g->PG2};
   gs.s[3] = {g->G.off_b2, g->X, 2, 0, p2.ldp, g->H, p2.splits, p2.part_stride, g->PG2};
-  emit_grads(g, GM_NET_G, gs, s, force_now);
-  return GM_OK;
+  return emit_grads(g, GM_NET_G, gs, s, force_now);
 }
 
 static int began_d_grad(gm_gan* g, StepPlans* sp, int B, float* loss_dev, cudaStream_t s) {
@@ -1219,12 +1203,11 @@ static int began_d_grad(gm_gan* g, StepPlans* sp, int B, float* loss_dev, cudaSt
   if ((rc = launch_plan(c, sp->be_dec_d, s))) return rc;   // DR = scaled sign(D(.) - .), row L1 sums -> slots_r
   const int nb = c->num_sms;
   const int ns = 2 * cdiv(g->X, 208);
-  launch_pdl("vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r, ns, 2 * g->Bmax, B, g->be_part);
-  launch_pdl("vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r + B, ns, 2 * g->Bmax, B, g->be_part + nb);
-  exchange_stats(g, g->be_part, nb, 1, 1, s);          // DX, DG of the K controller over the global batch
-  exchange_stats(g, g->be_part + nb, nb, 1, 1, s);
-  launch_pdl("began_loss_final_kernel", began_loss_final_kernel, 1, 256, 0, s, g->be_part, g->be_part + nb, nb, B * stat_world(g), 0, g->be_state, g->lossbuf);
-  c->launches += 3;
+  if ((rc = launch(c, "vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r, ns, 2 * g->Bmax, B, g->be_part))) return rc;
+  if ((rc = launch(c, "vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r + B, ns, 2 * g->Bmax, B, g->be_part + nb))) return rc;
+  if ((rc = exchange_stats(g, g->be_part, nb, 1, 1, s))) return rc;          // DX, DG of the K controller over the global batch
+  if ((rc = exchange_stats(g, g->be_part + nb, nb, 1, 1, s))) return rc;
+  if ((rc = launch(c, "began_loss_final_kernel", began_loss_final_kernel, 1, 256, 0, s, g->be_part, g->be_part + nb, nb, B * stat_world(g), 0, g->be_state, g->lossbuf))) return rc;
   if ((rc = launch_plan(c, sp->be_gwd, s))) return rc;
   if ((rc = launch_plan(c, sp->be_de_d, s))) return rc;
   if ((rc = launch_plan(c, sp->dw1d, s))) return rc;
@@ -1238,9 +1221,8 @@ static int began_d_grad(gm_gan* g, StepPlans* sp, int B, float* loss_dev, cudaSt
   gs.s[1] = {g->D.off_b1, g->H, 2, 0, pe.ldp, g->X, pe.splits, pe.part_stride, g->PD};
   gs.s[2] = {g->D.off_w2, g->X * g->H, 0, g->H, pd.ldp, 0, pd.splits, pd.part_stride, g->PWd};
   gs.s[3] = {g->D.off_b2, g->X, 2, 0, pd.ldp, g->H, pd.splits, pd.part_stride, g->PWd};
-  emit_grads(g, GM_NET_D, gs, s);
+  if ((rc = emit_grads(g, GM_NET_D, gs, s))) return rc;
   if (loss_dev) CU_OK(c, cudaMemcpyAsync(loss_dev, g->lossbuf, sizeof(float), cudaMemcpyDeviceToDevice, s));
-  CU_OK(c, cudaGetLastError());
   return GM_OK;
 }
 
@@ -1250,19 +1232,16 @@ static int began_g_grad(gm_gan* g, StepPlans* sp, int B, float* loss_dev, cudaSt
   if ((rc = launch_plan(c, sp->be_enc_g, s))) return rc;
   if ((rc = launch_plan(c, sp->be_dec_g, s))) return rc;
   const int nb = c->num_sms;
-  launch_pdl("vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r + B, 2 * cdiv(g->X, 208), 2 * g->Bmax, B, g->be_part + nb);
-  launch_pdl("began_loss_final_kernel", began_loss_final_kernel, 1, 256, 0, s, g->be_part, g->be_part + nb, nb, B, 1, g->be_state, g->lossbuf);
-  c->launches += 2;
+  if ((rc = launch(c, "vae_rowsum_kernel", vae_rowsum_kernel, nb, 256, 0, s, g->slots_r + B, 2 * cdiv(g->X, 208), 2 * g->Bmax, B, g->be_part + nb))) return rc;
+  if ((rc = launch(c, "began_loss_final_kernel", began_loss_final_kernel, 1, 256, 0, s, g->be_part, g->be_part + nb, nb, B, 1, g->be_state, g->lossbuf))) return rc;
   if ((rc = launch_plan(c, sp->be_de_g, s))) return rc;
   if ((rc = launch_plan(c, sp->be_dxg, s))) return rc;
-  launch_pdl("began_da2_kernel", began_da2_kernel, c->num_sms * 8, 256, 0, s, g->BT, g->DR + size_t(B) * g->XP, g->Xall + size_t(B) * g->XP, g->DA2, B, g->X, g->XP, g->lo);
-  c->launches++;
+  if ((rc = launch(c, "began_da2_kernel", began_da2_kernel, c->num_sms * 8, 256, 0, s, g->BT, g->DR + size_t(B) * g->XP, g->Xall + size_t(B) * g->XP, g->DA2, B, g->X, g->XP, g->lo))) return rc;
   if ((rc = launch_plan(c, sp->dw2g, s))) return rc;
   if ((rc = launch_plan(c, sp->dhg, s))) return rc;
   if ((rc = launch_plan(c, sp->dw1g, s))) return rc;
-  began_finalize_g(g, sp, s);
+  if ((rc = began_finalize_g(g, sp, s))) return rc;
   if (loss_dev) CU_OK(c, cudaMemcpyAsync(loss_dev, g->lossbuf, sizeof(float), cudaMemcpyDeviceToDevice, s));
-  CU_OK(c, cudaGetLastError());
   return GM_OK;
 }
 
@@ -1282,10 +1261,7 @@ extern "C" int gm_gan_began_state(gm_gan* g, float* host11, int set, gm_stream s
 extern "C" int gm_gan_began_control(gm_gan* g, float gamma, float lambda, float patience, gm_stream stream) {
   if (!g) return GM_ERR_ARG;
   if (g->d.variant != GM_BEGAN) return fail(g->ctx, GM_ERR_STATE, "not a BEGAN engine");
-  launch_pdl("began_control_kernel", began_control_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), g->be_state, gamma, lambda, patience);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "began_control_kernel", began_control_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), g->be_state, gamma, lambda, patience);
 }
 
 // real rows -> Xall[0:B] (bf16, ones column); with a sampler pool and no gather_idx the kernel draws the batch rows itself
@@ -1296,9 +1272,7 @@ static int stage_real_rows(gm_gan* g, const void* images, int img_fmt, const int
     if (B > g->pool_n) return fail(c, GM_ERR_ARG, "batch (%d) exceeds the sampler's pool (%lld)", B, g->pool_n);
     smp = make_sampler(g->pool_n, g->pool_seed, step, 0, g->dev_step ? g->dstep + 3 : nullptr);     // a fresh permutation every step (src/ns_gan.py:224)
   }
-  launch_pdl("stage_images_kernel", stage_images_kernel, c->num_sms * 8, 256, 0, s, images, img_fmt, gather_idx, g->Xall, B, g->X, g->XP, smp, g->lo);
-  c->launches++;
-  return GM_OK;
+  return launch(c, "stage_images_kernel", stage_images_kernel, c->num_sms * 8, 256, 0, s, images, img_fmt, gather_idx, g->Xall, B, g->X, g->XP, smp, g->lo);
 }
 
 // process_batch of the NEXT train_D (src/ns_gan.py:222-226) ahead of time: stages the real rows now; the following gm_gan_d_grad
@@ -1311,7 +1285,6 @@ extern "C" int gm_gan_d_stage(gm_gan* g, const void* images, int img_fmt, const 
   if (g->dev_step) return fail(g->ctx, GM_ERR_STATE, "gm_gan_d_stage is not available in device-step mode");
   if ((rc = stage_real_rows(g, images, img_fmt, gather_idx, batch, step, static_cast<cudaStream_t>(stream)))) return rc;
   g->staged_batch = batch;
-  CU_OK(g->ctx, cudaGetLastError());
   return GM_OK;
 }
 
@@ -1326,7 +1299,7 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   if ((rc = build_plans(g, batch, &sp))) return rc;
   const int B = batch;
   gm_ctx* c = g->ctx;
-  flush_pending(g, s);
+  if ((rc = flush_pending(g, s))) return rc;
   // real rows -> Xall[0:B] (bf16, ones column)
   if (g->staged_batch == B) {
     g->staged_batch = 0;       // the real rows are already in place (gm_gan_d_stage)
@@ -1335,7 +1308,7 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   }
   const unsigned long long* dptr = g->dev_step ? g->dstep + 3 : nullptr;   // device-step mode: the train_D call counter
   if ((rc = run_generator(g, sp, B, noise, seed, g->dev_step ? 0 : 2 * step, s, dptr))) return rc;
-  if (g->d.variant == GM_BEGAN) { rc = began_d_grad(g, sp, B, loss_dev, s); bump_step(g, 3, s); return rc; }
+  if (g->d.variant == GM_BEGAN) return (rc = began_d_grad(g, sp, B, loss_dev, s)) ? rc : bump_step(g, 3, s);
   const bool gp = g->nreg > 2;
   const int H = g->H, HP = g->HP, X = g->X, XP = g->XP;
   const float* w2 = g->par[GM_NET_D] + g->D.off_w2;
@@ -1343,31 +1316,29 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   const bool dra = g->d.variant == GM_DRA;
   if (dra) {
     // interpolated rows (region 2) around the real data
-    launch_pdl("moments_kernel", moments_kernel, c->num_sms * 2, 256, 0, s, g->Xall, B, X, XP, g->mom_part);
-    exchange_stats(g, g->mom_part, c->num_sms * 2, 2, 2, s);     // images.std() over the global batch
-    launch_pdl("moments_final_kernel", moments_final_kernel, 1, 256, 0, s, g->mom_part, c->num_sms * 2, float(double(B) * X * stat_world(g)), g->stats);
-    launch_pdl("xhat_kernel", xhat_kernel, c->num_sms * 8, 256, 0, s, g->Xall, g->Xall + size_t(2) * B * XP, B, X, XP,
-                                           aux, g->stats, seed, g->dev_step ? 0 : 2 * step, g->lc.dra_c, g->lo, dptr);
-    c->launches += 3;
+    if ((rc = launch(c, "moments_kernel", moments_kernel, c->num_sms * 2, 256, 0, s, g->Xall, B, X, XP, g->mom_part))) return rc;
+    if ((rc = exchange_stats(g, g->mom_part, c->num_sms * 2, 2, 2, s))) return rc;     // images.std() over the global batch
+    if ((rc = launch(c, "moments_final_kernel", moments_final_kernel, 1, 256, 0, s, g->mom_part, c->num_sms * 2, float(double(B) * X * stat_world(g)), g->stats))) return rc;
+    // xhat_kernel takes no programmatic serialisation: launched early behind the generator's output GEMM its CTAs would
+    // pile up on the first SMs that GEMM frees instead of spreading over the whole chip
+    if ((rc = launch(c, {"xhat_kernel", false}, xhat_kernel, c->num_sms * 8, 256, 0, s, g->Xall, g->Xall + size_t(2) * B * XP, B, X, XP,
+                     aux, g->stats, seed, g->dev_step ? 0 : 2 * step, g->lc.dra_c, g->lo, dptr))) return rc;
   }
   if ((rc = launch_plan(c, sp->d1_d, s))) return rc;
   if (g->d.variant == GM_WGP) {
     // U = w2 * relu'(a_hat) and the logit part of s(x_hat) from the pre-activations of the real / fake rows
-    launch_pdl("gp_hat_kernel", gp_hat_kernel, c->num_sms * 8, 256, 0, s, g->Aall, g->Aall + size_t(B) * HP, w2, g->DHall + size_t(2) * B * HP,
-               g->slots + 2 * B, 2 * cdiv(H, 208), g->nreg * g->Bmax, B, H, HP, aux, seed, g->dev_step ? 0 : 2 * step, g->lo, dptr);
-    c->launches++;
+    if ((rc = launch(c, "gp_hat_kernel", gp_hat_kernel, c->num_sms * 8, 256, 0, s, g->Aall, g->Aall + size_t(B) * HP, w2, g->DHall + size_t(2) * B * HP,
+               g->slots + 2 * B, 2 * cdiv(H, 208), g->nreg * g->Bmax, B, H, HP, aux, seed, g->dev_step ? 0 : 2 * step, g->lo, dptr))) return rc;
   }
-  launch_loss(g, B, 0, inv_global_batch, s);
-  launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall, g->ds, w2, g->DHall, g->dw2p, 2 * B, H, HP, g->dh_rows_per_iter, g->lo,
-             g->d.variant == GM_WGP ? 1 : 0);
-  launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p, g->dh_blocks, HP, HP, g->dw2sum);
-  c->launches += 2;
+  if ((rc = launch_loss(g, B, 0, inv_global_batch, s))) return rc;
+  if ((rc = launch(c, "dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall, g->ds, w2, g->DHall, g->dw2p, 2 * B, H, HP, g->dh_rows_per_iter, g->lo,
+             g->d.variant == GM_WGP ? 1 : 0))) return rc;
+  if ((rc = launch(c, "colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p, g->dh_blocks, HP, HP, g->dw2sum))) return rc;
   if (gp) {
     const size_t rreg = size_t(g->nreg - 1) * B;
     if (dra) {   // DRAGAN keeps a_hat (its penalty back-propagates through s(x_hat) too): U = 1[a_hat > 0] * w2 by a pass
-      launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, nullptr, w2, g->DHall + rreg * HP, nullptr,
-                                                            B, H, HP, g->dh_rows_per_iter, g->lo, 0);
-      c->launches++;
+      if ((rc = launch(c, "dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, nullptr, w2, g->DHall + rreg * HP, nullptr,
+                                                            B, H, HP, g->dh_rows_per_iter, g->lo, 0))) return rc;
     }
     if ((rc = launch_plan(c, sp->gp_v, s))) return rc;          // V = U W1 -> R region of Xall, ||V||^2 -> slots_v
     {
@@ -1386,20 +1357,17 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
     gpp.coef = g->coef; gpp.ds_gp = g->ds + 2 * B;
     gpp.part = g->gp_part; gpp.nblk = cdiv(B, kLossThreads) < c->num_sms * 2 ? cdiv(B, kLossThreads) : c->num_sms * 2;
     gpp.loss = g->lossbuf;
-    launch_pdl("gp_rows_kernel", gp_rows_kernel, gpp.nblk, kLossThreads, 0, s, gpp);
-    launch_pdl("gp_final_kernel", gp_final_kernel, 1, kLossThreads, 0, s, gpp);
-    launch_pdl("scale_rows_kernel", scale_rows_kernel, c->num_sms * 4, 256, 0, s, g->DHall + rreg * HP, g->coef, B, HP, g->lo);   // U <- coef * U
-    c->launches += 3;
+    if ((rc = launch(c, "gp_rows_kernel", gp_rows_kernel, gpp.nblk, kLossThreads, 0, s, gpp))) return rc;
+    if ((rc = launch(c, "gp_final_kernel", gp_final_kernel, 1, kLossThreads, 0, s, gpp))) return rc;
+    if ((rc = launch(c, "scale_rows_kernel", scale_rows_kernel, c->num_sms * 4, 256, 0, s, g->DHall + rreg * HP, g->coef, B, HP, g->lo))) return rc;   // U <- coef * U
     if ((rc = launch_plan(c, sp->gp_t, s))) return rc;          // T = coef (V W1^T) * mask -> DHg
     // dGP/dw2 = column sums of T (block partials; no output rows)
-    launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->DHg, nullptr, w2, static_cast<__nv_bfloat16*>(nullptr), g->dw2p2, B, H, HP, g->dh_rows_per_iter, g->lo, 0);
-    launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p2, g->dh_blocks, HP, HP, g->dw2sum + HP);
-    c->launches += 2;
+    if ((rc = launch(c, "dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->DHg, nullptr, w2, static_cast<__nv_bfloat16*>(nullptr), g->dw2p2, B, H, HP, g->dh_rows_per_iter, g->lo, 0))) return rc;
+    if ((rc = launch(c, "colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p2, g->dh_blocks, HP, HP, g->dw2sum + HP))) return rc;
     if (dra) {   // DRAGAN: the penalty also back-propagates through s(xhat)
-      launch_pdl("dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, g->ds + 2 * B, w2,
-                                                            g->DHall + size_t(2) * B * HP, g->dw2p3, B, H, HP, g->dh_rows_per_iter, g->lo, 0);
-      launch_pdl("colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p3, g->dh_blocks, HP, HP, g->dw2sum + 2 * HP);
-      c->launches += 2;
+      if ((rc = launch(c, "dh_kernel", dh_kernel, g->dh_blocks, g->dh_threads, dh_smem, s, g->Aall + size_t(2) * B * HP, g->ds + 2 * B, w2,
+                                                            g->DHall + size_t(2) * B * HP, g->dw2p3, B, H, HP, g->dh_rows_per_iter, g->lo, 0))) return rc;
+      if ((rc = launch(c, "colsum_kernel", colsum_kernel, cdiv(HP * 32, 256), 256, 0, s, g->dw2p3, g->dh_blocks, HP, HP, g->dw2sum + 2 * HP))) return rc;
     }
   }
   if ((rc = launch_plan(c, sp->dw1d, s))) return rc;
@@ -1412,12 +1380,10 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
   gs.s[1] = {g->D.off_b1, g->H, 2, 0, pw.ldp, g->X, pw.splits, pw.part_stride, g->PD};
   gs.s[2] = {g->D.off_w2, g->H, 3, 0, 0, 0, gp ? g->nreg - 1 : 1, (long long)HP, g->dw2sum};
   gs.s[3] = {g->D.off_b2, 1, 3, 0, 0, 0, gp ? 2 : 1, 2, g->lossbuf + 1};
-  emit_grads(g, GM_NET_D, gs, s);
+  if ((rc = emit_grads(g, GM_NET_D, gs, s))) return rc;
   if (loss_dev) CU_OK(c, cudaMemcpyAsync(loss_dev, g->lossbuf, sizeof(float), cudaMemcpyDeviceToDevice, s));
   g->last_rows = 2 * B;
-  bump_step(g, 3, s);
-  CU_OK(c, cudaGetLastError());
-  return GM_OK;
+  return bump_step(g, 3, s);
 }
 
 // train_G + backward; `staged`: the generator forward of this step was already enqueued by
@@ -1432,11 +1398,11 @@ static int g_grad_impl(gm_gan* g, int batch, const float* noise, float inv_globa
   if ((rc = build_plans(g, batch, &sp))) return rc;
   const int B = batch;
   gm_ctx* c = g->ctx;
-  flush_pending(g, s);
+  if ((rc = flush_pending(g, s))) return rc;
   if (!staged && (rc = run_generator(g, sp, B, noise, seed, g->dev_step ? 1 : 2 * step + 1, s, g->dev_step ? g->dstep + 2 : nullptr))) return rc;
-  if (g->d.variant == GM_BEGAN) { rc = began_g_grad(g, sp, B, loss_dev, s); bump_step(g, 2, s); return rc; }
+  if (g->d.variant == GM_BEGAN) return (rc = began_g_grad(g, sp, B, loss_dev, s)) ? rc : bump_step(g, 2, s);
   if ((rc = launch_plan(c, sp->d1_g, s))) return rc;
-  launch_loss(g, B, 1, inv_global_batch, s);
+  if ((rc = launch_loss(g, B, 1, inv_global_batch, s))) return rc;
   if ((rc = launch_plan(c, sp->dx, s))) return rc;
   if ((rc = launch_plan(c, sp->dw2g, s))) return rc;
   if ((rc = launch_plan(c, sp->dhg, s))) return rc;
@@ -1451,12 +1417,10 @@ static int g_grad_impl(gm_gan* g, int batch, const float* noise, float inv_globa
   gs.s[1] = {g->G.off_b1, g->H, 2, 0, p1.ldp, g->Z, p1.splits, p1.part_stride, g->PG1};
   gs.s[2] = {g->G.off_w2, g->X * g->H, 0, g->H, p2.ldp, 0, p2.splits, p2.part_stride, g->PG2};
   gs.s[3] = {g->G.off_b2, g->X, 2, 0, p2.ldp, g->H, p2.splits, p2.part_stride, g->PG2};
-  emit_grads(g, GM_NET_G, gs, s);
+  if ((rc = emit_grads(g, GM_NET_G, gs, s))) return rc;
   if (loss_dev) CU_OK(c, cudaMemcpyAsync(loss_dev, g->lossbuf, sizeof(float), cudaMemcpyDeviceToDevice, s));
   g->last_rows = B;
-  bump_step(g, 2, s);
-  CU_OK(c, cudaGetLastError());
-  return GM_OK;
+  return bump_step(g, 2, s);
 }
 
 extern "C" int gm_gan_g_grad(gm_gan* g, int batch, const float* noise, float inv_global_batch, uint64_t seed,
@@ -1469,7 +1433,6 @@ extern "C" int gm_gan_g_forward_stage(gm_gan* g, int batch, const float* noise, 
   StepPlans* sp;
   if ((rc = build_plans(g, batch, &sp))) return rc;
   if ((rc = run_generator(g, sp, batch, noise, seed, 2 * step + 1, static_cast<cudaStream_t>(stream)))) return rc;
-  CU_OK(g->ctx, cudaGetLastError());
   return GM_OK;
 }
 extern "C" int gm_gan_g_grad_staged(gm_gan* g, int batch, float inv_global_batch, float* loss_dev, gm_stream stream) {
@@ -1499,10 +1462,7 @@ extern "C" int gm_gan_sync_shadows_q(gm_gan* g, gm_stream stream) {
   memset(&a, 0, sizeof a);
   a.p = g->parQ; a.update = 0;
   q_adam_segs(g, a);
-  launch_pdl("adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, static_cast<cudaStream_t>(stream), a);
 }
 
 // train_Q + MI_loss.backward(): writes the flat G gradient (G's grad buffer), the flat Q
@@ -1516,7 +1476,7 @@ extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, f
   if (!noise) return fail(g->ctx, GM_ERR_ARG, "the Q step needs the structured noise tensor");
   if (zd + g->q_out != g->Z) return fail(g->ctx, GM_ERR_ARG, "z_dim (%d) + codes (%d) != generator input (%d)", zd, g->q_out, g->Z);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  flush_pending(g, s);
+  if ((rc = flush_pending(g, s))) return rc;
   StepPlans* sp;
   if ((rc = build_plans(g, batch, &sp))) return rc;
   const int B = batch;
@@ -1525,9 +1485,8 @@ extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, f
   if ((rc = launch_plan(c, sp->q1, s))) return rc;
   if ((rc = launch_plan(c, sp->q2, s))) return rc;
   const int nb = cdiv(B, kLossThreads) < c->num_sms * 2 ? cdiv(B, kLossThreads) : c->num_sms * 2;
-  launch_pdl("info_loss_kernel", info_loss_kernel, nb, kLossThreads, 0, s, g->INF, 32, noise, g->Z, zd, 10, 10, B, inv_global_batch, g->DINF, 64, g->q_part, g->lo);
-  launch_pdl("info_loss_final_kernel", info_loss_final_kernel, 1, kLossThreads, 0, s, g->q_part, nb, B, 10, g->lossbuf);
-  c->launches += 2;
+  if ((rc = launch(c, "info_loss_kernel", info_loss_kernel, nb, kLossThreads, 0, s, g->INF, 32, noise, g->Z, zd, 10, 10, B, inv_global_batch, g->DINF, 64, g->q_part, g->lo))) return rc;
+  if ((rc = launch(c, "info_loss_final_kernel", info_loss_final_kernel, 1, kLossThreads, 0, s, g->q_part, nb, B, 10, g->lossbuf))) return rc;
   if ((rc = launch_plan(c, sp->gq2, s))) return rc;
   if ((rc = launch_plan(c, sp->dhq, s))) return rc;
   if ((rc = launch_plan(c, sp->gq1, s))) return rc;
@@ -1545,7 +1504,7 @@ extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, f
   gs.s[1] = {g->G.off_b1, g->H, 2, 0, p1.ldp, g->Z, p1.splits, p1.part_stride, g->PG1};
   gs.s[2] = {g->G.off_w2, g->X * g->H, 0, g->H, p2.ldp, 0, p2.splits, p2.part_stride, g->PG2};
   gs.s[3] = {g->G.off_b2, g->X, 2, 0, p2.ldp, g->H, p2.splits, p2.part_stride, g->PG2};
-  emit_grads(g, GM_NET_G, gs, s, true);   // consumed by gm_gan_apply_mi, which reads the flat buffer
+  if ((rc = emit_grads(g, GM_NET_G, gs, s, true))) return rc;   // consumed by gm_gan_apply_mi, which reads the flat buffer
   GradSegs qs;
   memset(&qs, 0, sizeof qs);
   const GemmParams& q1 = sp->gq1.p;
@@ -1556,10 +1515,8 @@ extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, f
   qs.s[1] = {g->Qn.off_b1, g->H, 2, 0, q1.ldp, g->X, q1.splits, q1.part_stride, g->PQ1};
   qs.s[2] = {g->Qn.off_w2, g->q_out * g->H, 0, g->H, q2.ldp, 0, q2.splits, q2.part_stride, g->PQ2};
   qs.s[3] = {g->Qn.off_b2, g->q_out, 2, 0, q2.ldp, g->H, q2.splits, q2.part_stride, g->PQ2};
-  launch_pdl("finalize_grads_kernel", finalize_grads_kernel, cdiv(qs.total, 256), 256, 0, s, qs, g->grdQ);
-  c->launches += 2;
+  if ((rc = launch(c, "finalize_grads_kernel", finalize_grads_kernel, cdiv(qs.total, 256), 256, 0, s, qs, g->grdQ))) return rc;
   if (loss_dev) CU_OK(c, cudaMemcpyAsync(loss_dev, g->lossbuf, sizeof(float), cudaMemcpyDeviceToDevice, s));
-  CU_OK(c, cudaGetLastError());
   return GM_OK;
 }
 
@@ -1569,22 +1526,20 @@ extern "C" int gm_gan_apply_mi(gm_gan* g, const gm_adam_hp* hp, int step, gm_str
   if (!g || !hp || step <= 0) return g ? fail(g->ctx, GM_ERR_ARG, "gm_gan_apply_mi: bad argument") : GM_ERR_ARG;
   if (!g->parQ || !g->amQ || !g->avQ || !g->amG2 || !g->avG2) return fail(g->ctx, GM_ERR_STATE, "Q / MI optimizer state not bound");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  flush_pending(g, s);
+  int rc;
+  if ((rc = flush_pending(g, s))) return rc;
   AdamParams a;
   memset(&a, 0, sizeof a);
   a.p = g->par[GM_NET_G]; a.g = g->grd[GM_NET_G]; a.m = g->amG2; a.v = g->avG2;
   fill_adam(a, hp, step);
   adam_segs(g, GM_NET_G, a);
-  launch_pdl("adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, s, a);
+  if ((rc = launch(g->ctx, "adam_kernel", adam_kernel, cdiv(a.total, 256), 256, 0, s, a))) return rc;
   AdamParams q;
   memset(&q, 0, sizeof q);
   q.p = g->parQ; q.g = g->grdQ; q.m = g->amQ; q.v = g->avQ;
   fill_adam(q, hp, step);
   q_adam_segs(g, q);
-  launch_pdl("adam_kernel", adam_kernel, cdiv(q.total, 256), 256, 0, s, q);
-  g->ctx->launches += 2;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "adam_kernel", adam_kernel, cdiv(q.total, 256), 256, 0, s, q);
 }
 
 extern "C" int gm_gan_scores(gm_gan* g, float* dst, int n, gm_stream stream) {
@@ -1617,15 +1572,11 @@ extern "C" int gm_gan_generate(gm_gan* g, const float* noise, int n, float* imag
   int rc;
   if ((rc = build_plans(g, B, &sp))) return rc;
   // stage n noise rows (rows n..B-1 keep whatever they held; their outputs are not read)
-  launch_pdl("stage_noise_kernel", stage_noise_kernel, cdiv(n * ((g->Z + 8) / 8), 256), 256, 0, s, noise, g->Zb, n, g->Z, g->ZP, 0, 0, g->lo, static_cast<const unsigned long long*>(nullptr));
-  g->ctx->launches++;
+  if ((rc = launch(g->ctx, "stage_noise_kernel", stage_noise_kernel, cdiv(n * ((g->Z + 8) / 8), 256), 256, 0, s, noise, g->Zb, n, g->Z, g->ZP, 0, 0, g->lo, static_cast<const unsigned long long*>(nullptr)))) return rc;
   if ((rc = launch_plan(g->ctx, sp->g1, s))) return rc;
   if ((rc = launch_plan(g->ctx, sp->g2, s))) return rc;
   const long long tot = (long long)n * g->X;
-  launch_pdl("bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, s, g->Xall + size_t(B) * g->XP, g->XP, images, n, g->X, g->lo);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, s, g->Xall + size_t(B) * g->XP, g->XP, images, n, g->X, g->lo);
 }
 
 extern "C" int gm_gan_discriminate(gm_gan* g, const void* images, int img_fmt, int n, float* scores, gm_stream stream) {
@@ -1636,14 +1587,10 @@ extern "C" int gm_gan_discriminate(gm_gan* g, const void* images, int img_fmt, i
   StepPlans* sp;
   int rc;
   if ((rc = build_plans(g, n, &sp))) return rc;
-  launch_pdl("stage_images_kernel", stage_images_kernel, g->ctx->num_sms * 8, 256, 0, s, images, img_fmt, nullptr, g->Xall, n, g->X, g->XP, kNoSampler, g->lo);
-  g->ctx->launches++;
+  if ((rc = launch(g->ctx, "stage_images_kernel", stage_images_kernel, g->ctx->num_sms * 8, 256, 0, s, images, img_fmt, nullptr, g->Xall, n, g->X, g->XP, kNoSampler, g->lo))) return rc;
   if ((rc = launch_plan(g->ctx, sp->d1_x, s))) return rc;
-  launch_pdl("scores_kernel", scores_kernel, cdiv(n, 256), 256, 0, s, g->slots, 2 * cdiv(g->H, 208), g->nreg * g->Bmax, g->par[GM_NET_D] + g->D.off_b2,
+  return launch(g->ctx, "scores_kernel", scores_kernel, cdiv(n, 256), 256, 0, s, g->slots, 2 * cdiv(g->H, 208), g->nreg * g->Bmax, g->par[GM_NET_D] + g->D.off_b2,
                                             g->d.d_out_act, scores, n);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
 }
 
 // On-device batch sampling: with a pool set (and gather_idx == NULL) gm_gan_d_grad reads row
@@ -1683,7 +1630,7 @@ extern "C" int gm_gan_device_steps(gm_gan* g, unsigned long long* counters4_host
 // programmatic dependent launch on / off at run time (stream capture on drivers that reject programmatic edges)
 extern "C" int gm_ctx_set_pdl(gm_ctx* c, int on) {
   if (!c) return GM_ERR_ARG;
-  g_pdl = on != 0;
+  c->pdl = on != 0;
   return GM_OK;
 }
 
@@ -1710,10 +1657,7 @@ extern "C" int gm_gan_sample_indices(gm_gan* g, int batch, uint64_t step, int* i
   if (!g || !idx_dev || batch <= 0) return GM_ERR_ARG;
   if (g->pool_n > 0 && batch > g->pool_n) return fail(g->ctx, GM_ERR_ARG, "batch exceeds the pool");
   const Sampler smp = g->pool_n > 0 ? make_sampler(g->pool_n, g->pool_seed, step, 0) : kNoSampler;
-  launch_pdl("sample_indices_kernel", sample_indices_kernel, cdiv(batch, 256), 256, 0, static_cast<cudaStream_t>(stream), smp, batch, idx_dev);
-  g->ctx->launches++;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "sample_indices_kernel", sample_indices_kernel, cdiv(batch, 256), 256, 0, static_cast<cudaStream_t>(stream), smp, batch, idx_dev);
 }
 // the generator noise of a step as the train step draws it (net_step = 2*step for train_D, 2*step+1 for
 // train_G): Philox N(0,1) rounded to the bf16 operand the GEMM reads -> out_dev [batch, z] fp32
@@ -1722,13 +1666,10 @@ extern "C" int gm_gan_debug_noise(gm_gan* g, int batch, uint64_t seed, uint64_t 
   if (rc) return rc;
   if (!out_dev) return GM_ERR_ARG;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  launch_pdl("stage_noise_kernel", stage_noise_kernel, cdiv(batch * ((g->Z + 8) / 8), 256), 256, 0, s, static_cast<const float*>(nullptr), g->Zb, batch, g->Z, g->ZP,
-                                                   (unsigned long long)seed, (unsigned long long)(2 * step + (g_step ? 1 : 0)), g->lo, static_cast<const unsigned long long*>(nullptr));
+  if ((rc = launch(g->ctx, "stage_noise_kernel", stage_noise_kernel, cdiv(batch * ((g->Z + 8) / 8), 256), 256, 0, s, static_cast<const float*>(nullptr), g->Zb, batch, g->Z, g->ZP,
+                                                   (unsigned long long)seed, (unsigned long long)(2 * step + (g_step ? 1 : 0)), g->lo, static_cast<const unsigned long long*>(nullptr)))) return rc;
   const long long tot = (long long)batch * g->Z;
-  launch_pdl("bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, s, g->Zb, g->ZP, out_dev, batch, g->Z, g->lo);
-  g->ctx->launches += 2;
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
+  return launch(g->ctx, "bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, s, g->Zb, g->ZP, out_dev, batch, g->Z, g->lo);
 }
 
 // debug / test aid: an internal bf16 activation buffer as fp32 (hi + lo in split mode), out_dev [rows, cols];
@@ -1745,10 +1686,8 @@ extern "C" int gm_gan_debug_read(gm_gan* g, int which, int row0, int rows, int c
   if ((long long)row0 + rows > nrow[which])
     return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: rows [%d, %lld) run past the buffer's %lld rows", row0, (long long)row0 + rows, nrow[which]);
   const long long tot = (long long)rows * cols;
-  launch_pdl("bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream),
+  return launch(g->ctx, "bf16_rows_to_f32_kernel", bf16_rows_to_f32_kernel, unsigned((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream),
              src[which] + size_t(row0) * ld[which] + (plane == 2 ? g->lo : 0), ld[which], out_dev, rows, cols, plane == 0 ? g->lo : 0ll);
-  CU_OK(g->ctx, cudaGetLastError());
-  return GM_OK;
 }
 
 extern "C" int gm_gan_fisher_state(gm_gan* g, float* lambda_rho_host, int set, gm_stream stream) {

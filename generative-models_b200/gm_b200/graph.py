@@ -34,7 +34,7 @@ class GraphedGanStep:
                 self._one()
         except RuntimeError:
             # a driver that rejects programmatic-dependent-launch edges in a capture: plain edges instead
-            _lib.check(_lib.ctx(), _lib.lib().gm_ctx_set_pdl(_lib.ctx(), 0))
+            _lib.check(eng.h, _lib.lib().gm_ctx_set_pdl(eng.h, 0))
             self.pdl = False
             torch.cuda.synchronize()
             self.graph = torch.cuda.CUDAGraph()
@@ -57,7 +57,7 @@ class GraphedGanStep:
         torch.cuda.synchronize()
         self.eng.use_device_step(False)
         if not self.pdl:
-            _lib.check(_lib.ctx(), _lib.lib().gm_ctx_set_pdl(_lib.ctx(), 1))
+            _lib.check(self.eng.h, _lib.lib().gm_ctx_set_pdl(self.eng.h, 1))
 
 
 def graphed_gan_step(workload, steps):

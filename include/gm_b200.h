@@ -206,7 +206,8 @@ int gm_gan_attach_comm(gm_gan* gan, gm_comm* comm);
  * (NULL = zeros).  While on, the `step` arguments of those entry points are ignored. */
 int gm_gan_use_device_step(gm_gan* gan, int on, const unsigned long long* counters4_host, gm_stream stream);
 int gm_gan_device_steps(gm_gan* gan, unsigned long long* counters4_host, gm_stream stream);
-/* programmatic dependent launch on / off at run time (default on; GM_NO_PDL=1 starts with it off) */
+/* programmatic dependent launch on / off at run time for this context's launches (default on; GM_NO_PDL=1 creates the
+ * context with it off) */
 int gm_ctx_set_pdl(gm_ctx* ctx, int on);
 /* Loss constants the reference passes as train_D / train_G keyword arguments (defaults = the reference's):
  * gradient-penalty LAMBDA (src/w_gp_gan.py:177), DRAGAN's K and C (src/dra_gan.py:174), LSGAN's a, b, c
