@@ -104,7 +104,9 @@ enum PlanKind { PK_NT_208 = 0, PK_NT_64, PK_TN_256, PK_TN_64 };
 struct GemmPlan {
   CUtensorMap tmA, tmB;
   CUtensorMap tmA2, tmB2;   // residual (lo) planes of the operands in split mode, else copies of tmA / tmB
-  CUtensorMap tmBt, tmB2t;  // MN-major 208-wide plans: 16-column tail boxes of tmB / tmB2 (32-byte swizzle)
+  // MN-major 208-wide plans: 16-column tail boxes of tmB / tmB2 (32-byte swizzle).  K-major 208-wide plans: the boxes of
+  // the cluster ranks' shorter B shares (b_share_rows)
+  CUtensorMap tmBt, tmB2t;
   // output map of the K-major bf16 kernels (16-row x 32-column box, 64-byte swizzle), encoded at the first
   // launch because the epilogue (output pointer / leading dimension) is set after plan_gemm
   mutable CUtensorMap tmC;
@@ -229,8 +231,8 @@ static int launch_inst(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   }
   dim3 grid(pl.grid);
   if (CL > 1) {
-    // persistent: one cluster per item, up to the clusters the device holds at once (a GPC may hold an odd number of SMs).
-    // K-major clusters pair m-tiles, MN-major ones n-tiles (of an even count)
+    // persistent: one cluster per item, up to the clusters the device holds at once (a GPC need not hold a multiple of CL
+    // SMs).  K-major clusters group CL m-tiles, MN-major ones pair n-tiles (of an even count)
     const GemmParams& q = pl.p;
     const int items = (BMN ? q.m_tiles * (q.n_tiles / CL) : cdiv(q.m_tiles, CL) * q.n_tiles) * q.splits;
     grid = dim3(CL * (items < mc ? items : mc));
@@ -250,28 +252,27 @@ static int launch_tn(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   return launch_inst<208, true, true, kEpiUniversal, SPLIT, false, 2>(c, pl, s);
 }
 
-// split-operand plans (gm_prec GM_PREC_SPLIT): the universal epilogue with the residual-plane paths compiled in
+// split-operand plans (gm_prec GM_PREC_SPLIT): the universal epilogue with the residual-plane paths compiled in.  Their
+// K-major 208-wide kernel keeps 2-CTA clusters: it runs cooperatively, and as 4-CTA clusters (30 fit on an H100, 120 SMs)
+// it slowed the split-precision step by 5% (DESIGN §5)
+constexpr int kNtSplitCl = 2;
 template <int BN, bool AMN, bool BMN>
 static int launch_split(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
-  return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(c, pl, s);
+  if constexpr (BN == 208 && !AMN) return launch_inst<BN, AMN, BMN, kEpiUniversal, true, false, kNtSplitCl>(c, pl, s);
+  else return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(c, pl, s);
 }
 
-constexpr int kPingPongMaxKblocks = 7;   // K <= 448
-
 // K-major 128x208 kernel: the compile-time-specialised instance of the plan's epilogue signature when the train steps use
-// that signature, else the universal instance.
+// that signature, else the universal instance.  The specialised instances run their consumer warpgroups in ping-pong, so
+// each half-tile's epilogue hides under the other warpgroup's wgmma; the 4-CTA cluster's multicast keeps the B feed of
+// the half-tiles at that of the cooperative loop (DESIGN §3).
 static int launch_nt208(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   const GemmParams& p = pl.p;
   if (p.epi != EPI_BF16) return launch_inst<208, false, false>(c, pl, s);
-  // Short-K bias + activation GEMMs (G's two layers) are epilogue-bound: their consumer warpgroups run in ping-pong, so
-  // each half-tile's epilogue hides under the other warpgroup's wgmma.  Ping-pong loads the B tile once per 64-row half;
-  // from 8 k-blocks on, and with aux / row-dot epilogues, that extra feed cost more than it hid (DESIGN §5).
-  const bool pp = p.kblocks <= kPingPongMaxKblocks;
-#define NT208(S) case S: return launch_inst<208, false, false, S>(c, pl, s)
-#define NT208_PINGPONG(S) case S: return pp ? launch_inst<208, false, false, S, false, true>(c, pl, s) : launch_inst<208, false, false, S>(c, pl, s)
+#define NT208(S) case S: return launch_inst<208, false, false, S, false, true>(c, pl, s)
   switch (epi_sig(p)) {
-    NT208_PINGPONG(epi_sig(ACT_RELU, AUX_NONE, true, DOT_NONE));
-    NT208_PINGPONG(epi_sig(ACT_SIGMOID, AUX_NONE, true, DOT_NONE));
+    NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_NONE));
+    NT208(epi_sig(ACT_SIGMOID, AUX_NONE, true, DOT_NONE));
     NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W));
     NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W_MASK));
     NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_W_PRE));
@@ -285,7 +286,6 @@ static int launch_nt208(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
     default: return launch_inst<208, false, false>(c, pl, s);
   }
 #undef NT208
-#undef NT208_PINGPONG
 }
 
 [[nodiscard]] static int launch_plan(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
@@ -325,16 +325,19 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
                      int ldb, int ncover, int max_splits) {
   memset(pl, 0, sizeof *pl);
   if (M <= 0 || N <= 0 || K <= 0) return fail(c, GM_ERR_ARG, "gemm: bad extents %d %d %d", M, N, K);
-  int bn, boxn = 0, boxm = BM;
+  const int ntcl = c->plan_lo > 0 ? kNtSplitCl : kGemmCluster<208, false, false>;   // the launch_split / launch_nt208 instance
+  int bn, boxn = 0, boxm = BM, boxn_t = 0;
   if (mode == 0) {
     if (ncover <= 64) { pl->kind = PK_NT_64; bn = 64; boxn = 64; }
-    else {   // each CTA's share of the B tile; 64-row A boxes
-      pl->kind = PK_NT_208; bn = 208; boxn = 208 / kGemmCluster<208, false, false>; boxm = kGemmABoxRows<208, false>;
+    else {   // the cluster ranks' taller and shorter B shares (tmB, tmBt); 64-row A boxes
+      pl->kind = PK_NT_208; bn = 208; boxm = kGemmABoxRows<208, false>;
+      boxn = b_share_rows(208, ntcl, 0); boxn_t = b_share_rows(208, ntcl, ntcl - 1);
     }
     int rc = make_tmap(c, &pl->tmA, A, K, M, lda, BK, boxm);
     if (rc) return rc;
     rc = make_tmap(c, &pl->tmB, B, K, N, ldb, BK, boxn);
     if (rc) return rc;
+    if (boxn_t && (rc = make_tmap(c, &pl->tmBt, B, K, N, ldb, BK, boxn_t))) return rc;
   } else {
     // K (batch rows) need not be a multiple of 64: rows past the extent are TMA zero-fill.  Wide outputs take the 208-wide
     // tile, run as 2-CTA clusters over n-tile pairs, wherever it needs an even number of n-tiles and no more than the
@@ -367,6 +370,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     if (mode == 0) {
       if ((rc = make_tmap(c, &pl->tmA2, A2, K, M, lda, BK, boxm))) return rc;
       if ((rc = make_tmap(c, &pl->tmB2, B2, K, N, ldb, BK, boxn))) return rc;
+      if (boxn_t && (rc = make_tmap(c, &pl->tmB2t, B2, K, N, ldb, BK, boxn_t))) return rc;
     } else {
       if ((rc = make_tmap(c, &pl->tmA2, A2, M, K, lda, 64, BK))) return rc;
       if ((rc = make_tmap(c, &pl->tmB2, B2, N, K, ldb, 64, BK))) return rc;

@@ -18,10 +18,10 @@
 // the per-row epilogue; the scratch is then reused as the bf16 staging of the store.  Meanwhile
 // the producer keeps filling the smem ring with the next tile's operands.  Pipelines: smem ring
 // full/empty mbarriers (TMA <-> wgmma), static round-robin tile scheduler (grid = #SMs).  The 128 x 208
-// K-major kernel runs as 2-CTA clusters that share the B tile (kGemmCluster).  Its PINGPONG instances, launched for
-// short-K GEMMs with a plain bias + activation epilogue, run the two consumer warpgroups in ping-pong: each runs its 64
-// rows of a tile as a half-item of its own, the mainloops take turns through two named barriers, and each warpgroup's
-// epilogue runs under the other one's wgmma.  A ring stage then holds one half-item's 64 A rows and the whole B tile.
+// K-major kernel runs as 4-CTA clusters that share the B tile (kGemmCluster).  Its PINGPONG instances, launched for
+// every fixed epilogue signature, run the two consumer warpgroups in ping-pong: each runs its 64 rows of a tile as a
+// half-item of its own, the mainloops take turns through two named barriers, and each warpgroup's epilogue runs under
+// the other one's wgmma.  A ring stage then holds one half-item's 64 A rows and the whole B tile.
 // The 128 x 208 MN-major kernel (split-K weight gradients of the 400- and 401-wide layers) takes B as three 64-column
 // boxes and a 16-column tail box and runs as 2-CTA clusters over n-tile pairs that share the A tile.
 #pragma once
@@ -156,15 +156,23 @@ struct GemmCfg {
   static_assert(!PINGPONG || (STAGES == 5 && SMEM_BYTES <= kSmemBudget), "ping-pong ring");
 };
 
-// CTAs per cluster (the default of the kernel's CL).  The 128 x 208 K-major kernel runs as 2-CTA clusters on adjacent
-// m-tiles of one n-tile: both read the same B tile (a slice of the weight matrix), so each CTA loads BN / 2 of its rows
-// and multicasts them into both CTAs' stage.  That cuts the bytes L2 feeds each CTA per k-block from 43 008 to 29 696,
-// which bound the long-K mainloop.  The 128 x 208 MN-major kernel is launched with CL = 2 when its n-tile count is even:
-// the two n-tiles of one (split, m-tile) read the same A tile (128 columns of the same batch rows), so each CTA loads
-// one 64-column box of it and multicasts it into both CTAs' stage (49 152 -> 34 816 bytes per CTA and k-block with the
-// 208-wide B).
+// CTAs per cluster (the default of the kernel's CL).  The 128 x 208 K-major kernel runs as 4-CTA clusters on adjacent
+// m-tiles of one n-tile: all four read the same B tile (a slice of the weight matrix), so each CTA loads a quarter of
+// its rows and multicasts them into every CTA's stage.  Per 128 rows and k-block L2 then feeds a CTA 16 384 + 6 656 B
+// cooperatively, and 2 x (8 192 + 6 656) = 29 696 B in ping-pong, which loads the B tile once per 64-row half.  The
+// 128 x 208 MN-major kernel is launched with CL = 2 when its n-tile count is even: the two n-tiles of one (split,
+// m-tile) read the same A tile (128 columns of the same batch rows), so each CTA loads one 64-column box of it and
+// multicasts it into both CTAs' stage (49 152 -> 34 816 bytes per CTA and k-block with the 208-wide B).
 template <int BN, bool A_MN, bool B_MN>
-constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 2 : 1;
+constexpr int kGemmCluster = (BN == 208 && !A_MN && !B_MN) ? 4 : 1;
+// K-major B share of cluster rank r: whole 8-row (1 KB) swizzle atoms, so that every share lands on an atom boundary of
+// the stage and the B descriptor is that of one box.  The first (BN / 8) % CL ranks take one atom more: 208 rows over 4
+// CTAs are 56 + 56 + 48 + 48, at rows (and stage offsets of 128 B per row) 0, 56, 112, 160.  The producer loads the taller
+// shares through tmB / tmB2 and the shorter ones through tmBt / tmB2t.
+__host__ __device__ constexpr int b_share_rows(int bn, int cl, int r) { return 8 * (bn / 8 / cl + (r < bn / 8 % cl)); }
+__host__ __device__ constexpr int b_share_row0(int bn, int cl, int r) {
+  return 8 * (r * (bn / 8 / cl) + (r < bn / 8 % cl ? r : bn / 8 % cl));
+}
 // MN-major 208-wide B tile: three 64-column boxes (128-byte swizzle) and the last 16 columns as a box of their own
 // (32-byte swizzle, tensor map tmBt) behind them, read by an m64n192 and an m64n16 wgmma
 constexpr int kTnTail = 16;
@@ -172,7 +180,8 @@ constexpr int kTnTail = 16;
 // EPI: the fused epilogue's signature (epi_sig), or kEpiUniversal.
 // PINGPONG: the consumer warpgroups run the 64-row halves of each tile as half-items of their own (see the consumer loop)
 // CL: CTAs per cluster; with MN-major operands the cluster's CTAs take adjacent n-tiles of one m-tile.
-// tmBt / tmB2t: the 16-column tail boxes of tmB / tmB2 (MN-major 208-wide kernel only)
+// tmBt / tmB2t: the 16-column tail boxes of tmB / tmB2 (MN-major 208-wide kernel), or the shorter B shares of a
+// K-major cluster (b_share_rows)
 template <int BN, bool A_MN, bool B_MN, int EPI = kEpiUniversal, bool SPLIT = false, bool PINGPONG = false,
           int CL = kGemmCluster<BN, A_MN, B_MN>>
 // 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
@@ -195,9 +204,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   static_assert(A_MN == B_MN, "one operand form per kernel");
   // K-major: each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for
   // one box.  MN-major: each CTA's share of the A tile is one whole 64-column box, so the A descriptor is unchanged.
-  static_assert(CL == 1 || CL == 2, "cluster size");
-  static_assert(CL == 1 || (!B_MN && (BN / CL) % 8 == 0 && (Cfg::B_BYTES / CL) % 1024 == 0) || (B_MN && kTail && BM / CL == 64),
-                "multicast share");
+  static_assert(CL == 1 || CL == 2 || CL == 4, "cluster size");
+  static_assert(CL == 1 || (!B_MN && BN % 8 == 0 && BK * 2 == 128 && b_share_rows(BN, CL, CL - 1) > 0) ||
+                (B_MN && kTail && BM / CL == 64), "multicast share");
+  // K-major cluster: ranks below kBigShares load their B share through tmB / tmB2, the others through tmBt / tmB2t
+  constexpr int kBigShares = (BN / 8) % CL == 0 ? CL : (BN / 8) % CL;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -214,7 +225,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if constexpr (SPLIT) { tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmB2); }
-    if constexpr (kTail) { tma_prefetch_desc(&tmBt); if constexpr (SPLIT) tma_prefetch_desc(&tmB2t); }
+    if constexpr (kTail || (CL > 1 && !B_MN)) { tma_prefetch_desc(&tmBt); if constexpr (SPLIT) tma_prefetch_desc(&tmB2t); }
     if (p.tma_store) tma_prefetch_desc(&tmC);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
@@ -232,7 +243,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // Work items walk (split, m-group, n-group) with one item per cluster.  K-major: CTA rank r of a cluster takes m-tile
   // CL * group + r of the item's n-tile; m-tiles are rounded up to whole groups: a CTA on a tile past M loads its share
   // of B, computes on zero-filled A rows and stores nothing (every store is guarded by row < M or clipped at the tensor
-  // extent), so both CTAs walk the same k-blocks through the ring.  MN-major (n_tiles a multiple of CL): rank r takes
+  // extent), so all CTAs walk the same k-blocks through the ring.  MN-major (n_tiles a multiple of CL): rank r takes
   // n-tile CL * group + r of the item's m-tile; both CTAs share split and m-tile, so they walk the same k-blocks too.
   constexpr bool kPairN = CL > 1 && B_MN;
   const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
@@ -243,8 +254,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int total = tiles * p.splits;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
   // Ping-pong: an item is two half-items, rows [0, 64) for consumer warpgroup 0 and [64, 128) for warpgroup 1, whose
-  // k-blocks enter the ring one half after the other.  The second half is skipped in both CTAs of the cluster when rank
-  // 0's first row of it is past M (rank 1's rows are higher still), so the peers keep walking the same k-blocks.
+  // k-blocks enter the ring one half after the other.  The second half is skipped in all CTAs of the cluster when rank
+  // 0's first row of it is past M (the other ranks' rows are higher still), so the peers keep walking the same k-blocks.
   auto halves_of = [&](int rem) -> int {
     if constexpr (PP) return (rem / p.n_tiles) * CL * BM + Cfg::A_ROWS < p.M ? 2 : 1;
     else return 1;
@@ -296,8 +307,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               for (int a = 0; a < BM / 64; ++a)
                 tma_load_2d(a_dst + a * (BK * 128), ta, full_bar(stage), m0 + a * 64, k0);
             }
-            if constexpr (CL > 1 && !B_MN) {   // rows [n0 + r BN/CL, +BN/CL) into this and the peer CTA; the full barrier expects both shares
-              tma_load_2d_multicast(b_dst + rank * (Cfg::B_BYTES / CL), tb, full_bar(stage), k0, n0 + rank * (BN / CL), (1u << CL) - 1);
+            if constexpr (CL > 1 && !B_MN) {   // this rank's B share into every CTA; the full barrier expects all shares
+              const int r0 = b_share_row0(BN, CL, rank);
+              const CUtensorMap* const tbs = rank < kBigShares ? tb : (SPLIT && opart == 1) ? &tmB2t : &tmBt;
+              tma_load_2d_multicast(b_dst + r0 * (BK * 2), tbs, full_bar(stage), k0, n0 + r0, (1u << CL) - 1);
             } else if constexpr (!B_MN) {
               tma_load_2d(b_dst, tb, full_bar(stage), k0, n0);
             } else {
@@ -383,12 +396,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
       }
     };
-    // a stage this warp has finished reading is released in this CTA and in its cluster peer (whose producer multicasts into it)
+    // a stage this warp has finished reading is released in this CTA and in its cluster peers (whose producers multicast into it)
     auto release = [&](int s) {
       __syncwarp();
       if (lane == 0) {
         mbar_arrive(empty_bar(s));
-        if constexpr (CL > 1) mbar_arrive_cluster(mapa_shared(empty_bar(s), uint32_t(rank ^ 1)));
+#pragma unroll
+        for (int d = 1; d < CL; ++d) mbar_arrive_cluster(mapa_shared(empty_bar(s), uint32_t(rank ^ d)));
       }
     };
     int stage = 0;
