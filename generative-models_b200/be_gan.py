@@ -14,7 +14,8 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import parallel as par
 from gm_b200 import AdamHP, GmError
-from gm_b200.gan_api import builtin_step, Generator, GANTrainerBase, _EngineBacked, to_cuda, G_NET, D_NET
+from gm_b200.gan_api import (builtin_step, Generator, GANTrainerBase, _EngineBacked, EngineCall, began_reference_loop,
+                             refuse_multi_rank, slot_ring, _split_like, to_cuda, G_NET, D_NET)
 
 
 class Discriminator(_EngineBacked):
@@ -26,8 +27,25 @@ class Discriminator(_EngineBacked):
         self.decoder = nn.Linear(hidden_dim, image_size)
 
     def forward(self, x):
-        # inference-time use only: plain torch on the engine's fp32 master weights
-        return self.decoder(torch.relu(self.encoder(to_cuda(x))))
+        if not torch.is_grad_enabled():
+            # inference: plain torch on the engine's fp32 master weights
+            return self.decoder(torch.relu(self.encoder(to_cuda(x))))
+        # a user-written train_D / train_G (README.md:31): one autograd node over gm_gan_ae_forward / _backward, whose
+        # call keeps its activations in one of the engine's D row regions until its backward ran
+        x = to_cuda(x).float().contiguous()
+        eng = self._engine_for(x.shape[0], "Discriminator")
+        ring = slot_ring(eng, "Discriminator", eng.num_slots())
+        params = tuple(self.parameters())
+
+        def fwd(x):
+            slot, gen = ring.take()
+            return eng.ae_forward(slot, x), (slot, gen)
+
+        def bwd(handle, grads, need_dx):
+            ring.check(*handle)
+            flat, dx = eng.ae_backward(handle[0], grads[0].float().contiguous(), need_dx)
+            return dx, _split_like(flat, params)
+        return EngineCall.apply(x, fwd, bwd, *params)
 
 
 class BEGAN(nn.Module):
@@ -45,6 +63,11 @@ class BEGANTrainer(GANTrainerBase):
     variant = "began"
 
     def train(self, num_epochs, G_lr=1e-4, D_lr=1e-4, D_steps=1, GAMMA=0.50, LAMBDA=1e-3, K=0.00):
+        if self._has_custom_step():
+            # an overridden train_D / train_G: the reference's loop verbatim over the autograd nodes of model.G / model.D
+            refuse_multi_rank("train_D / train_G")
+            self._ensure_engine(getattr(self.train_iter, "batch_size", None) or next(iter(self.train_iter))[0].shape[0])
+            return began_reference_loop(self, num_epochs, G_lr, D_lr, D_steps, GAMMA, LAMBDA, K)
         par.require_single_process(self.name + "Trainer")
         hpG, hpD = AdamHP.make(G_lr), AdamHP.make(D_lr)
         epoch_steps = int(np.ceil(len(self.train_iter) / D_steps))

@@ -116,6 +116,11 @@ def lib():
     L.gm_gan_d_backward.argtypes = [vp, i, i, vp, vp, vp]
     L.gm_gan_g_forward.argtypes = [vp, vp, i, vp, vp]
     L.gm_gan_g_backward.argtypes = [vp, i, vp, vp]
+    L.gm_gan_ae_forward.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_gan_ae_backward.argtypes = [vp, i, i, vp, vp, vp]
+    L.gm_gan_num_q_slots.argtypes = [vp]
+    L.gm_gan_q_forward.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_gan_q_backward.argtypes = [vp, i, i, vp, vp, vp]
     L.gm_vae_create.argtypes = [vp, C.POINTER(VaeDesc), C.POINTER(vp)]
     L.gm_vae_destroy.argtypes = [vp]
     L.gm_vae_param_count.argtypes = [vp]

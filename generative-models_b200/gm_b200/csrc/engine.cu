@@ -682,6 +682,16 @@ struct gm_comm {
 
 struct CustomPlans {   // custom-loss path (engine_custom.inl): per-slot D forward / backward, G output kept in DA2
   GemmPlan d1[4], dw1[4], dx[4], g2;
+  GemmPlan ae_enc[2], ae_dec[2], ae_gwd[2], ae_de[2];   // BEGAN: the autoencoder D on the real / fake row regions
+};
+// InfoGAN's per-call Q (engine_custom.inl): each of kQSlots calls keeps its input and hidden rows until its backward ran;
+// the backward scratch (DINF, DHQ, the split-K partials PQ1 / PQ2) is the fused Q step's
+constexpr int kQSlots = 2;
+struct QCallBufs {
+  __nv_bfloat16 *X = nullptr, *H = nullptr;   // [x | 1], [relu(h) | 1]
+};
+struct QCallPlans {
+  GemmPlan q1[kQSlots], q2[kQSlots], gq2[kQSlots], dhq[kQSlots], gq1[kQSlots], dx[kQSlots];
 };
 
 struct gm_gan {
@@ -738,6 +748,9 @@ struct gm_gan {
   GradSegs pend_segs[2];
   std::map<int, StepPlans> plans;
   std::map<int, CustomPlans> cplans;
+  QCallBufs qs[kQSlots];     // per-call Q buffers, allocated on the first per-call Q entry
+  bool qs_ready = false;
+  std::map<int, QCallPlans> qplans;
   std::vector<void*> allocs;
   BfArena arena;
   long long lo = 0;          // arena.lo_off: > 0 in split-operand mode
@@ -889,7 +902,7 @@ extern "C" int gm_gan_bind(gm_gan* g, int net, float* p, float* gr, float* m, fl
   if (reinterpret_cast<uintptr_t>(p) & 15)
     return fail(g->ctx, GM_ERR_ARG, "parameter buffer must be 16-byte aligned");
   g->par[net] = p; g->grd[net] = gr; g->am[net] = m; g->av[net] = v;
-  g->plans.clear(); g->cplans.clear();
+  g->plans.clear(); g->cplans.clear(); g->qplans.clear();
   return GM_OK;
 }
 
@@ -1448,7 +1461,7 @@ extern "C" int gm_gan_bind_q(gm_gan* g, float* q_params, float* q_grads, float* 
   if (!g || !q_params || !q_grads) return g ? fail(g->ctx, GM_ERR_ARG, "gm_gan_bind_q: bad argument") : GM_ERR_ARG;
   if (g->d.variant != GM_INFO) return fail(g->ctx, GM_ERR_STATE, "gm_gan_bind_q: engine was not created with GM_INFO");
   g->parQ = q_params; g->grdQ = q_grads; g->amQ = q_m; g->avQ = q_v; g->amG2 = g_mi_m; g->avG2 = g_mi_v;
-  g->plans.clear(); g->cplans.clear();
+  g->plans.clear(); g->cplans.clear(); g->qplans.clear();
   return GM_OK;
 }
 extern "C" int gm_gan_q_param_count(const gm_gan* g) { return (g && g->d.variant == GM_INFO) ? g->Qn.total : GM_ERR_ARG; }
@@ -1682,11 +1695,12 @@ extern "C" int gm_gan_debug_read(gm_gan* g, int which, int row0, int rows, int c
   if (!g || !out_dev || rows <= 0 || cols <= 0 || row0 < 0) return GM_ERR_ARG;
   const int plane = which / 16;   // 0: hi + lo, 1: hi plane only, 2: lo plane only
   which %= 16;
-  const __nv_bfloat16* src[7] = {g->Zb, g->Hg, g->Xall, g->Aall, g->DHall, g->DA2, g->DHg};
-  const int ld[7] = {g->ZP, g->HP, g->XP, g->HP, g->HP, g->XP, g->HP};
-  const long long nrow[7] = {g->Bmax, g->Bmax, (long long)g->nreg * g->Bmax, (long long)g->nreg * g->Bmax,
-                             (long long)g->nreg * g->Bmax, g->Bmax, g->Bmax};
-  if (which < 0 || which > 6 || cols > ld[which]) return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: bad buffer / extent");
+  const __nv_bfloat16* src[9] = {g->Zb, g->Hg, g->Xall, g->Aall, g->DHall, g->DA2, g->DHg, g->qs[0].H, g->qs[1].H};
+  const int ld[9] = {g->ZP, g->HP, g->XP, g->HP, g->HP, g->XP, g->HP, g->HP, g->HP};
+  const long long nrow[9] = {g->Bmax, g->Bmax, (long long)g->nreg * g->Bmax, (long long)g->nreg * g->Bmax,
+                             (long long)g->nreg * g->Bmax, g->Bmax, g->Bmax, g->Bmax, g->Bmax};
+  static_assert(kQSlots == 2, "debug buffers 7, 8 are the Q call slots' hidden rows");
+  if (which < 0 || which > 8 || cols > ld[which] || !src[which]) return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: bad buffer / extent");
   if ((long long)row0 + rows > nrow[which])
     return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: rows [%d, %lld) run past the buffer's %lld rows", row0, (long long)row0 + rows, nrow[which]);
   const long long tot = (long long)rows * cols;

@@ -173,7 +173,7 @@ class GanEngine:
         check(self.h, lib().gm_gan_sample_indices(self.g, batch, int(step), _ptr(out), _stream()))
         return out
 
-    BUFFERS = {"Zb": 0, "Hg": 1, "Xall": 2, "Aall": 3, "DHall": 4, "DA2": 5, "DHg": 6}
+    BUFFERS = {"Zb": 0, "Hg": 1, "Xall": 2, "Aall": 3, "DHall": 4, "DA2": 5, "DHg": 6, "HQ0": 7, "HQ1": 8}
 
     def debug_read(self, which, row0, rows, cols, plane=0):
         """An internal bf16 activation buffer as fp32 [rows, cols] (plane 0: hi + lo in split mode, 1: hi, 2: lo); tests only."""
@@ -230,7 +230,11 @@ class GanEngine:
     # ---- custom-loss path (README.md:31): forward / backward halves as separate calls
     @property
     def supports_custom_loss(self):
-        return self.variant not in ("began",)        # BEGAN's D is an autoencoder (src/be_gan.py:63-76)
+        """True where Discriminator.forward is the scalar-score node (gm_gan_d_*); BEGAN's D is an autoencoder
+        (src/be_gan.py:63-76) with nodes of its own (ae_forward / ae_backward)"""
+        return self.variant not in ("began",)
+
+    supports_custom_g = True       # Generator.forward is a node on every variant (gm_gan_g_*)
 
     def num_slots(self):
         return lib().gm_gan_num_slots(self.g)
@@ -257,6 +261,20 @@ class GanEngine:
     def g_backward(self, dimages):
         check(self.h, lib().gm_gan_g_backward(self.g, dimages.shape[0], _ptr(dimages), _stream()))
         return self.grads[0]
+
+    def ae_forward(self, slot, x):
+        """BEGAN's Discriminator.forward (the autoencoder) on slot's row region: x [n, image_size] -> recon, fp32"""
+        n = x.shape[0]
+        out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_gan_ae_forward(self.g, slot, _ptr(x), n, _ptr(out), _stream()))
+        return out
+
+    def ae_backward(self, slot, drecon, need_dx):
+        """-> (flat D gradient (engine buffer, overwritten by the next call), dL/dx or None) of ae_forward's call on slot"""
+        n = drecon.shape[0]
+        dx = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32) if need_dx else None
+        check(self.h, lib().gm_gan_ae_backward(self.g, slot, n, _ptr(drecon), _ptr(dx), _stream()))
+        return self.grads[1], dx
 
     def began_state(self, values=None):
         """BEGAN device state (list of 11 floats, see include/gm_b200.h); pass values to set."""
@@ -350,6 +368,24 @@ class InfoGanEngine(GanEngine):
     def apply_mi(self, hp):
         self.mi_steps += 1
         check(self.h, lib().gm_gan_apply_mi(self.g, C.byref(hp), self.mi_steps, _stream()))
+
+    # ---- per-call Q (user-written train_Q)
+    def num_q_slots(self):
+        return lib().gm_gan_num_q_slots(self.g)
+
+    def q_forward(self, slot, x):
+        """Q.forward on slot's buffers: x [n, image_size] fp32 -> codes [n, disc + cont] fp32 (logits | continuous)"""
+        n = x.shape[0]
+        out = torch.empty(n, self.q_shapes[3][0], device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_gan_q_forward(self.g, slot, _ptr(x), n, _ptr(out), _stream()))
+        return out
+
+    def q_backward(self, slot, dcodes, need_dx):
+        """-> (flat Q gradient (q_grads, overwritten by the next call), dL/dx or None) of q_forward's call on slot"""
+        n = dcodes.shape[0]
+        dx = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32) if need_dx else None
+        check(self.h, lib().gm_gan_q_backward(self.g, slot, n, _ptr(dcodes), _ptr(dx), _stream()))
+        return self.q_grads, dx
 
 
 class VaeEngine:

@@ -73,7 +73,7 @@ class Generator(_EngineBacked):
     def forward(self, x):
         x = to_cuda(x).float().contiguous()
         eng = self._engine_for(x.shape[0], "Generator")
-        if torch.is_grad_enabled() and eng.supports_custom_loss:
+        if torch.is_grad_enabled() and eng.supports_custom_g:
             return _GForward.apply(x, eng, *self.parameters())     # custom-loss path (README.md:31)
         return eng.generate(x)
 
@@ -273,11 +273,15 @@ class FusedAdam(torch.optim.Optimizer):
                 _lib.adam_step(p.data, p.grad.contiguous(), st["exp_avg"], st["exp_avg_sq"], hp, st["step"])
 
 
-def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step=None):
+def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step=None, d_args=tuple, after_G=None,
+                   epoch_line=None):
     """The reference's loop verbatim (src/ns_gan.py:107-156) for a Trainer tr whose train_D / train_G were overridden: the
     override's torch loss drives the CUDA forward / backward kernels through model.G / model.D and their autograd nodes.
     after_step(), when given, runs after every optimizer step (the conv trainers mark their modules' parameters as newer
-    than their engine's)."""
+    than their engine's).  The BEGAN and InfoGAN loops (src/be_gan.py:109-205, src/info_gan.py:130-221) add to it:
+    d_args() gives train_D's extra arguments (BEGAN's K), train_D may return (D_loss, *rest), after_G(images, rest) runs
+    after each G step (BEGAN's K control and schedulers, InfoGAN's Q step) and epoch_line(epoch, G_losses, D_losses) is
+    the epoch's log line."""
     epoch_steps = int(np.ceil(len(tr.train_iter) / D_steps))
     for epoch in range(1, num_epochs + 1):
         tr.model.train()
@@ -287,7 +291,9 @@ def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step
             for _ in range(D_steps):
                 images = tr.process_batch(tr.train_iter)
                 D_optimizer.zero_grad()
-                D_loss = tr.train_D(images)
+                D_loss, rest = tr.train_D(images, *d_args()), ()
+                if isinstance(D_loss, tuple):
+                    D_loss, rest = D_loss[0], D_loss[1:]
                 D_loss.backward()
                 D_optimizer.step()
                 if after_step is not None:
@@ -301,13 +307,69 @@ def reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_step
             G_optimizer.step()
             if after_step is not None:
                 after_step()
+            if after_G is not None:
+                after_G(images, rest)
         G_losses, D_losses = torch.stack(G_losses).tolist(), torch.stack(D_losses).tolist()
         tr.Glosses.extend(G_losses)
         tr.Dlosses.extend(D_losses)
-        print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
+        if epoch_line is None:
+            print("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses)))
+        else:
+            print(epoch_line(epoch, G_losses, D_losses))
         tr.num_epochs += 1
         if tr.viz:
             tr.generate_images(epoch)
+
+
+def began_reference_loop(tr, num_epochs, G_lr, D_lr, D_steps, GAMMA, LAMBDA, K):
+    """src/be_gan.py:109-205 for a BEGANTrainer tr with an overridden train_D / train_G: FusedAdam for G and D, two
+    ReduceLROnPlateau on the convergence measure, and K <- clip(K + LAMBDA (GAMMA DX - DG), 0, 1) on the host after every
+    outer step"""
+    from torch.optim.lr_scheduler import ReduceLROnPlateau
+    G_optimizer = FusedAdam([p for p in tr.model.G.parameters() if p.requires_grad], lr=G_lr)
+    D_optimizer = FusedAdam([p for p in tr.model.D.parameters() if p.requires_grad], lr=D_lr)
+    G_scheduler = ReduceLROnPlateau(G_optimizer, factor=0.50, threshold=0.01, patience=5 * len(tr.train_iter))
+    D_scheduler = ReduceLROnPlateau(D_optimizer, factor=0.50, threshold=0.01, patience=5 * len(tr.train_iter))
+    st = dict(K=K, convergence=float("nan"))
+
+    def control(images, rest):
+        DX_loss, DG_loss = rest
+        st["convergence"] = (DX_loss + torch.abs(GAMMA * DX_loss - DG_loss)).item()
+        K_update = (st["K"] + LAMBDA * (GAMMA * DX_loss - DG_loss)).item()
+        st["K"] = min(max(0, K_update), 1)
+        D_scheduler.step(st["convergence"])
+        G_scheduler.step(st["convergence"])
+
+    def line(epoch, G_losses, D_losses):
+        return ("Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f, K: %.4f, Convergence Measure: %.4f"
+                % (epoch, num_epochs, np.mean(G_losses), np.mean(D_losses), st["K"], st["convergence"]))
+    reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, d_args=lambda: (st["K"],), after_G=control,
+                   epoch_line=line)
+
+
+def info_reference_loop(tr, num_epochs, G_lr, D_lr, D_steps):
+    """src/info_gan.py:130-221 for an InfoGANTrainer tr with an overridden train_D / train_G / train_Q: FusedAdam for D and
+    G, and MI_optimizer = FusedAdam over G's and Q's parameters with moments of its own, stepped after every G step"""
+    G_params = [p for p in tr.model.G.parameters() if p.requires_grad]
+    D_optimizer = FusedAdam([p for p in tr.model.D.parameters() if p.requires_grad], lr=D_lr)
+    G_optimizer = FusedAdam(G_params, lr=G_lr)
+    MI_optimizer = FusedAdam(G_params + [p for p in tr.model.Q.parameters() if p.requires_grad], lr=G_lr)
+    MI_losses = []
+
+    def q_step(images, rest):
+        MI_optimizer.zero_grad()
+        MI_loss = tr.train_Q(images)
+        MI_losses.append(MI_loss.detach())
+        MI_loss.backward()
+        MI_optimizer.step()
+
+    def line(epoch, G_losses, D_losses):
+        mi = torch.stack(MI_losses).tolist()
+        MI_losses.clear()
+        tr.MIlosses.extend(mi)
+        return "Epoch[%d/%d], G Loss: %.4f, D Loss: %.4f, MI Loss: %.4f" % (epoch, num_epochs, np.mean(G_losses),
+                                                                             np.mean(D_losses), np.mean(mi))
+    reference_loop(tr, num_epochs, G_optimizer, D_optimizer, D_steps, after_G=q_step, epoch_line=line)
 
 
 def has_custom_compute_batch(tr):
@@ -315,11 +377,12 @@ def has_custom_compute_batch(tr):
     return not getattr(type(tr).compute_batch, "_gm_builtin", False)
 
 
-def refuse_multi_rank():
-    """an overridden compute_batch trains on one process: refused under a process group of more than one rank"""
+def refuse_multi_rank(what="compute_batch"):
+    """an overridden compute_batch (or train_D / train_G / train_Q: `what`) trains on one process: refused under a
+    process group of more than one rank"""
     from . import parallel as par
     if par.world_size() > 1:
-        raise GmError("an overridden compute_batch trains on one process; data-parallel training runs the built-in step")
+        raise GmError("an overridden %s trains on one process; data-parallel training runs the built-in step" % what)
 
 
 def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=None):

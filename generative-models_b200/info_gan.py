@@ -5,6 +5,8 @@ G's input is noise z plus a one-hot categorical code and a Gaussian continuous c
 auxiliary network Q (src/info_gan.py:78-94) recovers the codes from G's output and the
 mutual-information step trains G and Q with a third Adam (src/info_gan.py:146-148,196-205).
 """
+import weakref
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -12,7 +14,9 @@ import torch.nn as nn
 from utils import *  # noqa: F401,F403
 from gm_b200 import parallel as par
 from gm_b200 import AdamHP, GmError, InfoGanEngine
-from gm_b200.gan_api import builtin_step, Generator as _Generator, Discriminator as _Discriminator, GANTrainerBase, GradHandoff, flat_pairs, to_cuda, G_NET, D_NET
+from gm_b200.gan_api import (builtin_step, Generator as _Generator, Discriminator as _Discriminator, GANTrainerBase, GradHandoff,
+                             EngineCall, _EngineBacked, info_reference_loop, refuse_multi_rank, slot_ring, _split_like, flat_pairs,
+                             to_cuda, G_NET, D_NET)
 
 
 class Generator(_Generator):
@@ -34,7 +38,7 @@ class Discriminator(_Discriminator):
         self.discriminator = nn.Linear(hidden_dim, output_dim)
 
 
-class Q(nn.Module):
+class Q(_EngineBacked):
     """ Auxiliary network Q(c|x) (src/info_gan.py:78-94); parameters live in the engine """
 
     def __init__(self, image_size, hidden_dim, disc_dim, cont_dim):
@@ -44,8 +48,26 @@ class Q(nn.Module):
         self.inference = nn.Linear(hidden_dim, disc_dim + cont_dim)
 
     def forward(self, x):
-        # inference-time use only (plain torch on the engine's master weights)
-        inferred = self.inference(torch.relu(self.linear(to_cuda(x))))
+        if not torch.is_grad_enabled():
+            # inference: plain torch on the engine's master weights
+            inferred = self.inference(torch.relu(self.linear(to_cuda(x))))
+            return inferred[:, :self.disc_dim], inferred[:, self.disc_dim:]
+        # a user-written train_Q (README.md:31): one autograd node over gm_gan_q_forward / _backward with buffers of its
+        # own per live call, so Q(G(z)) can await its backward while G's does
+        x = to_cuda(x).float().contiguous()
+        eng = self._engine_for(x.shape[0], "Q")
+        ring = slot_ring(eng, "Q", eng.num_q_slots())
+        params = tuple(self.parameters())
+
+        def fwd(x):
+            slot, gen = ring.take()
+            return eng.q_forward(slot, x), (slot, gen)
+
+        def bwd(handle, grads, need_dx):
+            ring.check(*handle)
+            flat, dx = eng.q_backward(handle[0], grads[0].float().contiguous(), need_dx)
+            return dx, _split_like(flat, params)
+        inferred = EngineCall.apply(x, fwd, bwd, *params)
         return inferred[:, :self.disc_dim], inferred[:, self.disc_dim:]
 
 
@@ -69,6 +91,11 @@ class InfoGANTrainer(GANTrainerBase):
     def __init__(self, model, train_iter, val_iter, test_iter, viz=False):
         super().__init__(model, train_iter, val_iter, test_iter, viz)
         self.MIlosses = []
+        if isinstance(getattr(model, "Q", None), _EngineBacked):
+            object.__setattr__(model.Q, "_owner", weakref.ref(self))
+
+    def _has_custom_step(self):
+        return super()._has_custom_step() or not getattr(type(self).train_Q, "_gm_builtin", False)
 
     def _ensure_engine(self, batch):
         if self._engine is not None and batch <= self._max_batch:
@@ -86,6 +113,7 @@ class InfoGANTrainer(GANTrainerBase):
         eng.load_q([p.data for p in qp])
         for p, v in zip(qp, eng.q_views()):
             p.data = v
+        m.Q._attach(eng, None)
         if old is not None:
             for a, b in ((eng.exp_avg, old.exp_avg), (eng.exp_avg_sq, old.exp_avg_sq)):
                 for net in (G_NET, D_NET):
@@ -99,6 +127,12 @@ class InfoGANTrainer(GANTrainerBase):
 
     def train(self, num_epochs, G_lr=2e-4, D_lr=2e-4, D_steps=1):
         """ src/info_gan.py:130-221: per outer step D update(s), G update, then the Q / MI update """
+        if self._has_custom_step():
+            # an overridden train_D / train_G / train_Q: the reference's loop verbatim over the autograd nodes of model.G /
+            # model.D / model.Q
+            refuse_multi_rank("train_D / train_G / train_Q")
+            self._ensure_engine(getattr(self.train_iter, "batch_size", None) or next(iter(self.train_iter))[0].shape[0])
+            return info_reference_loop(self, num_epochs, G_lr, D_lr, D_steps)
         par.require_single_process(self.name + "Trainer")
         hpG, hpD = AdamHP.make(G_lr), AdamHP.make(D_lr)
         epoch_steps = int(np.ceil(len(self.train_iter) / D_steps))
@@ -162,6 +196,7 @@ class InfoGANTrainer(GANTrainerBase):
         loss = eng.g_grad(images.shape[0], noise=noise.float().contiguous())
         return self._loss_tensor(G_NET, loss)
 
+    @builtin_step
     def train_Q(self, images, LAMBDA=1):
         """ src/info_gan.py:269-304: returns MI_loss; .backward() delivers the G and Q gradients """
         if LAMBDA != 1:

@@ -229,7 +229,8 @@ int gm_gan_sample_indices(gm_gan* gan, int batch, uint64_t step, int* idx_dev, g
 int gm_gan_debug_noise(gm_gan* gan, int batch, uint64_t seed, uint64_t step, int g_step, float* out_dev, gm_stream stream);
 
 /* test aid: an internal bf16 activation buffer as fp32 (hi + lo planes summed in split mode) -> out_dev [rows, cols];
- * which: 0 noise operand, 1 G hidden, 2 image rows [real|fake|...], 3 D hidden, 4 D hidden gradient, 5 dL/dG-pre-sigmoid, 6 G hidden gradient */
+ * which: 0 noise operand, 1 G hidden, 2 image rows [real|fake|...], 3 D hidden, 4 D hidden gradient, 5 dL/dG-pre-sigmoid, 6 G hidden gradient,
+ * 7 / 8 the hidden rows of per-call Q slot 0 / 1 (InfoGAN, after a gm_gan_q_forward) */
 int gm_gan_debug_read(gm_gan* gan, int which, int row0, int rows, int cols, float* out_dev, gm_stream stream);
 
 /* D outputs of the last *_grad call (D step: batch real then batch fake; G step:
@@ -237,7 +238,7 @@ int gm_gan_debug_read(gm_gan* gan, int which, int row0, int rows, int cols, floa
 int gm_gan_scores(gm_gan* gan, float* dst_dev, int n, gm_stream stream);
 /* ---- custom-loss path --------------------------------------------------------
  * README.md:31 tells users to "edit train_D and train_G": a loss written in torch on
- * DX_score / DG_score must still train.  These four calls are Generator.forward /
+ * DX_score / DG_score must still train.  These calls are Generator.forward /
  * Discriminator.forward (src/ns_gan.py:43-46,57-60) and their backward halves as
  * separate entry points; the host wraps them in torch.autograd.Function objects
  * (gm_b200/gan_api.py).  `slot` in [0, gm_gan_num_slots) picks the row region that keeps
@@ -250,8 +251,23 @@ int gm_gan_d_forward(gm_gan* gan, int slot, const float* x_dev, int batch, float
 int gm_gan_d_backward(gm_gan* gan, int slot, int batch, const float* dscore_dev, float* dx_dev, gm_stream stream);
 /* images_dev[batch, image_size] = G(noise_dev[batch, z]) keeping the activations for one backward */
 int gm_gan_g_forward(gm_gan* gan, const float* noise_dev, int batch, float* images_dev, gm_stream stream);
-/* dimages_dev[batch, image_size] = dL/dG(z) -> flat G gradient */
+/* dimages_dev[batch, image_size] = dL/dG(z) -> flat G gradient (every variant, BEGAN included) */
 int gm_gan_g_backward(gm_gan* gan, int batch, const float* dimages_dev, gm_stream stream);
+/* BEGAN (GM_BEGAN engines, which refuse gm_gan_d_forward / _backward): Discriminator.forward is the
+ * autoencoder (src/be_gan.py:63-76).  recon_dev [batch, image_size] fp32 = D(x_dev); slot as above.
+ * The backward takes drecon_dev [batch, image_size] = dL/dD(x) and writes the flat D gradient
+ * [enc.W | enc.b | dec.W | dec.b] and, when dx_dev is not null, dx_dev [batch, image_size] = dL/dx
+ * through the autoencoder only.  bf16 engines only (GM_ERR_UNSUPPORTED in split precision). */
+int gm_gan_ae_forward(gm_gan* gan, int slot, const float* x_dev, int batch, float* recon_dev, gm_stream stream);
+int gm_gan_ae_backward(gm_gan* gan, int slot, int batch, const float* drecon_dev, float* dx_dev, gm_stream stream);
+/* InfoGAN (GM_INFO engines, Q bound): Q.forward (src/info_gan.py:78-94) per call, `slot` in
+ * [0, gm_gan_num_q_slots) with buffers of its own (allocated on first use).  codes_dev [batch, 20]
+ * fp32 = [categorical logits | continuous codes].  The backward takes dcodes_dev [batch, 20] and
+ * writes the flat Q gradient (the bound q_grads buffer) and, when dx_dev is not null, dx_dev
+ * [batch, image_size] = dL/dx.  bf16 engines only. */
+int gm_gan_num_q_slots(const gm_gan* gan);
+int gm_gan_q_forward(gm_gan* gan, int slot, const float* x_dev, int batch, float* codes_dev, gm_stream stream);
+int gm_gan_q_backward(gm_gan* gan, int slot, int batch, const float* dcodes_dev, float* dx_dev, gm_stream stream);
 
 /* Generator.forward (src/ns_gan.py:43-46) for sampling: noise [n, z] fp32 -> images
  * [n, image_size] fp32. */
