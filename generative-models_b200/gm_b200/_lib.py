@@ -186,6 +186,11 @@ def lib():
     L.gm_vae_debug_read.argtypes = [vp, i, i, i, i, vp, vp]
     L.gm_vae_set_sampler.argtypes = [vp, C.c_longlong, C.c_longlong, C.c_longlong, u64]
     L.gm_gan_fisher_state.argtypes = [vp, C.POINTER(C.c_float), i, vp]
+    L.gm_bir_vae_create.argtypes = [vp, C.POINTER(VaeDesc), f, C.POINTER(vp)]
+    L.gm_bir_vae_grad.argtypes = [vp, vp, i, vp, i, vp, vp, f, u64, u64, vp, vp]
+    L.gm_bir_vae_forward.argtypes = [vp, vp, i, i, vp, vp, f, u64, u64, vp, vp, vp, vp]
+    L.gm_bir_vae_last_latent.argtypes = [vp, vp, vp, i, vp]
+    L.gm_mmd_gaussian.argtypes = [vp, vp, vp, i, i, f, vp, vp, vp]
     _lib = L
     return L
 

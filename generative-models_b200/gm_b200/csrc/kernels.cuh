@@ -800,6 +800,199 @@ __global__ void vae_losses_final_kernel(const double* __restrict__ part_r, int n
   if (threadIdx.x == 0) { losses[0] = float(a); losses[1] = float(b); }
 }
 
+// ---------------------------------------------------------------- BIR-VAE (src/bir_vae.py:80-95,190-222)
+// mu fp32 [rows, ldm] (the z-wide head) -> z = mu + eps (src/bir_vae.py:88-94) as fp32 zf [rows, z] and as the decoder's
+// bf16 operand [rows, ldz] with a ones column at z, and the MMD's prior sample p [rows, z].  eps: the caller's eps_in
+// (already at the reference's scale), else std * N(0,1); p: the caller's p_in, else N(0,1).  The Philox draws are keyed
+// by seed xor a constant of their own, so no VAE or GAN draw reaches them.  One thread per (row, 8-column group).
+__global__ void bir_latent_kernel(const float* __restrict__ mu, int ldm, const float* __restrict__ eps_in,
+                                  float* __restrict__ eps_out, const float* __restrict__ p_in, float* __restrict__ p_out,
+                                  float* __restrict__ zf, __nv_bfloat16* __restrict__ zb, int ldz, int rows, int z, float std_,
+                                  unsigned long long seed, unsigned long long stream_id, long long lo_off) {
+  griddep_sync();
+  const int groups = ldz / 8, gz = (z + 8) / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)rows * gz) return;
+  const int r = int(t / gz), g = int(t % gz), c0 = g * 8;
+  float e[8], q[8], v[8];
+  if (c0 < z) {
+    const unsigned long long cell = (unsigned long long)r * groups + g;
+    if (eps_in == nullptr) {
+      curandStatePhilox4_32_10_t st;
+      curand_init(seed ^ 0x2545F4914F6CDD1Dull, cell, stream_id * 64ull, &st);
+      const float4 a = curand_normal4(&st), b = curand_normal4(&st);
+      e[0] = a.x; e[1] = a.y; e[2] = a.z; e[3] = a.w; e[4] = b.x; e[5] = b.y; e[6] = b.z; e[7] = b.w;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) e[j] *= std_;
+    }
+    if (p_in == nullptr) {
+      curandStatePhilox4_32_10_t st;
+      curand_init(seed ^ 0x9FB21C651E98DF25ull, cell, stream_id * 64ull, &st);
+      const float4 a = curand_normal4(&st), b = curand_normal4(&st);
+      q[0] = a.x; q[1] = a.y; q[2] = a.z; q[3] = a.w; q[4] = b.x; q[5] = b.y; q[6] = b.z; q[7] = b.w;
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    float o = (c == z) ? 1.f : 0.f;
+    if (c < z) {
+      const long long i = (long long)r * z + c;
+      const float ee = eps_in ? eps_in[i] : e[j];
+      eps_out[i] = ee;
+      p_out[i] = p_in ? p_in[i] : q[j];
+      o = mu[(long long)r * ldm + c] + ee;
+      zf[i] = o;
+    }
+    v[j] = o;
+  }
+  store_bf16x8(zb + (long long)r * ldz + c0, v, lo_off);
+  for (int pg = gz + g; pg < groups; pg += gz) {      // this thread's share of the row's zero padding
+    reinterpret_cast<uint4*>(zb)[(long long)r * groups + pg] = make_uint4(0, 0, 0, 0);
+    if (lo_off) reinterpret_cast<uint4*>(zb + lo_off)[(long long)r * groups + pg] = make_uint4(0, 0, 0, 0);
+  }
+}
+
+// the latent upstream of the BIR step: [dz_dec + dz_mmd | 0] -> bf16 [rows, ld] (no KL term, dmu = dz)
+__global__ void bir_dlatent_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ dzm,
+                                   __nv_bfloat16* __restrict__ out, int ld, int rows, int z, long long lo_off) {
+  griddep_sync();
+  const int groups = ld / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)rows * groups) return;
+  const int r = int(t / groups), c0 = int(t % groups) * 8;
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    v[j] = c < z ? dz[(long long)r * lddz + c] + dzm[(long long)r * z + c] : 0.f;
+  }
+  store_bf16x8(out + (long long)r * ld + c0, v, lo_off);
+}
+
+// Gaussian-kernel MMD (src/bir_vae.py:190-222), k(a, b) = exp(-|a - b|^2 / Z^2), over z [rows, Z] and p [rows, Z]:
+//   mmd = lambda (sum_ij k(p_i,p_j) + sum_ij k(z_i,z_j) - 2 sum_ij k(p_i,z_j))
+//   dz_i = lambda 4/Z^2 ((R_zp,i - R_zz,i) z_i + sum_j k(z_i,z_j) z_j - sum_j k(z_i,p_j) p_j),  R_x,i = sum_j k(z_i,x_j)
+// Flash-attention style: a CTA owns kMmdRows rows (blockIdx.y 0: rows of z against the columns of z, then of p;
+// 1: rows of p against the columns of p) and streams kMmdCols-column tiles through shared memory; nothing of size
+// rows x rows is stored.  kMmdLanes threads share a row, lane l taking columns l, l + 8, ...  Distances are formed from
+// fp32 differences (no |a|^2 + |b|^2 - 2ab cancellation) and exponentiated with expf.  Each tile's row sums and
+// sum_j k_ij x_j are fp32; the lanes combine them in a fixed butterfly and add them to fp64 accumulators, so identical
+// inputs give identical bits.  part[blockIdx.y * gridDim.x + blockIdx.x] = the CTA's share of mmd / lambda (fp64).
+constexpr int kMmdRows = 32, kMmdLanes = 8, kMmdCols = 128;
+
+template <int n, int N>
+__device__ __forceinline__ void mmd_halve(float (&v)[N], int off, bool upper) {
+  // one reduce-scatter step of the lane butterfly: keep one half of v[0, n), add the partner lane's copy of that half
+#pragma unroll
+  for (int i = 0; i < n / 2; ++i) {
+    const float send = upper ? v[i] : v[i + n / 2], keep = upper ? v[i + n / 2] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+  }
+}
+
+template <int ZT, bool GRAD>
+__global__ void __launch_bounds__(kMmdRows * kMmdLanes) mmd_tile_kernel(const float* __restrict__ z, const float* __restrict__ p,
+                                                                         int rows, int zd, float inv_z2, double gscale,
+                                                                         float* __restrict__ dz, double* __restrict__ part) {
+  static_assert(ZT % 8 == 0 && ZT <= 64, "ZT: a multiple of 8, at most 64");
+  constexpr int ZS = ZT + 4;                 // padded column stride: 8 lanes' 16-byte reads hit distinct banks
+  __shared__ __align__(16) float col_s[kMmdCols * ZS];
+  __shared__ double rs_s[kMmdRows];
+  griddep_sync();
+  const bool zrows = blockIdx.y == 0;
+  const int lane = threadIdx.x % kMmdLanes, rl = threadIdx.x / kMmdLanes;
+  const int r = blockIdx.x * kMmdRows + rl;
+  const bool valid = r < rows;
+  const float* src = zrows ? z : p;
+  float a[ZT];
+#pragma unroll
+  for (int d = 0; d < ZT; ++d) a[d] = (valid && d < zd) ? src[(long long)r * zd + d] : 0.f;
+  double s_same = 0.0, s_cross = 0.0;
+  double acc[GRAD ? ZT / kMmdLanes : 1];
+#pragma unroll
+  for (int q = 0; q < (GRAD ? ZT / kMmdLanes : 1); ++q) acc[q] = 0.0;
+  const int nsets = zrows ? 2 : 1;
+  for (int set = 0; set < nsets; ++set) {
+    const float* cols = (zrows && set == 0) ? z : p;
+    const bool same = set == 0;
+    for (int c0 = 0; c0 < rows; c0 += kMmdCols) {
+      __syncthreads();
+      for (int e = threadIdx.x; e < kMmdCols * ZT; e += kMmdRows * kMmdLanes) {
+        const int j = e / ZT, d = e % ZT;
+        col_s[j * ZS + d] = (c0 + j < rows && d < zd) ? cols[(long long)(c0 + j) * zd + d] : 0.f;
+      }
+      __syncthreads();
+      float rsum = 0.f;
+      float f[GRAD ? ZT : 1];
+#pragma unroll
+      for (int d = 0; d < (GRAD ? ZT : 1); ++d) f[d] = 0.f;
+      const int ncol = min(kMmdCols, rows - c0);
+#pragma unroll 2
+      for (int jj = lane; jj < ncol; jj += kMmdLanes) {
+        const float4* cv = reinterpret_cast<const float4*>(col_s + jj * ZS);
+        float d0 = 0.f, d1 = 0.f;              // two chains: even / odd 4-wide chunks
+#pragma unroll
+        for (int d = 0; d < ZT; d += 4) {
+          const float4 c = cv[d / 4];
+          const float x0 = a[d] - c.x, x1 = a[d + 1] - c.y, x2 = a[d + 2] - c.z, x3 = a[d + 3] - c.w;
+          float& s = (d / 4) % 2 ? d1 : d0;
+          s = fmaf(x0, x0, s); s = fmaf(x1, x1, s); s = fmaf(x2, x2, s); s = fmaf(x3, x3, s);
+        }
+        const float k = expf(-((d0 + d1) * inv_z2));
+        rsum += k;
+        if constexpr (GRAD) {
+#pragma unroll
+          for (int d = 0; d < ZT; d += 4) {
+            const float4 c = cv[d / 4];
+            f[d] = fmaf(k, c.x, f[d]); f[d + 1] = fmaf(k, c.y, f[d + 1]); f[d + 2] = fmaf(k, c.z, f[d + 2]); f[d + 3] = fmaf(k, c.w, f[d + 3]);
+          }
+        }
+      }
+      rsum += __shfl_xor_sync(0xffffffffu, rsum, 4);
+      rsum += __shfl_xor_sync(0xffffffffu, rsum, 2);
+      rsum += __shfl_xor_sync(0xffffffffu, rsum, 1);
+      if (same) s_same += rsum; else s_cross += rsum;
+      if constexpr (GRAD) {
+        if (zrows) {                          // block-uniform: the shuffles below see every lane
+          mmd_halve<ZT>(f, 4, lane & 4);
+          mmd_halve<ZT / 2>(f, 2, lane & 2);
+          mmd_halve<ZT / 4>(f, 1, lane & 1);
+          // lane l now holds dims [l ZT/8, (l + 1) ZT/8) of the tile's sum_j k_ij x_j
+#pragma unroll
+          for (int q = 0; q < ZT / kMmdLanes; ++q) acc[q] += same ? double(f[q]) : -double(f[q]);
+        }
+      }
+    }
+  }
+  if (lane == 0) rs_s[rl] = valid ? (zrows ? s_same - 2.0 * s_cross : s_same) : 0.0;
+  if constexpr (GRAD) {
+    if (zrows && valid) {
+#pragma unroll
+      for (int q = 0; q < ZT / kMmdLanes; ++q) {
+        const int d = lane * (ZT / kMmdLanes) + q;
+        if (d < zd) dz[(long long)r * zd + d] = float(gscale * ((s_cross - s_same) * double(z[(long long)r * zd + d]) + acc[q]));
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int i = 0; i < kMmdRows; ++i) t += rs_s[i];
+    part[blockIdx.y * gridDim.x + blockIdx.x] = t;
+  }
+}
+
+// mmd = lambda * (sum of the tile kernel's CTA partials, fixed order) -> out[0]
+__global__ void mmd_final_kernel(const double* __restrict__ part, int n, double lambda, float* __restrict__ out) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  double t = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) t += part[i];
+  t = block_sum<256>(t, sh);
+  if (threadIdx.x == 0) out[0] = float(lambda * t);
+}
+
 // ---------------------------------------------------------------- InfoGAN Q head (src/info_gan.py:290-302)
 // inf fp32 [rows, ldi]: [0,nd) categorical logits, [nd, nd+nc) continuous code.  noise fp32
 // [rows, ldn]: columns [zd, zd+nd) one-hot target, [zd+nd, zd+nd+nc) continuous target.

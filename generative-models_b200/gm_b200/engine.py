@@ -555,3 +555,82 @@ class VaeEngine:
         """device bytes one encoder slot and one decoder slot hold (allocated on the first per-call use)"""
         XP, HP, ZP, B = (self.image_size + 16) // 16 * 16, (self.hidden_dim + 16) // 16 * 16, (self.z_dim + 64) // 64 * 64, self.max_batch
         return 2 * B * (XP + HP) + 4 * B * 64, 2 * B * (ZP + HP + XP)
+
+
+class BirVaeEngine(VaeEngine):
+    """One MLP BIR-VAE (x -> hidden -> mu ; z = mu + eps ; z -> hidden -> x) on one GPU: the VAE engine in its BIR mode
+    (gm_bir_vae_create).  Flat layout [enc.linear.W, .b, enc.mu.W, .b, dec.linear.W, .b, dec.recon.W, .b].  eps_std is
+    the standard deviation of eps (the reference's set_var, src/bir_vae.py:82,91)."""
+    NAMES = ["encoder.linear.weight", "encoder.linear.bias", "encoder.mu.weight", "encoder.mu.bias",
+             "decoder.linear.weight", "decoder.linear.bias", "decoder.recon.weight", "decoder.recon.bias"]
+
+    def __init__(self, image_size=784, hidden_dim=400, z_dim=20, eps_std=1.0, max_batch=64, device=None, precision="bf16"):
+        if not torch.cuda.is_available():
+            raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
+        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.h = _lib.ctx(self.device.index)
+        self.image_size, self.hidden_dim, self.z_dim, self.max_batch = image_size, hidden_dim, z_dim, max_batch
+        self.precision, self.eps_std = precision, float(eps_std)
+        d = VaeDesc(image_size, hidden_dim, z_dim, max_batch, PRECISIONS[precision])
+        self.g = C.c_void_p()
+        check(self.h, lib().gm_bir_vae_create(self.h, C.byref(d), self.eps_std, C.byref(self.g)))
+        n = lib().gm_vae_param_count(self.g)
+        kw = dict(device=self.device, dtype=torch.float32)
+        self.params, self.grads = torch.zeros(n, **kw), torch.zeros(n, **kw)
+        self.exp_avg, self.exp_avg_sq = torch.zeros(n, **kw), torch.zeros(n, **kw)
+        self.loss_buf = torch.zeros(2, **kw)
+        check(self.h, lib().gm_vae_bind(self.g, _ptr(self.params), _ptr(self.grads), _ptr(self.exp_avg), _ptr(self.exp_avg_sq)))
+        X, H, Z = image_size, hidden_dim, z_dim
+        self.shapes = [(H, X), (H,), (Z, H), (Z,), (H, Z), (H,), (X, H), (X,)]
+        self.steps = 0
+
+    def grad(self, images, eps=None, prior=None, lam=1000.0, fmt="f32", gather_idx=None, batch=None, seed=0, step=0):
+        """compute_batch + backward (src/bir_vae.py:148-188). Returns the device tensor [mse, mmd]."""
+        B = batch if batch is not None else (gather_idx.numel() if gather_idx is not None else images.shape[0])
+        check(self.h, lib().gm_bir_vae_grad(self.g, _ptr(images), IMG_FMTS[fmt], _ptr(gather_idx), B, _ptr(eps), _ptr(prior),
+                                            float(lam), seed, step, _ptr(self.loss_buf), _stream()))
+        return self.loss_buf
+
+    def forward(self, images, eps=None, prior=None, lam=1000.0, fmt="f32", want_images=True, want_latent=True,
+                want_losses=False, seed=0, step=0):
+        """-> (images or None, mu or None, losses [mse, mmd] or None)"""
+        n = images.shape[0]
+        kw = dict(device=self.device, dtype=torch.float32)
+        out = torch.empty(n, self.image_size, **kw) if want_images else None
+        mu = torch.empty(n, self.z_dim, **kw) if want_latent else None
+        ls = torch.empty(2, **kw) if want_losses else None
+        check(self.h, lib().gm_bir_vae_forward(self.g, _ptr(images.contiguous()), IMG_FMTS[fmt], n, _ptr(eps), _ptr(prior),
+                                               float(lam), seed, step, _ptr(out), _ptr(mu), _ptr(ls), _stream()))
+        return out, mu, ls
+
+    def last_latent(self, batch):
+        """(z, p) [batch, z] fp32 of the last grad() / forward()"""
+        z = torch.empty(batch, self.z_dim, device=self.device, dtype=torch.float32)
+        p = torch.empty_like(z)
+        check(self.h, lib().gm_bir_vae_last_latent(self.g, _ptr(z), _ptr(p), batch, _stream()))
+        return z, p
+
+    def encoder_forward(self, slot, x):
+        """Encoder.forward on slot's buffers: x [n, image_size] fp32 -> mu [n, z] fp32"""
+        n = x.shape[0]
+        mu = torch.empty(n, self.z_dim, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_vae_encoder_forward(self.g, slot, _ptr(x.contiguous()), n, _ptr(mu), _stream()))
+        return mu
+
+    def encoder_backward(self, slot, n, dmu):
+        """-> {encoder parameter name: gradient} of encoder_forward's call on slot"""
+        grads = torch.empty_like(self.params)
+        check(self.h, lib().gm_vae_encoder_backward(self.g, slot, n, _ptr(dmu.float().contiguous()), _ptr(grads), _stream()))
+        return {k: v for k, v in self.views(grads).items() if k.startswith("encoder.")}
+
+
+def mmd_gaussian(z, p, lam=1.0, want_grad=True):
+    """gm_mmd_gaussian on fp32 CUDA tensors z, p [B, Z]: -> (mmd [1] device tensor, dmmd/dz [B, Z] or None)"""
+    if z.shape != p.shape or z.dim() != 2:
+        raise GmError("mmd_gaussian: z and p must both be [batch, z_dim] (got %s, %s)" % (tuple(z.shape), tuple(p.shape)))
+    z, p = z.float().contiguous(), p.float().contiguous()
+    out = torch.empty(1, device=z.device, dtype=torch.float32)
+    dz = torch.empty_like(z) if want_grad else None
+    h = _lib.ctx(z.device.index)
+    check(h, lib().gm_mmd_gaussian(h, _ptr(z), _ptr(p), z.shape[0], z.shape[1], float(lam), _ptr(out), _ptr(dz), _stream()))
+    return out, dz

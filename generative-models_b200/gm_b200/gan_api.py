@@ -385,13 +385,19 @@ def refuse_multi_rank(what="compute_batch"):
         raise GmError("an overridden %s trains on one process; data-parallel training runs the built-in step" % what)
 
 
-def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=None):
+VAE_EPOCH_LINE = "Epoch[%d/%d], Total Loss: %.4f, Reconst Loss: %.4f, KL Div: %.7f, Val Loss: %.4f"
+
+
+def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=None, second="kl_loss",
+                       epoch_line=VAE_EPOCH_LINE):
     """The reference's train loop verbatim (src/vae.py:127-191 when compute_batch returns (recon, kl), src/ae.py:84-145 when
     it returns one loss) for a VAE-family trainer tr whose compute_batch was overridden: the override's torch loss drives the
     CUDA forward / backward kernels through the model's encoder / decoder autograd nodes, FusedAdam (coupled weight decay,
     as torch.optim.Adam) steps the module parameters, validation runs tr.evaluate (which calls the override) in eval mode.
     train_iter is read on the host.  after_step(), when given, runs after every optimizer step.  best_model is
-    deepcopy(tr.model), a detached copy with its own inference engine."""
+    deepcopy(tr.model), a detached copy with its own inference engine.  With two losses, the second one's per-step values
+    go to the list tr.<second> and epoch_line formats (epoch, epochs, total, first, second, validation) - the BIR-VAE
+    passes its own (src/bir_vae.py:164-174)."""
     optimizer = FusedAdam([p for p in tr.model.parameters() if p.requires_grad], lr=lr, weight_decay=weight_decay)
     for epoch in range(1, num_epochs + 1):
         tr.model.train()
@@ -412,7 +418,7 @@ def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=
                 epoch_recon.append(recon_loss.item())
                 epoch_kl.append(kl_diverge.item())
         if two_losses:
-            tr.kl_loss.extend(epoch_kl)
+            getattr(tr, second).extend(epoch_kl)
             tr.recon_loss.extend(epoch_recon)
         else:
             tr.recon_loss.extend(epoch_loss)
@@ -422,8 +428,7 @@ def compute_batch_loop(tr, num_epochs, lr, weight_decay, two_losses, after_step=
             tr.best_model = deepcopy(tr.model)
             tr.best_val_loss = val_loss
         if two_losses:
-            print("Epoch[%d/%d], Total Loss: %.4f, Reconst Loss: %.4f, KL Div: %.7f, Val Loss: %.4f"
-                  % (epoch, num_epochs, np.mean(epoch_loss), np.mean(epoch_recon), np.mean(epoch_kl), val_loss))
+            print(epoch_line % (epoch, num_epochs, np.mean(epoch_loss), np.mean(epoch_recon), np.mean(epoch_kl), val_loss))
         else:
             print("Epoch[%d/%d], Train Loss: %.4f, Val Loss: %.4f" % (epoch, num_epochs, np.mean(epoch_loss), val_loss))
         tr.num_epochs += 1

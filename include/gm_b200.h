@@ -355,6 +355,38 @@ int gm_vae_decoder_backward(gm_vae* vae, int slot, int batch, const float* dimag
  * Refuses, with nothing launched: rows or x not positive, ld below x or not a multiple of 8, dout not 4-byte or
  * out_rows not 16-byte aligned; GM_ERR_UNSUPPORTED for 2^31 threads or more. */
 int gm_sigmoid_upstream_rows(gm_ctx* ctx, const float* dout_dev, void* out_rows_dev, int rows, int x, int ld, gm_stream stream);
+/* ---- BIR-VAE (src/bir_vae.py): a BIR mode of the VAE engine ---------------------------------
+ * Encoder x -> hidden -> mu (no log_var head), z = mu + eps with eps of standard deviation eps_std (the reference's
+ * set_var = 4^(-I / z_dim), which np.random.normal takes as a standard deviation), the VAE's Decoder.  Flat fp32 layout:
+ * [enc.linear.W | .b | enc.mu.W | enc.mu.b | dec.linear.W | .b | dec.recon.W | .b].  The engine is a gm_vae: bind,
+ * sync_shadows, apply, set_sampler, set_lazy_grads, materialize_grads, last_eps, debug_read (6: [dmu | 0]), decode and
+ * the per-call entries serve it unchanged (the encoder's output and upstream are mu / dmu [batch, z]);
+ * gm_vae_grad / gm_vae_forward refuse it, and the gm_bir_vae_* entries refuse a VAE engine, with GM_ERR_ARG.
+ * gm_bir_vae_create accepts 1 <= z_dim <= 32 and hidden_dim <= 447, and refuses GM_PREC_SPLIT with GM_ERR_UNSUPPORTED. */
+int gm_bir_vae_create(gm_ctx* ctx, const gm_vae_desc* desc, float eps_std, gm_vae** out);
+/* compute_batch + (mse_loss + mmd_loss).backward() (src/bir_vae.py:148-188): mse = sum (x - out)^2,
+ * mmd = lambda * gm_mmd_gaussian(z, p); writes the flat gradient and losses_dev[0..1] = {mse, mmd}.  eps_dev [batch, z]
+ * (already at the eps_std scale) and prior_dev [batch, z] fp32, each NULL for on-device Philox draws (eps_std * N(0,1)
+ * and N(0,1), on streams of their own). */
+int gm_bir_vae_grad(gm_vae* vae, const void* images_dev, int img_fmt, const int* gather_idx_dev, int batch,
+                    const float* eps_dev, const float* prior_dev, float lambda, uint64_t seed, uint64_t step,
+                    float* losses_dev, gm_stream stream);
+/* BIRVAE.forward (+ the losses of compute_batch) without gradients: evaluate / reconstruct.  Any of out_images_dev
+ * [n, image_size], mu_dev [n, z], losses_dev [2] = {mse, mmd} may be NULL. */
+int gm_bir_vae_forward(gm_vae* vae, const void* images_dev, int img_fmt, int n, const float* eps_dev, const float* prior_dev,
+                       float lambda, uint64_t seed, uint64_t step, float* out_images_dev, float* mu_dev, float* losses_dev,
+                       gm_stream stream);
+/* z = mu + eps and the prior sample p of the last gm_bir_vae_grad / gm_bir_vae_forward -> [batch, z] fp32 each (nullable). */
+int gm_bir_vae_last_latent(gm_vae* vae, float* z_dev, float* p_dev, int batch, gm_stream stream);
+/* Gaussian-kernel maximum mean discrepancy (src/bir_vae.py:190-222), k(a, b) = exp(-|a - b|^2 / z_dim^2), of
+ * z_dev [batch, z_dim] against p_dev [batch, z_dim] fp32:
+ *   mmd_dev[0] = lambda (sum_ij k(p_i,p_j) + sum_ij k(z_i,z_j) - 2 sum_ij k(p_i,z_j))
+ *   dz_dev (nullable) [batch, z_dim] = d mmd / dz = lambda 4/z_dim^2 (-sum_j k(z_i,z_j)(z_i - z_j) + sum_j k(z_i,p_j)(z_i - p_j)).
+ * Tiled through shared memory (nothing of size batch x batch is stored), fp32 terms, fp64 sums across tiles, fixed
+ * reduction order: identical inputs give identical bits.  Refuses null or misaligned pointers and batch <= 0 with
+ * GM_ERR_ARG, z_dim outside [1, 64] or batch * z_dim >= 2^31 with GM_ERR_UNSUPPORTED, before anything is launched. */
+int gm_mmd_gaussian(gm_ctx* ctx, const float* z_dev, const float* p_dev, int batch, int z_dim, float lambda, float* mmd_dev,
+                    float* dz_dev, gm_stream stream);
 
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
