@@ -191,6 +191,12 @@ def lib():
     L.gm_bir_vae_forward.argtypes = [vp, vp, i, i, vp, vp, f, u64, u64, vp, vp, vp, vp]
     L.gm_bir_vae_last_latent.argtypes = [vp, vp, vp, i, vp]
     L.gm_mmd_gaussian.argtypes = [vp, vp, vp, i, i, f, vp, vp, vp]
+    L.gm_cvae_create.argtypes = [vp, C.POINTER(VaeDesc), i, C.POINTER(vp)]
+    L.gm_cvae_grad.argtypes = [vp, vp, i, vp, vp, i, vp, u64, u64, vp, vp]
+    L.gm_cvae_forward.argtypes = [vp, vp, i, vp, i, vp, u64, u64, vp, vp, vp, vp]
+    L.gm_cvae_decode.argtypes = [vp, vp, vp, i, vp, vp]
+    L.gm_cvae_encoder_forward.argtypes = [vp, i, vp, vp, i, vp, vp]
+    L.gm_cvae_decoder_forward.argtypes = [vp, i, vp, vp, i, vp, vp]
     _lib = L
     return L
 

@@ -870,6 +870,117 @@ __global__ void bir_dlatent_kernel(const float* __restrict__ dz, int lddz, const
   store_bf16x8(out + (long long)r * ld + c0, v, lo_off);
 }
 
+// ---------------------------------------------------------------- conditional VAE
+// The conditional rows [v | onehot(y) | 1 | 0] of the CVAE's encoder input (v = x) and decoder input (v = z): column
+// w + k is 1 for k == y (k < ncls), column w + ncls is the ones column of the bias-gradient trick, the rest is zero.
+// A label outside [0, ncls) gives a zero one-hot: no column is ever addressed by a label.
+__device__ __forceinline__ float cvae_cond_col(int k, int y, int ncls) {
+  return k < ncls ? (k == y ? 1.f : 0.f) : (k == ncls ? 1.f : 0.f);
+}
+
+// images (fp32 | 1-bit packed) [*, x] and int labels [*] -> bf16 encoder rows [rows, ld] = [x | onehot(y) | 1 | 0].
+// Row r reads source row idx[r], else the epoch sampler's draw, else r, for the image and its label alike; the label
+// is also stored to lab_out[r] (nullable) for the latent kernel.  One warp per row, lane l writing the 16-byte groups
+// l, l + 32, ...; x % 8 == 0, so a group holds pixels only or label / pad columns only.
+__global__ void cvae_stage_kernel(const void* __restrict__ src, int fmt, const int* __restrict__ idx, const int* __restrict__ labels,
+                                  int* __restrict__ lab_out, __nv_bfloat16* __restrict__ dst, int rows, int x, int ncls, int ld,
+                                  const Sampler smp) {
+  griddep_sync();
+  const int groups = ld / 8, xg = x >> 3;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  for (int r = w; r < rows; r += nwarps) {
+    const long long sr = idx ? (long long)idx[r] : smp.n ? (long long)sampler_index(smp, smp.offset + (unsigned long long)r) : (long long)r;
+    const int y = __ldg(labels + sr);
+    if (lane == 0 && lab_out) lab_out[r] = y;
+    for (int g = lane; g < groups; g += 32) {
+      float v[8];
+      if (g < xg) {
+        if (fmt == IMG_BITS) {
+          const uint32_t b = __ldg(reinterpret_cast<const uint8_t*>(src) + sr * xg + g);   // np.packbits order: MSB first
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = (b >> (7 - j)) & 1u ? 1.f : 0.f;
+        } else {
+          const float* s = reinterpret_cast<const float*>(src) + sr * x + g * 8;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = __ldg(s + j);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = cvae_cond_col(g * 8 + j - x, y, ncls);
+      }
+      store_bf16x8(dst + ((long long)r * groups + g) * 8, v, 0);
+    }
+  }
+}
+
+// vae_reparam_kernel on the conditional latent row: z = mu + eps*exp(lv/2) -> bf16 [rows, ldz] = [z | onehot(lab[r]) | 1 | 0].
+// The thread <-> (row, group) mapping, the Philox cells and the KL partials are vae_reparam_kernel's, so the same mu,
+// log_var and seed give the same eps, z and kl bits as the VAE; only the columns from z on carry the label.
+__global__ void cvae_reparam_kernel(const float* __restrict__ mulv, int ldm, const float* __restrict__ eps_in,
+                                    float* __restrict__ eps_out, const int* __restrict__ lab, __nv_bfloat16* __restrict__ zb,
+                                    int ldz, int rows, int z, int ncls, unsigned long long seed, unsigned long long stream_id,
+                                    double* __restrict__ part) {
+  griddep_sync();
+  __shared__ double sh[256 / 32];
+  const int groups = ldz / 8, gz = (z + 8) / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  double kl = 0.0;
+  if (t < (long long)rows * gz) {
+    const int r = int(t / gz), g = int(t % gz), c0 = g * 8;
+    const int y = lab[r];
+    float v[8], e[8];
+    if (eps_in == nullptr && c0 < z) {
+      curandStatePhilox4_32_10_t st;
+      curand_init(seed ^ 0x5851F42D4C957F2Dull, (unsigned long long)r * groups + g, stream_id * 64ull, &st);
+      const float4 a = curand_normal4(&st), b = curand_normal4(&st);
+      e[0] = a.x; e[1] = a.y; e[2] = a.z; e[3] = a.w; e[4] = b.x; e[5] = b.y; e[6] = b.z; e[7] = b.w;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = c0 + j;
+      float o;
+      if (c < z) {
+        const float mu = mulv[(long long)r * ldm + c], lv = mulv[(long long)r * ldm + z + c];
+        const float ee = eps_in ? eps_in[(long long)r * z + c] : e[j];
+        eps_out[(long long)r * z + c] = ee;
+        o = mu + ee * expf(0.5f * lv);
+        kl += 0.5 * ((double)mu * mu + exp((double)lv) - lv - 1.0);
+      } else {
+        o = cvae_cond_col(c - z, y, ncls);
+      }
+      v[j] = o;
+    }
+    store_bf16x8(zb + (long long)r * ldz + c0, v, 0);
+    for (int pg = gz + g; pg < groups; pg += gz) {      // this thread's share of the row's label and padding groups
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = cvae_cond_col(pg * 8 + j - z, y, ncls);
+      store_bf16x8(zb + (long long)r * ldz + pg * 8, v, 0);
+    }
+  }
+  kl = block_sum<256>(kl, sh);
+  if (threadIdx.x == 0 && part) part[blockIdx.x] = kl;
+}
+
+// caller latents z fp32 [rows, z] and int labels [rows] -> bf16 [rows, ld] = [z | onehot(y) | 1 | 0] (decode, the
+// per-call decoder).  One thread per (row, 16-byte group).
+__global__ void cvae_latent_rows_kernel(const float* __restrict__ zin, const int* __restrict__ labels, __nv_bfloat16* __restrict__ zb,
+                                        int ld, int rows, int z, int ncls) {
+  griddep_sync();
+  const int groups = ld / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)rows * groups) return;
+  const int r = int(t / groups), c0 = int(t % groups) * 8;
+  const int y = labels[r];
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    v[j] = c < z ? zin[(long long)r * z + c] : cvae_cond_col(c - z, y, ncls);
+  }
+  store_bf16x8(zb + (long long)r * ld + c0, v, 0);
+}
+
 // Gaussian-kernel MMD (src/bir_vae.py:190-222), k(a, b) = exp(-|a - b|^2 / Z^2), over z [rows, Z] and p [rows, Z]:
 //   mmd = lambda (sum_ij k(p_i,p_j) + sum_ij k(z_i,z_j) - 2 sum_ij k(p_i,z_j))
 //   dz_i = lambda 4/Z^2 ((R_zp,i - R_zz,i) z_i + sum_j k(z_i,z_j) z_j - sum_j k(z_i,p_j) p_j),  R_x,i = sum_j k(z_i,x_j)

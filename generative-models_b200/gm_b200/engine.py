@@ -397,6 +397,13 @@ class VaeEngine:
              "decoder.recon.weight", "decoder.recon.bias"]
 
     def __init__(self, image_size=784, hidden_dim=400, z_dim=20, max_batch=64, device=None, precision="bf16"):
+        X, H, Z = image_size, hidden_dim, z_dim
+        self._open(image_size, hidden_dim, z_dim, max_batch, device, precision, lambda h, d, out: lib().gm_vae_create(h, d, out),
+                   [(H, X), (H,), (Z, H), (Z, H), (Z,), (Z,), (H, Z), (H,), (X, H), (X,)])
+
+    def _open(self, image_size, hidden_dim, z_dim, max_batch, device, precision, create, shapes):
+        """create(ctx, desc, out) one engine of the gm_vae family, bind its flat fp32 buffers; shapes: the tensors of the
+        flat layout in NAMES order"""
         if not torch.cuda.is_available():
             raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -405,15 +412,14 @@ class VaeEngine:
         self.precision = precision
         d = VaeDesc(image_size, hidden_dim, z_dim, max_batch, PRECISIONS[precision])
         self.g = C.c_void_p()
-        check(self.h, lib().gm_vae_create(self.h, C.byref(d), C.byref(self.g)))
+        check(self.h, create(self.h, C.byref(d), C.byref(self.g)))
         n = lib().gm_vae_param_count(self.g)
         kw = dict(device=self.device, dtype=torch.float32)
         self.params, self.grads = torch.zeros(n, **kw), torch.zeros(n, **kw)
         self.exp_avg, self.exp_avg_sq = torch.zeros(n, **kw), torch.zeros(n, **kw)
         self.loss_buf = torch.zeros(2, **kw)
         check(self.h, lib().gm_vae_bind(self.g, _ptr(self.params), _ptr(self.grads), _ptr(self.exp_avg), _ptr(self.exp_avg_sq)))
-        X, H, Z = image_size, hidden_dim, z_dim
-        self.shapes = [(H, X), (H,), (Z, H), (Z, H), (Z,), (Z,), (H, Z), (H,), (X, H), (X,)]
+        self.shapes = shapes
         self.steps = 0
 
     def __del__(self):
@@ -565,24 +571,11 @@ class BirVaeEngine(VaeEngine):
              "decoder.linear.weight", "decoder.linear.bias", "decoder.recon.weight", "decoder.recon.bias"]
 
     def __init__(self, image_size=784, hidden_dim=400, z_dim=20, eps_std=1.0, max_batch=64, device=None, precision="bf16"):
-        if not torch.cuda.is_available():
-            raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
-        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
-        self.h = _lib.ctx(self.device.index)
-        self.image_size, self.hidden_dim, self.z_dim, self.max_batch = image_size, hidden_dim, z_dim, max_batch
-        self.precision, self.eps_std = precision, float(eps_std)
-        d = VaeDesc(image_size, hidden_dim, z_dim, max_batch, PRECISIONS[precision])
-        self.g = C.c_void_p()
-        check(self.h, lib().gm_bir_vae_create(self.h, C.byref(d), self.eps_std, C.byref(self.g)))
-        n = lib().gm_vae_param_count(self.g)
-        kw = dict(device=self.device, dtype=torch.float32)
-        self.params, self.grads = torch.zeros(n, **kw), torch.zeros(n, **kw)
-        self.exp_avg, self.exp_avg_sq = torch.zeros(n, **kw), torch.zeros(n, **kw)
-        self.loss_buf = torch.zeros(2, **kw)
-        check(self.h, lib().gm_vae_bind(self.g, _ptr(self.params), _ptr(self.grads), _ptr(self.exp_avg), _ptr(self.exp_avg_sq)))
+        self.eps_std = float(eps_std)
         X, H, Z = image_size, hidden_dim, z_dim
-        self.shapes = [(H, X), (H,), (Z, H), (Z,), (H, Z), (H,), (X, H), (X,)]
-        self.steps = 0
+        self._open(image_size, hidden_dim, z_dim, max_batch, device, precision,
+                   lambda h, d, out: lib().gm_bir_vae_create(h, d, self.eps_std, out),
+                   [(H, X), (H,), (Z, H), (Z,), (H, Z), (H,), (X, H), (X,)])
 
     def grad(self, images, eps=None, prior=None, lam=1000.0, fmt="f32", gather_idx=None, batch=None, seed=0, step=0):
         """compute_batch + backward (src/bir_vae.py:148-188). Returns the device tensor [mse, mmd]."""
@@ -622,6 +615,127 @@ class BirVaeEngine(VaeEngine):
         grads = torch.empty_like(self.params)
         check(self.h, lib().gm_vae_encoder_backward(self.g, slot, n, _ptr(dmu.float().contiguous()), _ptr(grads), _stream()))
         return {k: v for k, v in self.views(grads).items() if k.startswith("encoder.")}
+
+
+class ClassIds:
+    """Class labels checked against an engine's num_classes and held as an int32 tensor on its device (CvaeEngine.class_ids)"""
+    __slots__ = ("t", "num_classes")
+
+    def __init__(self, t, num_classes):
+        self.t, self.num_classes = t, num_classes
+
+    def __len__(self):
+        return self.t.numel()
+
+
+def class_ids(labels, num_classes, device, n=None):
+    """labels (class ids in [0, num_classes): an integer tensor, array or sequence of shape [m] or [m, 1], with m == n when
+    n is given) -> ClassIds on device.  Anything else - a one-hot matrix included - raises GmError here, on the host,
+    before the labels are uploaded or a kernel runs."""
+    import numpy as np
+    def count(m):
+        if n is not None and m != n:
+            raise GmError("%d labels for %d rows" % (m, n))
+    if isinstance(labels, ClassIds):
+        if labels.num_classes != num_classes or labels.t.device != device:
+            raise GmError("labels were checked for %d classes on %s, not %d on %s"
+                          % (labels.num_classes, labels.t.device, num_classes, device))
+        count(len(labels))
+        return labels
+    t = labels if torch.is_tensor(labels) else torch.as_tensor(np.asarray(labels))
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise GmError("labels must be integer class ids (got dtype %s)" % t.dtype)
+    if not (t.dim() == 1 or (t.dim() == 2 and t.shape[1] == 1)):
+        raise GmError("labels must be class ids of shape [n] or [n, 1], not one-hot or other rows (got shape %s)"
+                      % (tuple(t.shape),))
+    t = t.reshape(-1)
+    count(t.numel())
+    if t.numel() == 0:
+        raise GmError("labels are empty")
+    if t.numel() >= 2 ** 31:
+        raise GmError("more than 2^31 labels")
+    lo, hi = int(t.min()), int(t.max())
+    if lo < 0 or hi >= num_classes:
+        raise GmError("labels must be in [0, %d) (got values in [%d, %d])" % (num_classes, lo, hi))
+    return ClassIds(t.to(device=device, dtype=torch.int32).contiguous(), num_classes)
+
+
+class CvaeEngine(VaeEngine):
+    """One MLP conditional VAE (x, y -> hidden -> (mu, log_var) ; z, y -> hidden -> x) on one GPU: the VAE engine in its
+    CVAE mode (gm_cvae_create).  The flat layout is the VAE's, with encoder.linear.weight (H, X + C) and
+    decoder.linear.weight (H, Z + C): the one-hot columns follow the x (z) columns.  Every entry that takes labels takes
+    integer class ids or a ClassIds from class_ids()."""
+
+    def __init__(self, image_size=784, hidden_dim=400, z_dim=20, num_classes=10, max_batch=64, device=None, precision="bf16"):
+        if precision != "bf16":
+            raise GmError("the CVAE engine runs in bf16 only (got precision=%r)" % (precision,))
+        self.num_classes = int(num_classes)
+        X, H, Z, K = image_size, hidden_dim, z_dim, self.num_classes
+        self._open(image_size, hidden_dim, z_dim, max_batch, device, precision,
+                   lambda h, d, out: lib().gm_cvae_create(h, d, self.num_classes, out),
+                   [(H, X + K), (H,), (Z, H), (Z, H), (Z,), (Z,), (H, Z + K), (H,), (X, H), (X,)])
+
+    def class_ids(self, labels, n=None):
+        """labels checked for this engine (exactly n of them when n is given) -> ClassIds on its device"""
+        return class_ids(labels, self.num_classes, self.device, n)
+
+    def set_sampler(self, n_pool, batches_per_epoch, seed=0, batch_size=0):
+        super().set_sampler(n_pool, batches_per_epoch, seed, batch_size)
+        self._pool_n = int(n_pool)
+
+    def grad(self, images, labels, eps=None, fmt="f32", gather_idx=None, batch=None, seed=0, step=0):
+        """compute_batch + backward on (images, labels). Returns the device tensor [recon, kl].  With gather_idx or the
+        epoch sampler, labels is the pool's label array, read at each gathered row."""
+        B = batch if batch is not None else (gather_idx.numel() if gather_idx is not None else images.shape[0])
+        pool = getattr(self, "_pool_n", 0)
+        # one label per image the kernels may read: the whole image pool with gather_idx or the sampler, else the batch
+        y = self.class_ids(labels, images.shape[0] if gather_idx is not None else pool if pool > 0 else B)
+        check(self.h, lib().gm_cvae_grad(self.g, _ptr(images), IMG_FMTS[fmt], _ptr(y.t), _ptr(gather_idx), B, _ptr(eps), seed, step,
+                                         _ptr(self.loss_buf), _stream()))
+        return self.loss_buf
+
+    def forward(self, images, labels, eps=None, fmt="f32", want_images=True, want_latent=True, want_losses=False, seed=0, step=0):
+        n = images.shape[0]
+        y = self.class_ids(labels, n)
+        kw = dict(device=self.device, dtype=torch.float32)
+        out = torch.empty(n, self.image_size, **kw) if want_images else None
+        ml = torch.empty(n, 2 * self.z_dim, **kw) if want_latent else None
+        ls = torch.empty(2, **kw) if want_losses else None
+        check(self.h, lib().gm_cvae_forward(self.g, _ptr(images.contiguous()), IMG_FMTS[fmt], _ptr(y.t), n, _ptr(eps), seed, step,
+                                            _ptr(out), _ptr(ml), _ptr(ls), _stream()))
+        mu = ml[:, :self.z_dim] if ml is not None else None
+        lv = ml[:, self.z_dim:] if ml is not None else None
+        return out, mu, lv, ls
+
+    def decode(self, z, labels):
+        n = z.shape[0]
+        y = self.class_ids(labels, n)
+        out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_cvae_decode(self.g, _ptr(z.contiguous().float()), _ptr(y.t), n, _ptr(out), _stream()))
+        return out
+
+    def encoder_forward(self, slot, x, labels):
+        """Encoder.forward on slot's buffers: x [n, image_size] fp32, labels [n] -> (mu, log_var) [n, z] fp32"""
+        n = x.shape[0]
+        y = self.class_ids(labels, n)
+        ml = torch.empty(n, 2 * self.z_dim, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_cvae_encoder_forward(self.g, slot, _ptr(x.contiguous()), _ptr(y.t), n, _ptr(ml), _stream()))
+        return ml[:, :self.z_dim], ml[:, self.z_dim:]
+
+    def decoder_forward(self, slot, z, labels):
+        """Decoder.forward on slot's buffers: z [n, z] fp32, labels [n] -> images [n, image_size] fp32"""
+        n = z.shape[0]
+        y = self.class_ids(labels, n)
+        out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_cvae_decoder_forward(self.g, slot, _ptr(z.contiguous()), _ptr(y.t), n, _ptr(out), _stream()))
+        return out
+
+    def slot_bytes(self):
+        """device bytes one encoder slot and one decoder slot hold (allocated on the first per-call use)"""
+        K = self.num_classes
+        XP, HP, B = (self.image_size + K + 16) // 16 * 16, (self.hidden_dim + 16) // 16 * 16, self.max_batch
+        ZP = (self.z_dim + K + 64) // 64 * 64
+        return 2 * B * (XP + HP) + 4 * B * 64, 2 * B * (ZP + HP + XP)
 
 
 def mmd_gaussian(z, p, lam=1.0, want_grad=True):

@@ -387,6 +387,37 @@ int gm_bir_vae_last_latent(gm_vae* vae, float* z_dev, float* p_dev, int batch, g
  * GM_ERR_ARG, z_dim outside [1, 64] or batch * z_dim >= 2^31 with GM_ERR_UNSUPPORTED, before anything is launched. */
 int gm_mmd_gaussian(gm_ctx* ctx, const float* z_dev, const float* p_dev, int batch, int z_dim, float lambda, float* mmd_dev,
                     float* dz_dev, gm_stream stream);
+/* ---- conditional VAE (cvae.py): a CVAE mode of the VAE engine -------------------------------
+ * Encoder q(z | x, y) on [x | onehot(y)], Decoder p(x | z, y) on [z | onehot(y)], the VAE's heads, losses and Adam.  The
+ * flat fp32 layout is gm_vae's with enc.linear.W (hidden, x + C) and dec.linear.W (hidden, z + C), the one-hot columns
+ * after the x (z) columns.  Labels are int32 class ids; a label outside [0, C) is given a zero one-hot (callers are
+ * expected to refuse it first).  The engine is a gm_vae: bind, sync_shadows, apply, set_sampler, set_lazy_grads,
+ * materialize_grads, last_eps, debug_read, gm_vae_encoder_backward and gm_vae_decoder_backward serve it unchanged (their
+ * gradients include the label columns; dz stays [batch, z]).  gm_vae_grad, gm_vae_forward, gm_vae_decode and the
+ * gm_vae_{encoder,decoder}_forward entries refuse it, and the gm_cvae_* entries refuse any other engine, with GM_ERR_ARG.
+ * gm_cvae_create accepts num_classes >= 1 with z_dim + num_classes <= 63 and hidden_dim <= 447, z_dim <= 32 as
+ * gm_vae_create does; unlike gm_vae_create it also accepts an odd z_dim (the decoder biases are then read from an aligned
+ * copy).  It refuses GM_PREC_SPLIT with GM_ERR_UNSUPPORTED.  Every gm_cvae_* entry refuses a
+ * null input or labels pointer, misalignment, and a batch outside (0, max_batch] with GM_ERR_ARG, and an image format
+ * other than GM_IMG_F32 / GM_IMG_BITS with GM_ERR_UNSUPPORTED, before anything is launched. */
+int gm_cvae_create(gm_ctx* ctx, const gm_vae_desc* desc, int num_classes, gm_vae** out);
+/* compute_batch + (recon + kl).backward() on the conditional rows: losses_dev[0..1] = {recon, kl}.  labels_dev follows the
+ * images' indexing: with gather_idx_dev, or with the epoch sampler (gm_vae_set_sampler), it is the pool's label array
+ * and row r reads the label of the image it gathers.  eps_dev [batch, z] fp32 or NULL for on-device Philox (the same
+ * draws gm_vae_grad makes for the same seed and step). */
+int gm_cvae_grad(gm_vae* vae, const void* images_dev, int img_fmt, const int* labels_dev, const int* gather_idx_dev, int batch,
+                 const float* eps_dev, uint64_t seed, uint64_t step, float* losses_dev, gm_stream stream);
+/* CVAE.forward (+ losses) without gradients; any of out_images_dev [n, image_size], mu_logvar_dev [n, 2 z] and
+ * losses_dev [2] may be NULL. */
+int gm_cvae_forward(gm_vae* vae, const void* images_dev, int img_fmt, const int* labels_dev, int n, const float* eps_dev,
+                    uint64_t seed, uint64_t step, float* out_images_dev, float* mu_logvar_dev, float* losses_dev, gm_stream stream);
+/* Decoder.forward for sampling: z_dev [n, z] fp32, labels_dev [n] -> out_images_dev [n, image_size] fp32. */
+int gm_cvae_decode(gm_vae* vae, const float* z_dev, const int* labels_dev, int n, float* out_images_dev, gm_stream stream);
+/* the per-call encoder / decoder forward halves with their labels (slots as gm_vae_encoder_forward / _decoder_forward) */
+int gm_cvae_encoder_forward(gm_vae* vae, int slot, const float* x_dev, const int* labels_dev, int batch, float* mu_logvar_dev,
+                            gm_stream stream);
+int gm_cvae_decoder_forward(gm_vae* vae, int slot, const float* z_dev, const int* labels_dev, int batch, float* images_dev,
+                            gm_stream stream);
 
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
