@@ -197,6 +197,20 @@ def lib():
     L.gm_cvae_decode.argtypes = [vp, vp, vp, i, vp, vp]
     L.gm_cvae_encoder_forward.argtypes = [vp, i, vp, vp, i, vp, vp]
     L.gm_cvae_decoder_forward.argtypes = [vp, i, vp, vp, i, vp, vp]
+    L.gm_aae_create.argtypes = [vp, C.POINTER(VaeDesc), C.POINTER(vp)]
+    L.gm_aae_d_param_count.argtypes = [vp]
+    L.gm_aae_bind_d.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    L.gm_aae_sync_shadows_d.argtypes = [vp, vp]
+    L.gm_aae_recon_grad.argtypes = [vp, vp, i, vp, i, u64, vp, vp]
+    L.gm_aae_d_grad.argtypes = [vp, i, vp, u64, u64, vp, vp]
+    L.gm_aae_g_grad.argtypes = [vp, i, vp, vp]
+    L.gm_aae_apply_d.argtypes = [vp, C.POINTER(AdamHP), i, vp]
+    L.gm_aae_apply_g.argtypes = [vp, C.POINTER(AdamHP), i, vp]
+    L.gm_aae_forward.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
+    L.gm_aae_last_prior.argtypes = [vp, vp, i, vp]
+    L.gm_aae_num_d_slots.argtypes = [vp]
+    L.gm_aae_d_forward.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_aae_d_backward.argtypes = [vp, i, i, vp, vp, vp]
     _lib = L
     return L
 

@@ -853,21 +853,73 @@ __global__ void bir_latent_kernel(const float* __restrict__ mu, int ldm, const f
   }
 }
 
-// the latent upstream of the BIR step: [dz_dec + dz_mmd | 0] -> bf16 [rows, ld] (no KL term, dmu = dz)
-__global__ void bir_dlatent_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ dzm,
+// the latent upstream of the BIR step: [dz_dec + dz_mmd | 0] -> bf16 [rows, ld] (no KL term, dmu = dz).  The AAE's
+// deterministic code feeds the same path: its reconstruction phase passes dzm == nullptr (dmu = dz), its regularisation
+// phase also a per-row factor rs (dmu = rs[r] dz: the G loss's dL/ds times the latent D's input gradient M W1).
+__global__ void bir_dlatent_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ dzm, const float* __restrict__ rs,
                                    __nv_bfloat16* __restrict__ out, int ld, int rows, int z, long long lo_off) {
   griddep_sync();
   const int groups = ld / 8;
   const long long t = blockIdx.x * 256ll + threadIdx.x;
   if (t >= (long long)rows * groups) return;
   const int r = int(t / groups), c0 = int(t % groups) * 8;
+  const float f = rs ? rs[r] : 1.f;
   float v[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = c0 + j;
-    v[j] = c < z ? dz[(long long)r * lddz + c] + dzm[(long long)r * z + c] : 0.f;
+    float o = 0.f;
+    if (c < z) {
+      o = dz[(long long)r * lddz + c];
+      if (rs) o *= f;
+      if (dzm) o += dzm[(long long)r * z + c];
+    }
+    v[j] = o;
   }
   store_bf16x8(out + (long long)r * ld + c0, v, lo_off);
+}
+
+// ---------------------------------------------------------------- adversarial autoencoder
+// Latent rows [v | 1 | 0] -> bf16 [nprior + nfake, ld]: the latent discriminator's operand rows (prior half, then the
+// encoder's half) and the decoder's input rows (nprior = 0).  Rows [0, nprior): the prior sample z_p ~ N(0, I), the
+// caller's p_in or else Philox keyed by (seed, step) with the VAE eps's cell convention (subsequence r * (ld / 8) + group,
+// offset 64 step) under a seed constant of its own, also stored to p_out [nprior, z].  Rows [nprior, nprior + nfake): the
+// deterministic code z = mu (fp32, ld ldm).  One thread per (row, 8-column group of the latent row).
+__global__ void aae_latent_rows_kernel(const float* __restrict__ mu, int ldm, int nfake, const float* __restrict__ p_in,
+                                       float* __restrict__ p_out, int nprior, __nv_bfloat16* __restrict__ zb, int ldz, int z,
+                                       unsigned long long seed, unsigned long long step) {
+  griddep_sync();
+  const int groups = ldz / 8, gz = (z + 8) / 8;
+  const long long t = blockIdx.x * 256ll + threadIdx.x;
+  if (t >= (long long)(nprior + nfake) * gz) return;
+  const int r = int(t / gz), g = int(t % gz), c0 = g * 8;
+  const bool prior = r < nprior;
+  float q[8];
+  if (prior && p_in == nullptr && c0 < z) {
+    curandStatePhilox4_32_10_t st;
+    curand_init(seed ^ 0xC2B2AE3D27D4EB4Full, (unsigned long long)r * groups + g, step * 64ull, &st);
+    const float4 a = curand_normal4(&st), b = curand_normal4(&st);
+    q[0] = a.x; q[1] = a.y; q[2] = a.z; q[3] = a.w; q[4] = b.x; q[5] = b.y; q[6] = b.z; q[7] = b.w;
+  }
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j;
+    float o = (c == z) ? 1.f : 0.f;
+    if (c < z) {
+      if (prior) {
+        const long long i = (long long)r * z + c;
+        o = p_in ? p_in[i] : q[j];
+        p_out[i] = o;
+      } else {
+        o = mu[(long long)(r - nprior) * ldm + c];
+      }
+    }
+    v[j] = o;
+  }
+  store_bf16x8(zb + (long long)r * ldz + c0, v, 0);
+  for (int pg = gz + g; pg < groups; pg += gz)      // this thread's share of the row's zero padding
+    reinterpret_cast<uint4*>(zb)[(long long)r * groups + pg] = make_uint4(0, 0, 0, 0);
 }
 
 // ---------------------------------------------------------------- conditional VAE

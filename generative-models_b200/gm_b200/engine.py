@@ -617,6 +617,148 @@ class BirVaeEngine(VaeEngine):
         return {k: v for k, v in self.views(grads).items() if k.startswith("encoder.")}
 
 
+class AaeEngine(VaeEngine):
+    """One MLP adversarial autoencoder on one GPU: the VAE engine in its AAE mode (gm_aae_create).  Encoder x -> hidden ->
+    z (deterministic), Decoder z -> hidden -> x, and a latent discriminator Dz z -> hidden -> 1 with flat parameters,
+    gradient and Adam state of its own (d_params, ...) and optimizer_G's moments over the encoder (enc_g_exp_avg, ...).
+    One train step: recon_grad, apply (optimizer_R over encoder + decoder), d_grad, apply_d, g_grad, apply_g."""
+    NAMES = BirVaeEngine.NAMES
+    D_NAMES = ["discriminator.linear.weight", "discriminator.linear.bias", "discriminator.discriminate.weight",
+               "discriminator.discriminate.bias"]
+
+    def __init__(self, image_size=784, hidden_dim=400, z_dim=20, max_batch=64, device=None, precision="bf16"):
+        if precision != "bf16":
+            raise GmError("the AAE engine runs in bf16 only (got precision=%r)" % (precision,))
+        X, H, Z = image_size, hidden_dim, z_dim
+        self._open(image_size, hidden_dim, z_dim, max_batch, device, precision, lambda h, d, out: lib().gm_aae_create(h, d, out),
+                   [(H, X), (H,), (Z, H), (Z,), (H, Z), (H,), (X, H), (X,)])
+        nd = lib().gm_aae_d_param_count(self.g)
+        kw = dict(device=self.device, dtype=torch.float32)
+        self.d_params, self.d_grads = torch.zeros(nd, **kw), torch.zeros(nd, **kw)
+        self.d_exp_avg, self.d_exp_avg_sq = torch.zeros(nd, **kw), torch.zeros(nd, **kw)
+        ne = H * X + H + Z * H + Z                 # the encoder prefix of the flat layout
+        self.n_enc = ne
+        self.enc_g_exp_avg, self.enc_g_exp_avg_sq = torch.zeros(ne, **kw), torch.zeros(ne, **kw)
+        check(self.h, lib().gm_aae_bind_d(self.g, _ptr(self.d_params), _ptr(self.d_grads), _ptr(self.d_exp_avg),
+                                          _ptr(self.d_exp_avg_sq), _ptr(self.enc_g_exp_avg), _ptr(self.enc_g_exp_avg_sq)))
+        self.d_shapes = [(H, Z), (H,), (1, H), (1,)]
+        self.d_loss_buf, self.g_loss_buf = torch.zeros(1, **kw), torch.zeros(1, **kw)
+        self.d_steps, self.g_steps = 0, 0
+
+    # ---- the latent discriminator's parameters
+    def d_views(self, flat=None):
+        """{discriminator parameter name: view into the flat D buffer}"""
+        flat = self.d_params if flat is None else flat
+        out, off = {}, 0
+        for name, shp in zip(self.D_NAMES, self.d_shapes):
+            n = 1
+            for s in shp:
+                n *= s
+            out[name] = flat[off:off + n].view(shp)
+            off += n
+        return out
+
+    def views(self, flat=None):
+        """{parameter name: view}: the encoder / decoder of the main buffer (or of `flat`), and with no `flat` the
+        discriminator's views of d_params too"""
+        out = super().views(flat)
+        if flat is None:
+            out.update(self.d_views())
+        return out
+
+    def load(self, tensors):
+        main = {k: v for k, v in tensors.items() if not k.startswith("discriminator.")}
+        dv = self.d_views()
+        for name, src in tensors.items():
+            if name.startswith("discriminator."):
+                dv[name].copy_(torch.as_tensor(src, dtype=torch.float32).reshape(dv[name].shape))
+        VaeEngine.load(self, main)
+        self.sync_shadows_d()
+
+    def sync_shadows_d(self):
+        check(self.h, lib().gm_aae_sync_shadows_d(self.g, _stream()))
+
+    def sync_all(self):
+        self.sync_shadows()
+        self.sync_shadows_d()
+
+    sync_if_stale = sync_all
+
+    def reset_optimizer(self):
+        """zero the three Adam states: optimizer_R (encoder + decoder), optimizer_D and optimizer_G (encoder)"""
+        super().reset_optimizer()
+        for t in (self.d_exp_avg, self.d_exp_avg_sq, self.enc_g_exp_avg, self.enc_g_exp_avg_sq):
+            t.zero_()
+        self.d_steps, self.g_steps = 0, 0
+
+    # ---- the three phases of one train step
+    def recon_grad(self, images, fmt="f32", gather_idx=None, batch=None, step=0):
+        """phase 1, recon = sum (x - D(E(x)))^2 and its gradient.  Returns the device tensor [recon] (a view of loss_buf)."""
+        B = batch if batch is not None else (gather_idx.numel() if gather_idx is not None else images.shape[0])
+        check(self.h, lib().gm_aae_recon_grad(self.g, _ptr(images), IMG_FMTS[fmt], _ptr(gather_idx), B, int(step),
+                                              _ptr(self.loss_buf), _stream()))
+        return self.loss_buf[:1]
+
+    def d_grad(self, batch, prior=None, seed=0, step=0):
+        """phase 2 on the batch recon_grad staged: D_loss and Dz's gradient (d_grads); prior [batch, z] or the device draw"""
+        if prior is not None:
+            prior = prior.float().contiguous()
+        check(self.h, lib().gm_aae_d_grad(self.g, batch, _ptr(prior), int(seed), int(step), _ptr(self.d_loss_buf), _stream()))
+        return self.d_loss_buf
+
+    def g_grad(self, batch):
+        """phase 3 on phase 2's encoding: G_loss and the encoder prefix of grads"""
+        check(self.h, lib().gm_aae_g_grad(self.g, batch, _ptr(self.g_loss_buf), _stream()))
+        return self.g_loss_buf
+
+    def apply_d(self, hp):
+        self.d_steps += 1
+        check(self.h, lib().gm_aae_apply_d(self.g, C.byref(hp), self.d_steps, _stream()))
+
+    def apply_g(self, hp):
+        self.g_steps += 1
+        check(self.h, lib().gm_aae_apply_g(self.g, C.byref(hp), self.g_steps, _stream()))
+
+    def last_prior(self, batch):
+        out = torch.empty(batch, self.z_dim, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_aae_last_prior(self.g, _ptr(out), batch, _stream()))
+        return out
+
+    def forward(self, images, fmt="f32", want_images=True, want_latent=True, want_losses=False):
+        """-> (images or None, z or None, losses [recon] or None)"""
+        n = images.shape[0]
+        kw = dict(device=self.device, dtype=torch.float32)
+        out = torch.empty(n, self.image_size, **kw) if want_images else None
+        z = torch.empty(n, self.z_dim, **kw) if want_latent else None
+        ls = torch.empty(1, **kw) if want_losses else None
+        check(self.h, lib().gm_aae_forward(self.g, _ptr(images.contiguous()), IMG_FMTS[fmt], n, _ptr(out), _ptr(z), _ptr(ls),
+                                           _stream()))
+        return out, z, ls
+
+    BUFFERS = dict(VaeEngine.BUFFERS, ZD=8, AD=9, DHD=10)
+
+    encoder_forward = BirVaeEngine.encoder_forward
+    encoder_backward = BirVaeEngine.encoder_backward
+
+    # ---- the per-call latent D (user-written train_D / train_G)
+    def num_d_slots(self):
+        return lib().gm_aae_num_d_slots(self.g)
+
+    def d_forward(self, slot, z):
+        """Dz.forward on slot's rows: z [n, z] fp32 -> scores [n] fp32"""
+        n = z.shape[0]
+        out = torch.empty(n, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_aae_d_forward(self.g, slot, _ptr(z.float().contiguous()), n, _ptr(out), _stream()))
+        return out
+
+    def d_backward(self, slot, dscores, need_dz):
+        """-> ({discriminator parameter name: gradient} (views of d_grads, overwritten by the next call), dL/dz or None)"""
+        n = dscores.shape[0]
+        dz = torch.empty(n, self.z_dim, device=self.device, dtype=torch.float32) if need_dz else None
+        check(self.h, lib().gm_aae_d_backward(self.g, slot, n, _ptr(dscores.reshape(-1).float().contiguous()), _ptr(dz), _stream()))
+        return self.d_views(self.d_grads), dz
+
+
 class ClassIds:
     """Class labels checked against an engine's num_classes and held as an int32 tensor on its device (CvaeEngine.class_ids)"""
     __slots__ = ("t", "num_classes")

@@ -323,7 +323,8 @@ int gm_vae_set_lazy_grads(gm_vae* vae, int on, gm_stream stream);
 int gm_vae_materialize_grads(gm_vae* vae, gm_stream stream);
 /* eps of the last gm_vae_grad / gm_vae_forward call (src/vae.py:104; the Philox draw when eps_dev was NULL) -> out_dev [batch, z] */
 int gm_vae_last_eps(gm_vae* vae, float* out_dev, int batch, gm_stream stream);
-/* test aid: an internal bf16 buffer of the last gm_vae_grad as fp32 (hi + lo planes summed in split mode) -> out_dev [rows, cols];
+/* test aid: an internal bf16 buffer of the last gm_vae_grad as fp32 (hi + lo planes summed in split mode) -> out_dev [rows, cols]
+ * (AAE engines also: 8 the latent D rows [z | 1 | 0], 9 its hidden rows, 10 their gradient, 2 max_batch rows each);
  * which: 0 image rows, 1 encoder hidden, 2 latent z, 3 decoder hidden, 4 dL/d recon pre-sigmoid, 5 decoder hidden gradient,
  * 6 [dmu | dlog_var], 7 encoder hidden gradient */
 int gm_vae_debug_read(gm_vae* vae, int which, int row0, int rows, int cols, float* out_dev, gm_stream stream);
@@ -418,6 +419,52 @@ int gm_cvae_encoder_forward(gm_vae* vae, int slot, const float* x_dev, const int
                             gm_stream stream);
 int gm_cvae_decoder_forward(gm_vae* vae, int slot, const float* z_dev, const int* labels_dev, int batch, float* images_dev,
                             gm_stream stream);
+
+/* ---- adversarial autoencoder (aae.py; Makhzani et al. 2015): an AAE mode of the VAE engine --------------------------
+ * Encoder x -> hidden (ReLU) -> z (the deterministic code z = mu), Decoder z -> hidden (ReLU) -> x (sigmoid), and a latent
+ * discriminator Dz z -> hidden (ReLU) -> 1 (sigmoid), the probability that z came from the prior N(0, I).  The main flat
+ * layout is the BIR-VAE's [enc.linear.W | .b | enc.mu.W | .b | dec.linear.W | .b | dec.recon.W | .b]; Dz has a block of
+ * its own [W1 (hidden, z) | b1 | w2 (1, hidden) | b2].  One train step is three phases, each followed by its optimizer:
+ *   gm_aae_recon_grad + gm_vae_apply      recon = sum (x - D(E(x)))^2, Adam over encoder + decoder (optimizer_R)
+ *   gm_aae_d_grad + gm_aae_apply_d        D_loss = -mean(log(Dz(z_p) + 1e-8) + log(1 - Dz(E(x)) + 1e-8)) (optimizer_D)
+ *   gm_aae_g_grad + gm_aae_apply_g        G_loss = -mean(log(Dz(E(x)) + 1e-8)), Adam over the encoder (optimizer_G)
+ * Each phase sees the parameters the previous one updated: gm_aae_d_grad encodes the batch gm_aae_recon_grad staged
+ * once more, and gm_aae_g_grad reuses that encoding.  The engine is a gm_vae: bind, sync_shadows, apply, set_sampler,
+ * set_lazy_grads, materialize_grads, debug_read, decode and the gm_vae_{encoder,decoder}_{forward,backward} entries serve
+ * it as they serve a BIR-VAE engine; gm_vae_grad, gm_vae_forward, gm_vae_last_eps and the gm_bir_vae_* / gm_cvae_* entries
+ * refuse it, and the gm_aae_* entries refuse any other engine, with GM_ERR_ARG.  gm_aae_create accepts what
+ * gm_bir_vae_create accepts (1 <= z_dim <= 32, hidden_dim <= 447) and refuses GM_PREC_SPLIT with GM_ERR_UNSUPPORTED. */
+int gm_aae_create(gm_ctx* ctx, const gm_vae_desc* desc, gm_vae** out);
+int gm_aae_d_param_count(const gm_vae* vae);
+/* Dz's flat fp32 parameters, gradient and Adam moments (16-byte aligned parameters), and optimizer_G's moments over the
+ * encoder prefix [enc.linear.W | .b | enc.mu.W | .b] of the main layout; the moment pointers may be NULL until an apply. */
+int gm_aae_bind_d(gm_vae* vae, float* d_params_dev, float* d_grads_dev, float* d_exp_avg_dev, float* d_exp_avg_sq_dev,
+                  float* enc_g_exp_avg_dev, float* enc_g_exp_avg_sq_dev);
+int gm_aae_sync_shadows_d(gm_vae* vae, gm_stream stream);
+/* phase 1: losses_dev[0] = recon; the flat gradient (or, with lazy gradients, its partials for gm_vae_apply).  The rows are
+ * read as gm_vae_grad reads them (gather_idx_dev, the epoch sampler at `step`, or rows 0..batch-1). */
+int gm_aae_recon_grad(gm_vae* vae, const void* images_dev, int img_fmt, const int* gather_idx_dev, int batch, uint64_t step,
+                      float* losses_dev, gm_stream stream);
+/* phase 2 on the batch phase 1 staged (GM_ERR_STATE otherwise): prior_dev [batch, z] fp32, or NULL for N(0, 1) Philox
+ * draws keyed by (seed, step); loss_dev[0] = D_loss; Dz's flat gradient. */
+int gm_aae_d_grad(gm_vae* vae, int batch, const float* prior_dev, uint64_t seed, uint64_t step, float* loss_dev, gm_stream stream);
+/* phase 3 on the batch phase 2 encoded (GM_ERR_STATE otherwise): loss_dev[0] = G_loss; the encoder prefix of the flat
+ * gradient (the decoder's segments keep phase 1's values). */
+int gm_aae_g_grad(gm_vae* vae, int batch, float* loss_dev, gm_stream stream);
+int gm_aae_apply_d(gm_vae* vae, const gm_adam_hp* hp, int step, gm_stream stream);
+int gm_aae_apply_g(gm_vae* vae, const gm_adam_hp* hp, int step, gm_stream stream);
+/* AAE.forward (+ recon) without gradients; any of out_images_dev [n, image_size], z_dev [n, z], losses_dev [1] may be NULL. */
+int gm_aae_forward(gm_vae* vae, const void* images_dev, int img_fmt, int n, float* out_images_dev, float* z_dev, float* losses_dev,
+                   gm_stream stream);
+/* the prior sample z_p of the last gm_aae_d_grad -> out_dev [batch, z] fp32 */
+int gm_aae_last_prior(gm_vae* vae, float* out_dev, int batch, gm_stream stream);
+/* Dz.forward and its backward for a user-written train_D / train_G: slot in [0, gm_aae_num_d_slots) keeps one call's
+ * activations until its backward, which only reads them (it may run more than once).  gm_aae_d_forward: z_dev [batch, z]
+ * fp32 -> scores_dev [batch] fp32.  gm_aae_d_backward: dscores_dev [batch] -> Dz's flat gradient (the bound buffer) and,
+ * when dz_dev is not NULL, dz_dev [batch, z] fp32.  A fused gm_aae_d_grad / gm_aae_g_grad reuses the slots' rows. */
+int gm_aae_num_d_slots(const gm_vae* vae);
+int gm_aae_d_forward(gm_vae* vae, int slot, const float* z_dev, int batch, float* scores_dev, gm_stream stream);
+int gm_aae_d_backward(gm_vae* vae, int slot, int batch, const float* dscores_dev, float* dz_dev, gm_stream stream);
 
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
