@@ -49,6 +49,11 @@ class VaeDesc(C.Structure):
                 ("dtype_mode", C.c_int)]
 
 
+class SghmcHP(C.Structure):
+    """include/gm_b200.h: gm_sghmc_hp (gm_bgan_apply)"""
+    _fields_ = [("lr", C.c_float), ("alpha", C.c_float), ("prior_std", C.c_float), ("data_size", C.c_float)]
+
+
 class GanDesc(C.Structure):
     _fields_ = [("image_size", C.c_int), ("hidden_dim", C.c_int), ("z_dim", C.c_int),
                 ("max_batch", C.c_int), ("variant", C.c_int), ("d_out_act", C.c_int), ("dtype_mode", C.c_int)]
@@ -211,6 +216,14 @@ def lib():
     L.gm_aae_num_d_slots.argtypes = [vp]
     L.gm_aae_d_forward.argtypes = [vp, i, vp, i, vp, vp]
     L.gm_aae_d_backward.argtypes = [vp, i, i, vp, vp, vp]
+    L.gm_bgan_create.argtypes = [vp, C.POINTER(GanDesc), i, C.POINTER(vp)]
+    L.gm_bgan_num_samples.argtypes = [vp]
+    L.gm_bgan_g_stride.argtypes = [vp]
+    L.gm_bgan_d_grad.argtypes = [vp, vp, i, vp, i, vp, u64, u64, vp, vp]
+    L.gm_bgan_g_grad.argtypes = [vp, i, vp, u64, u64, vp, vp]
+    L.gm_bgan_apply.argtypes = [vp, i, C.POINTER(SghmcHP), u64, u64, vp]
+    L.gm_bgan_generate.argtypes = [vp, i, vp, i, vp, vp]
+    L.gm_bgan_sghmc_noise.argtypes = [vp, i, u64, u64, vp, vp]
     _lib = L
     return L
 

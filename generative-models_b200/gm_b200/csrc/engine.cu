@@ -667,6 +667,14 @@ struct StepPlans {
   GemmPlan be_enc_d, be_dec_d, be_gwd, be_de_d, be_enc_g, be_dec_g, be_de_g, be_dxg;   // BEGAN autoencoder-discriminator
 };
 
+// Bayesian GAN (engine_bayes.inl): the generator GEMMs once per sample (pointer offsets into the stacked operand copies,
+// noise, hidden and fake rows), D's over the real and every sample's fake rows at once
+constexpr int kBganMaxSamples = 16;
+struct BayesPlans {
+  GemmPlan g1[kBganMaxSamples], g2[kBganMaxSamples], dw2g[kBganMaxSamples], dhg[kBganMaxSamples], dw1g[kBganMaxSamples];
+  GemmPlan d1_d, dw1d, d1_g, dx;
+};
+
 struct gm_comm {
   gm_ctx* ctx = nullptr;
   int rank = 0, world = 1, nblocks = 0;
@@ -754,7 +762,20 @@ struct gm_gan {
   std::vector<void*> allocs;
   BfArena arena;
   long long lo = 0;          // arena.lo_off: > 0 in split-operand mode
+  // Bayes mode (gm_bgan_create): nsamp > 0 generator samples, stacked in G's flat block g_stride floats apart (a multiple
+  // of 4: every sample starts on 16 bytes).  Only the gm_bgan_* entries and the shared ones (bind, sync_shadows,
+  // param_count, set_sampler, discriminate, debug_read) serve such an engine.
+  int nsamp = 0, g_stride = 0;
+  std::map<int, BayesPlans> bplans;
 };
+
+// The point-estimate entries (Adam, the fused and per-call steps, data parallelism, device steps, Q and BEGAN) refuse a
+// Bayes-mode engine before anything is launched
+static int refuse_bayes(gm_gan* g, const char* what) {
+  return fail(g->ctx, GM_ERR_ARG, "%s cannot serve a Bayesian GAN engine (use the gm_bgan_* entries)", what);
+}
+#define REFUSE_BAYES(g, what) do { if ((g) && (g)->nsamp) return refuse_bayes((g), (what)); } while (0)
+static int bgan_sync_shadows(gm_gan* g, int net, cudaStream_t s);
 
 // Zeroed device buffers of an engine (gm_gan, gm_vae), freed by its destroy.  bf16 buffers come from the engine's arena
 // (finalised at the end of create) unless T is given explicitly, as for the VAE's per-call slot buffers.
@@ -894,6 +915,7 @@ extern "C" int gm_gan_create(gm_ctx* c, const gm_gan_desc* d, gm_gan** out) {
 
 extern "C" int gm_gan_param_count(const gm_gan* g, int net) {
   if (!g) return GM_ERR_ARG;
+  if (net == GM_NET_G && g->nsamp) return g->nsamp * g->g_stride;   // the stacked samples (engine_bayes.inl)
   return net == GM_NET_G ? g->G.total : g->D.total;
 }
 
@@ -902,7 +924,7 @@ extern "C" int gm_gan_bind(gm_gan* g, int net, float* p, float* gr, float* m, fl
   if (reinterpret_cast<uintptr_t>(p) & 15)
     return fail(g->ctx, GM_ERR_ARG, "parameter buffer must be 16-byte aligned");
   g->par[net] = p; g->grd[net] = gr; g->am[net] = m; g->av[net] = v;
-  g->plans.clear(); g->cplans.clear(); g->qplans.clear();
+  g->plans.clear(); g->cplans.clear(); g->qplans.clear(); g->bplans.clear();
   return GM_OK;
 }
 
@@ -929,6 +951,7 @@ static void adam_segs(gm_gan* g, int net, AdamParams& a) {
 extern "C" int gm_gan_sync_shadows(gm_gan* g, int net, gm_stream stream) {
   if (!g || net < 0 || net > 1) return GM_ERR_ARG;
   if (!g->par[net]) return fail(g->ctx, GM_ERR_STATE, "net %d not bound", net);
+  if (g->nsamp) return bgan_sync_shadows(g, net, static_cast<cudaStream_t>(stream));
   AdamParams a;
   memset(&a, 0, sizeof a);
   a.p = g->par[net];
@@ -945,6 +968,7 @@ static int bump_step(gm_gan* g, int which, cudaStream_t s) {
 
 
 extern "C" int gm_gan_apply(gm_gan* g, int net, const gm_adam_hp* hp, int step, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_apply");
   if (!g || net < 0 || net > 1 || !hp || step <= 0) return g ? fail(g->ctx, GM_ERR_ARG, "gm_gan_apply: bad argument") : GM_ERR_ARG;
   if (!g->par[net] || !g->am[net] || !g->av[net]) return fail(g->ctx, GM_ERR_STATE, "net %d not fully bound", net);
   AdamParams a;
@@ -964,6 +988,7 @@ extern "C" int gm_gan_apply(gm_gan* g, int net, const gm_adam_hp* hp, int step, 
 extern "C" int gm_gan_set_lazy_grads(gm_gan* g, int on, gm_stream stream) {
   if (!g) return GM_ERR_ARG;
   int rc;
+  if (on) REFUSE_BAYES(g, "gm_gan_set_lazy_grads");
   if (!on && (rc = flush_pending(g, static_cast<cudaStream_t>(stream)))) return rc;
   g->lazy = on != 0;
   return GM_OK;
@@ -1264,6 +1289,7 @@ static int began_g_grad(gm_gan* g, StepPlans* sp, int B, float* loss_dev, cudaSt
 
 // BEGAN device state: host get/set of [K, inv_b, -K inv_b, DX, DG, best, bad, lr_scale, inv_b, inv_b, convergence]
 extern "C" int gm_gan_began_state(gm_gan* g, float* host11, int set, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_began_state");
   if (!g || !host11) return GM_ERR_ARG;
   if (g->d.variant != GM_BEGAN) return fail(g->ctx, GM_ERR_STATE, "not a BEGAN engine");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1276,6 +1302,7 @@ extern "C" int gm_gan_began_state(gm_gan* g, float* host11, int set, gm_stream s
 }
 // K <- clip(K + LAMBDA (GAMMA DX - DG), 0, 1) and the plateau schedulers (src/be_gan.py:186-195)
 extern "C" int gm_gan_began_control(gm_gan* g, float gamma, float lambda, float patience, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_began_control");
   if (!g) return GM_ERR_ARG;
   if (g->d.variant != GM_BEGAN) return fail(g->ctx, GM_ERR_STATE, "not a BEGAN engine");
   return launch(g->ctx, "began_control_kernel", began_control_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), g->be_state, gamma, lambda, patience);
@@ -1296,6 +1323,7 @@ static int stage_real_rows(gm_gan* g, const void* images, int img_fmt, const int
 // with the same batch skips its own staging.  Nothing of a G step reads those rows, so a data-parallel host enqueues this
 // between gm_gan_exchange_begin(G) and gm_gan_apply_allreduce(G).  `step` = the step argument the later gm_gan_d_grad gets.
 extern "C" int gm_gan_d_stage(gm_gan* g, const void* images, int img_fmt, const int* gather_idx, int batch, uint64_t step, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_d_stage");
   int rc = check_step_args(g, batch);
   if (rc) return rc;
   if (!images) return fail(g->ctx, GM_ERR_ARG, "images is null");
@@ -1308,6 +1336,7 @@ extern "C" int gm_gan_d_stage(gm_gan* g, const void* images, int img_fmt, const 
 extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const int* gather_idx, int batch,
                              const float* noise, const float* aux, float inv_global_batch, uint64_t seed,
                              uint64_t step, float* loss_dev, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_d_grad");
   int rc = check_step_args(g, batch);
   if (rc) return rc;
   if (!images) return fail(g->ctx, GM_ERR_ARG, "images is null");
@@ -1408,6 +1437,7 @@ extern "C" int gm_gan_d_grad(gm_gan* g, const void* images, int img_fmt, const i
 // while the D-gradient exchange is still in flight on another stream)
 static int g_grad_impl(gm_gan* g, int batch, const float* noise, float inv_global_batch, uint64_t seed, uint64_t step,
                        float* loss_dev, gm_stream stream, bool staged) {
+  REFUSE_BAYES(g, "gm_gan_g_grad");
   int rc = check_step_args(g, batch);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1445,6 +1475,7 @@ extern "C" int gm_gan_g_grad(gm_gan* g, int batch, const float* noise, float inv
   return g_grad_impl(g, batch, noise, inv_global_batch, seed, step, loss_dev, stream, false);
 }
 extern "C" int gm_gan_g_forward_stage(gm_gan* g, int batch, const float* noise, uint64_t seed, uint64_t step, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_g_forward_stage");
   int rc = check_step_args(g, batch);
   if (rc) return rc;
   StepPlans* sp;
@@ -1458,6 +1489,7 @@ extern "C" int gm_gan_g_grad_staged(gm_gan* g, int batch, float inv_global_batch
 
 // ---- InfoGAN: auxiliary network Q and the mutual-information step (src/info_gan.py:269-304,196-205)
 extern "C" int gm_gan_bind_q(gm_gan* g, float* q_params, float* q_grads, float* q_m, float* q_v, float* g_mi_m, float* g_mi_v) {
+  REFUSE_BAYES(g, "gm_gan_bind_q");
   if (!g || !q_params || !q_grads) return g ? fail(g->ctx, GM_ERR_ARG, "gm_gan_bind_q: bad argument") : GM_ERR_ARG;
   if (g->d.variant != GM_INFO) return fail(g->ctx, GM_ERR_STATE, "gm_gan_bind_q: engine was not created with GM_INFO");
   g->parQ = q_params; g->grdQ = q_grads; g->amQ = q_m; g->avQ = q_v; g->amG2 = g_mi_m; g->avG2 = g_mi_v;
@@ -1474,6 +1506,7 @@ static void q_adam_segs(gm_gan* g, AdamParams& a) {
   a.seg[1] = {g->Qn.off_w2, g->q_out * g->H, g->H, g->Wq2_s, g->H, g->Wq2_t, 64};
 }
 extern "C" int gm_gan_sync_shadows_q(gm_gan* g, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_sync_shadows_q");
   if (!g || !g->parQ) return g ? fail(g->ctx, GM_ERR_STATE, "Q not bound") : GM_ERR_ARG;
   AdamParams a;
   memset(&a, 0, sizeof a);
@@ -1487,6 +1520,7 @@ extern "C" int gm_gan_sync_shadows_q(gm_gan* g, gm_stream stream) {
 // z, one-hot code at [zd, zd+10), continuous code at [zd+10, zd+20)).
 extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, float inv_global_batch, float* loss_dev,
                              gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_q_grad");
   int rc = check_step_args(g, batch);
   if (rc) return rc;
   if (g->d.variant != GM_INFO || !g->parQ) return fail(g->ctx, GM_ERR_STATE, "bind Q first (GM_INFO engines only)");
@@ -1540,6 +1574,7 @@ extern "C" int gm_gan_q_grad(gm_gan* g, int batch, const float* noise, int zd, f
 // MI_optimizer.step(): Adam over G (with its OWN moment buffers, separate from G_optimizer's)
 // and over Q (src/info_gan.py:146-148,205); refreshes both nets' operand copies.
 extern "C" int gm_gan_apply_mi(gm_gan* g, const gm_adam_hp* hp, int step, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_apply_mi");
   if (!g || !hp || step <= 0) return g ? fail(g->ctx, GM_ERR_ARG, "gm_gan_apply_mi: bad argument") : GM_ERR_ARG;
   if (!g->parQ || !g->amQ || !g->avQ || !g->amG2 || !g->avG2) return fail(g->ctx, GM_ERR_STATE, "Q / MI optimizer state not bound");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1579,6 +1614,7 @@ __global__ void bf16_rows_to_f32_kernel(const __nv_bfloat16* __restrict__ src, i
 }
 
 extern "C" int gm_gan_generate(gm_gan* g, const float* noise, int n, float* images, gm_stream stream) {
+  REFUSE_BAYES(g, "gm_gan_generate");
   if (!g || !images || n <= 0) return GM_ERR_ARG;
   if (!g->par[0]) return fail(g->ctx, GM_ERR_STATE, "bind G first");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1622,6 +1658,7 @@ extern "C" int gm_gan_discriminate(gm_gan* g, const void* images, int img_fmt, i
 // calls, train_D calls}; the `step` arguments of those entry points are ignored while the mode is on.
 extern "C" int gm_gan_use_device_step(gm_gan* g, int on, const unsigned long long* counters4_host, gm_stream stream) {
   if (!g) return GM_ERR_ARG;
+  if (on) REFUSE_BAYES(g, "gm_gan_use_device_step");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (on) {
     if (!g->dstep) {
@@ -1697,8 +1734,9 @@ extern "C" int gm_gan_debug_read(gm_gan* g, int which, int row0, int rows, int c
   which %= 16;
   const __nv_bfloat16* src[9] = {g->Zb, g->Hg, g->Xall, g->Aall, g->DHall, g->DA2, g->DHg, g->qs[0].H, g->qs[1].H};
   const int ld[9] = {g->ZP, g->HP, g->XP, g->HP, g->HP, g->XP, g->HP, g->HP, g->HP};
-  const long long nrow[9] = {g->Bmax, g->Bmax, (long long)g->nreg * g->Bmax, (long long)g->nreg * g->Bmax,
-                             (long long)g->nreg * g->Bmax, g->Bmax, g->Bmax, g->Bmax, g->Bmax};
+  // a Bayes-mode engine holds num_g x max_batch noise, G hidden and dL/dG rows and (1 + num_g) x max_batch image / D rows
+  const long long J = g->nsamp ? g->nsamp : 1, nr = g->nsamp ? 1 + J : g->nreg;
+  const long long nrow[9] = {J * g->Bmax, J * g->Bmax, nr * g->Bmax, nr * g->Bmax, nr * g->Bmax, J * g->Bmax, g->Bmax, g->Bmax, g->Bmax};
   static_assert(kQSlots == 2, "debug buffers 7, 8 are the Q call slots' hidden rows");
   if (which < 0 || which > 8 || cols > ld[which] || !src[which]) return fail(g->ctx, GM_ERR_ARG, "gm_gan_debug_read: bad buffer / extent");
   if ((long long)row0 + rows > nrow[which])
@@ -1723,3 +1761,4 @@ extern "C" int gm_gan_fisher_state(gm_gan* g, float* lambda_rho_host, int set, g
 #include "engine_comm.inl"
 #include "engine_vae.inl"
 #include "engine_conv.inl"
+#include "engine_bayes.inl"

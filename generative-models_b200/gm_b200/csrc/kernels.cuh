@@ -1399,6 +1399,103 @@ __global__ void adam_kernel(const AdamParams a) {
   adam_element(a, i, g);
 }
 
+// ---------------------------------------------------------------- Bayesian GAN (engine_bayes.inl)
+// D step over the real rows [0, B) and nfake generator samples' fake rows [B, (1 + nfake) B) of the NS loss
+// (src/ns_gan.py:191): U_D = -mean_i log(D(x_i) + eps) - mean_{j,i} log(1 - D(G_j(z_ji)) + eps).  Real rows weigh p.inv_b,
+// fake rows inv_b_fake = 1/(nfake B); the loss sums the fake rows' terms times w_fake = 1/nfake before loss_finalize's
+// division by B.  With nfake = 1 every value and every sum is loss_pass_kernel<2>'s (NS, sigmoid output), bit for bit.
+__global__ void __launch_bounds__(kLossThreads) bgan_d_loss_kernel(const LossParams p, int nfake, float inv_b_fake, double w_fake) {
+  griddep_sync();
+  __shared__ double sh[kLossThreads / 32];
+  const int rows = (1 + nfake) * p.B;
+  const float b2 = p.b2[0];
+  double a0 = 0, a1 = 0;
+  for (int r = blockIdx.x * kLossThreads + threadIdx.x; r < rows; r += gridDim.x * kLossThreads) {
+    float s = 0.f;
+    for (int k = 0; k < p.nslots; ++k) s += p.slots[(long long)k * p.slot_ld + r];
+    s = s + b2;
+    const float d = act_out(s, p.out_act);
+    const bool fake = r >= p.B;
+    float l, g;
+    if (!fake) { l = -logf(d + kEps); g = -1.f / (d + kEps); }
+    else { l = -logf((1.f - d) + kEps); g = 1.f / ((1.f - d) + kEps); }
+    const float dsr = g * (fake ? inv_b_fake : p.inv_b) * act_grad(s, d, p.out_act);
+    p.ds[r] = dsr;
+    if (p.d_out) p.d_out[r] = d;
+    a0 += fake ? double(l) * w_fake : double(l);
+    a1 += dsr;
+  }
+  a0 = block_sum<kLossThreads>(a0, sh); a1 = block_sum<kLossThreads>(a1, sh);
+  if (threadIdx.x == 0) {
+    double* out = p.partR + (long long)blockIdx.x * 4;
+    out[0] = a0; out[1] = a1; out[2] = 0.0; out[3] = 0.0;
+  }
+  __shared__ bool last;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = atomicAdd(p.done, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (last) {
+    __threadfence();
+    loss_finalize(p, sh);
+    if (threadIdx.x == 0) *p.done = 0u;
+  }
+}
+
+// Stochastic-gradient Hamiltonian Monte Carlo (Saatchi & Wilson 2017, Algorithm 1 with beta = 0) over a flat block of
+// `total` = samples x stride floats, elementwise with momentum v:
+//   v <- (1 - alpha) v - lr (g + theta / (prior_std^2 N)) + sqrt(2 alpha lr / N) xi,   theta <- theta + v
+// Element i belongs to sample i / stride at offset i % stride of that sample's layout (offsets >= n are alignment padding
+// and left alone).  xi ~ N(0, 1) is Philox with subsequence i at `offset` ((step, net) of the update), so every element,
+// sample, net and step draws its own number.  After the update the element is written to its sample's bf16 operand
+// copies (seg[k].shadow + sample x sh_stride[k], as adam_kernel writes one net's).  update 0: refresh the copies only;
+// xi_out: write xi for every element of the block and nothing else (test aid).
+struct SghmcParams {
+  float* p; const float* g; float* v;
+  int total, stride, n;
+  float lr, alpha, prior_scale, noise_scale;   // prior_scale = 1 / (prior_std^2 N), noise_scale = sqrt(2 alpha lr / N)
+  unsigned long long seed, offset;
+  int update;
+  float* xi_out;
+  AdamSeg seg[2]; int nseg;
+  long long sh_stride[2], sht_stride[2];       // elements between consecutive samples' K-major / transposed copies
+};
+
+__device__ __forceinline__ float sghmc_xi(const SghmcParams& a, int i) {
+  curandStatePhilox4_32_10_t st;
+  curand_init(a.seed, (unsigned long long)i, a.offset, &st);
+  return curand_normal(&st);
+}
+
+__global__ void sghmc_kernel(const SghmcParams a) {
+  griddep_sync();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.total) return;
+  if (a.xi_out) { a.xi_out[i] = sghmc_xi(a, i); return; }
+  const int smp = i / a.stride, k = i - smp * a.stride;
+  if (k >= a.n) return;
+  float p = a.p[i];
+  if (a.update) {
+    const float gp = a.g[i] + p * a.prior_scale;
+    const float v = (1.f - a.alpha) * a.v[i] - a.lr * gp + a.noise_scale * sghmc_xi(a, i);
+    a.v[i] = v;
+    p = p + v;
+    a.p[i] = p;
+  }
+#pragma unroll 1
+  for (int q = 0; q < a.nseg; ++q) {
+    const AdamSeg& s = a.seg[q];
+    const int j = k - s.off;
+    if (j < 0 || j >= s.n) continue;
+    const int r = j / s.cols, c = j % s.cols;
+    const __nv_bfloat16 b = __float2bfloat16_rn(p);
+    if (s.shadow) s.shadow[smp * a.sh_stride[q] + (long long)r * s.ld_s + c] = b;
+    if (s.shadow_t) s.shadow_t[smp * a.sht_stride[q] + (long long)c * s.ld_t + r] = b;
+    return;
+  }
+}
+
 // ---------------------------------------------------------------- gradient all-reduce fused into Adam
 // Data-parallel optimizer step in ONE kernel per rank (SURVEY.md 8e: the only exchange of the
 // path is the SUM of the flat D / G gradient): block b

@@ -890,3 +890,91 @@ def mmd_gaussian(z, p, lam=1.0, want_grad=True):
     h = _lib.ctx(z.device.index)
     check(h, lib().gm_mmd_gaussian(h, _ptr(z), _ptr(p), z.shape[0], z.shape[1], float(lam), _ptr(out), _ptr(dz), _stream()))
     return out, dz
+
+
+class BayesGanEngine(GanEngine):
+    """One MLP Bayesian GAN on one GPU: the GAN engine in its Bayes mode (gm_bgan_create), num_g generator samples and
+    one discriminator with the NS energies, every net moved by SGHMC (include/gm_b200.h).  params[G] stacks the samples
+    [sample 0 | sample 1 | ...], `stride` floats apart, each in GanEngine's G layout; views(G, sample=j) are sample j's
+    tensors.  momentum[net] is SGHMC's v (bound in the exp_avg slot); there is no second moment."""
+
+    def __init__(self, image_size=784, hidden_dim=400, z_dim=20, num_g=10, max_batch=64, device=None, precision="bf16"):
+        if precision != "bf16":
+            raise GmError("the Bayesian GAN engine runs in bf16 only (got precision=%r)" % (precision,))
+        if not 1 <= int(num_g) <= 16:
+            raise GmError("num_g must be in [1, 16] (got %r)" % (num_g,))
+        if not torch.cuda.is_available():
+            raise GmError("gm_b200 needs a CUDA (H100) device; there is no CPU fallback")
+        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.h = _lib.ctx(self.device.index)
+        self.image_size, self.hidden_dim, self.z_dim, self.max_batch = image_size, hidden_dim, z_dim, max_batch
+        self.variant, self.precision, self.num_g = "ns", precision, int(num_g)
+        d = GanDesc(image_size, hidden_dim, z_dim, max_batch, VARIANTS["ns"], OUT_ACTS["sigmoid"], PRECISIONS[precision])
+        self.g = C.c_void_p()
+        check(self.h, lib().gm_bgan_create(self.h, C.byref(d), self.num_g, C.byref(self.g)))
+        self.stride = lib().gm_bgan_g_stride(self.g)
+        self.n = [lib().gm_gan_param_count(self.g, G), lib().gm_gan_param_count(self.g, D)]
+        kw = dict(device=self.device, dtype=torch.float32)
+        self.params = [torch.zeros(n, **kw) for n in self.n]
+        self.grads = [torch.zeros(n, **kw) for n in self.n]
+        self.momentum = [torch.zeros(n, **kw) for n in self.n]
+        self.loss_buf = torch.zeros(2, **kw)
+        for net in (G, D):
+            check(self.h, lib().gm_gan_bind(self.g, net, _ptr(self.params[net]), _ptr(self.grads[net]),
+                                            _ptr(self.momentum[net]), None))
+        H, X, Z = hidden_dim, image_size, z_dim
+        self.shapes = [[(H, Z), (H,), (X, H), (X,)], [(H, X), (H,), (1, H), (1,)]]
+
+    def views(self, net, flat=None, sample=0):
+        """[W1, b1, W2, b2] of D, or of generator sample `sample`, as views into `flat` (default: the parameters)"""
+        flat = self.params[net] if flat is None else flat
+        if net == G:
+            if not 0 <= sample < self.num_g:
+                raise GmError("sample %d outside [0, %d)" % (sample, self.num_g))
+            flat = flat[sample * self.stride:(sample + 1) * self.stride]
+        return GanEngine.views(self, net, flat)
+
+    def load(self, net, tensors, sample=0):
+        """Copy [W1, b1, W2, b2] into D or into generator sample `sample` and refresh the bf16 copies."""
+        for dst, src in zip(self.views(net, sample=sample), tensors):
+            dst.copy_(torch.as_tensor(src, dtype=torch.float32).reshape(dst.shape))
+        self.sync_shadows(net)
+
+    def reset_optimizer(self):
+        """v <- 0 for both nets (SGHMC's momentum starts at rest)"""
+        for m in self.momentum:
+            m.zero_()
+
+    def d_grad(self, images, noise=None, fmt="f32", gather_idx=None, batch=None, seed=0, step=0, loss_out=None):
+        """U_D and D's gradient; noise [num_g * batch, z] (sample-major) or the device's Philox draw"""
+        B = batch if batch is not None else (gather_idx.numel() if gather_idx is not None else images.shape[0])
+        dst = self.loss_buf[0] if loss_out is None else loss_out
+        check(self.h, lib().gm_bgan_d_grad(self.g, _ptr(images), IMG_FMTS[fmt], _ptr(gather_idx), B, _ptr(noise), int(seed),
+                                           int(step), _ptr(dst), _stream()))
+        return dst
+
+    def g_grad(self, batch, noise=None, seed=0, step=0, loss_out=None):
+        """mean_j U_j and each sample's gradient in its slice of grads[G]"""
+        dst = self.loss_buf[1] if loss_out is None else loss_out
+        check(self.h, lib().gm_bgan_g_grad(self.g, batch, _ptr(noise), int(seed), int(step), _ptr(dst), _stream()))
+        return dst
+
+    def apply(self, net, hp, seed=0, step=0):
+        """one SGHMC update of net (hp: _lib.SghmcHP) and the refresh of its operand copies"""
+        check(self.h, lib().gm_bgan_apply(self.g, net, C.byref(hp), int(seed), int(step), _stream()))
+
+    def sghmc_noise(self, net, seed, step):
+        """the xi apply(net, seed=seed, step=step) draws, over the net's whole flat block (tests)"""
+        out = torch.empty(self.n[net], device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_bgan_sghmc_noise(self.g, net, int(seed), int(step), _ptr(out), _stream()))
+        return out
+
+    def generate(self, sample, noise):
+        """Generator.forward of sample `sample`: noise [n, z] -> images [n, image_size]"""
+        n = noise.shape[0]
+        out = torch.empty(n, self.image_size, device=self.device, dtype=torch.float32)
+        check(self.h, lib().gm_bgan_generate(self.g, int(sample), _ptr(noise.contiguous().float()), n, _ptr(out), _stream()))
+        return out
+
+    supports_custom_loss = False
+    supports_custom_g = False

@@ -466,6 +466,50 @@ int gm_aae_num_d_slots(const gm_vae* vae);
 int gm_aae_d_forward(gm_vae* vae, int slot, const float* z_dev, int batch, float* scores_dev, gm_stream stream);
 int gm_aae_d_backward(gm_vae* vae, int slot, int batch, const float* dscores_dev, float* dz_dev, gm_stream stream);
 
+/* ---- Bayesian GAN (bayes_gan.py; Saatchi & Wilson 2017): a Bayes mode of the GAN engine ----------------------------
+ * J = num_g generator samples G_1..G_J (src/ns_gan.py:35-46 each) from the posterior over the generator weights and one
+ * discriminator (src/ns_gan.py:49-60, sigmoid output).  For a real batch x of B rows each G_j draws its own B noise rows:
+ *   U_D = -mean_i log(D(x_i) + 1e-8) - mean_{j,i} log(1 - D(G_j(z_ji)) + 1e-8)   (the second mean over all J B fake rows)
+ *   U_j = -mean_i log(D(G_j(z_ji)) + 1e-8)                                        (per sample; the reported loss is mean_j U_j)
+ * With J = 1 these are NSGAN's losses and the entries below compute what gm_gan_d_grad / gm_gan_g_grad of a GM_NS engine
+ * compute, bit for bit.  Every net is moved by stochastic-gradient Hamiltonian Monte Carlo (gm_bgan_apply), elementwise
+ * with momentum v and prior N(0, prior_std^2 I) on the per-example scale of the gradient g:
+ *   v <- (1 - alpha) v - lr (g + theta / (prior_std^2 data_size)) + sqrt(2 alpha lr / data_size) xi,  theta <- theta + v
+ * xi ~ N(0, 1) is drawn in the kernel by Philox keyed by (seed, step, net), the flat element index as subsequence.
+ * G's flat block stacks the samples, [sample 0 | sample 1 | ...], each in gm_gan_create's G layout and
+ * gm_bgan_g_stride floats apart (G's parameter count rounded up to a multiple of 4); gm_gan_param_count(G) is
+ * num_g x that stride and D's block is gm_gan_create's.  gm_gan_bind takes each net's momentum v in the exp_avg slot
+ * (exp_avg_sq may be NULL); gm_gan_sync_shadows refreshes every sample's operand copies; gm_gan_set_sampler,
+ * gm_gan_discriminate and gm_gan_debug_read (rows: noise, G hidden and dL/dG-pre-sigmoid num_g x max_batch, images and
+ * D rows (1 + num_g) x max_batch) serve the engine too.  The other gm_gan_* entries (Adam and its all-reduce, the
+ * fused and staged steps, lazy gradients on, device-step mode, gm_gan_attach_comm, the per-call forward / backward
+ * entries, gm_gan_generate, Q and BEGAN) refuse it with GM_ERR_ARG, and the gm_bgan_* entries refuse any other engine
+ * with GM_ERR_ARG, before anything is launched.  gm_bgan_create needs desc->variant GM_NS, d_out_act GM_OUT_SIGMOID and
+ * 1 <= num_g <= 16 (GM_ERR_ARG otherwise) besides what gm_gan_create needs, and refuses GM_PREC_SPLIT and a
+ * (1 + num_g) x max_batch whose row-buffer indices overflow 32 bits with GM_ERR_UNSUPPORTED. */
+typedef struct {
+  float lr, alpha, prior_std, data_size;   /* data_size: N, the size of the training set */
+} gm_sghmc_hp;
+int gm_bgan_create(gm_ctx* ctx, const gm_gan_desc* desc, int num_g, gm_gan** out);
+int gm_bgan_num_samples(const gm_gan* gan);   /* num_g; 0 for an engine of gm_gan_create */
+int gm_bgan_g_stride(const gm_gan* gan);      /* floats between consecutive samples in G's flat block */
+/* U_D and D's flat gradient: the real rows are staged as gm_gan_d_grad stages them (image formats, gather_idx_dev, the
+ * resident sampler at `step`), each sample's generator runs on its noise rows (noise_dev [num_g * batch, z] fp32,
+ * sample-major, or NULL for Philox draws keyed by (seed, 2 step): gm_gan_d_grad's for num_g = 1), then D on all
+ * (1 + num_g) batch rows.  loss_dev[0] = U_D. */
+int gm_bgan_d_grad(gm_gan* gan, const void* images_dev, int img_fmt, const int* gather_idx_dev, int batch,
+                   const float* noise_dev, uint64_t seed, uint64_t step, float* loss_dev, gm_stream stream);
+/* the U_j and their gradients, sample j's in its slice of G's flat gradient; noise as above (Philox stream 2 step + 1);
+ * loss_dev[0] = mean_j U_j. */
+int gm_bgan_g_grad(gm_gan* gan, int batch, const float* noise_dev, uint64_t seed, uint64_t step, float* loss_dev, gm_stream stream);
+/* one SGHMC update of `net` (the bound gradient and momentum) and the refresh of its operand copies.  Refuses lr < 0, alpha
+ * outside [0, 1], prior_std <= 0 and data_size <= 0 with GM_ERR_ARG. */
+int gm_bgan_apply(gm_gan* gan, int net, const gm_sghmc_hp* hp, uint64_t seed, uint64_t step, gm_stream stream);
+/* Generator.forward of sample `sample` for inference: noise_dev [n, z] fp32 -> images_dev [n, image_size] fp32 */
+int gm_bgan_generate(gm_gan* gan, int sample, const float* noise_dev, int n, float* images_dev, gm_stream stream);
+/* test aid: the xi gm_bgan_apply(net, seed, step) draws, for every element of the net's flat block -> out_dev */
+int gm_bgan_sghmc_noise(gm_gan* gan, int net, uint64_t seed, uint64_t step, float* out_dev, gm_stream stream);
+
 /* ---- conv building blocks (DCGAN path, BASELINE configs[4]; README.md:68,96 recommends DCGAN, the reference has no
  * implementation).  NHWC bf16 activations as row-major matrices [B*H*W, C]; a 4x4 stride-2 pad-1 convolution is
  * gm_im2col_k4s2 + gm_gemm_bf16, a transposed convolution gm_gemm_bf16 + gm_col2im_k4s2; their gradients are the same
