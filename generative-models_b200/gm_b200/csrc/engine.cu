@@ -37,7 +37,9 @@ struct gm_ctx {
   // gm_prof_enable: 0 off, 1 CUDA events around every GEMM launch (gm_prof_collect sums them by plan kind), 2 around every
   // launch (gm_prof_report sums them by kernel name: in-stream durations including the launch gaps)
   int prof = 0;
-  struct ProfRec { const char* name; int kind; double flops; cudaEvent_t e0, e1; };   // name: level 2 only; kind -1: not a GEMM
+  // name: level 2 only; kind -1: not a GEMM.  launches: 2 for a GEMM run as a main and a companion grid (launch_pp208),
+  // timed as one span: an event between the two grids would hold the companion back until the main grid completes
+  struct ProfRec { const char* name; int kind; double flops; cudaEvent_t e0, e1; int launches; };
   std::vector<ProfRec> prof_recs;
 };
 
@@ -107,6 +109,7 @@ struct GemmPlan {
   // MN-major 208-wide plans: 16-column tail boxes of tmB / tmB2 (32-byte swizzle).  K-major 208-wide plans: the boxes of
   // the cluster ranks' shorter B shares (b_share_rows)
   CUtensorMap tmBt, tmB2t;
+  CUtensorMap tmBc;         // K-major 208-wide plans: B in the 104-row shares of a 2-CTA companion grid (launch_pp208)
   // output map of the K-major bf16 kernels (16-row x 32-column box, 64-byte swizzle), encoded at the first
   // launch because the epilogue (output pointer / leading dimension) is set after plan_gemm
   mutable CUtensorMap tmC;
@@ -116,6 +119,7 @@ struct GemmPlan {
   int bn;         // tile width: the TN kind (PK_TN_256) runs 208- or 256-wide tiles
   int grid;
   double flops;   // algorithmic 2*M*N*K of the logical problem (no padding)
+  bool one_grid;  // gm_gemm_bf16: one GEMM kernel per call, never a main + companion pair (launch_pp208)
 };
 
 // Profile name of a GEMM launch: plan kind and epilogue signature, output type, K class, split (interned)
@@ -139,14 +143,19 @@ static const char* gemm_name(const GemmPlan& pl) {
 }
 
 // What launch() accounts a kernel as: its name (a GEMM is named by its plan), whether it takes programmatic stream
-// serialisation, and for a GEMM its plan (kind and FLOPs for gm_prof_collect) and cluster size.
+// serialisation, and for a GEMM its plan (kind for gm_prof_collect), the FLOPs of this launch's share of the plan and
+// its cluster size.  span: SPAN_OWN times the launch on its own; a main grid (SPAN_OPEN) and the companion grid right
+// behind it (SPAN_CLOSE) share one profile record, which counts both launches.
+enum : int { SPAN_OWN = 0, SPAN_OPEN = 1, SPAN_CLOSE = 2 };
 struct KernelTag {
   const char* name;
   bool pdl = true;
   const GemmPlan* plan = nullptr;
   int cluster = 1;
+  double flops = 0.0;
+  int span = SPAN_OWN;
   KernelTag(const char* n, bool pdl_ = true) : name(n), pdl(pdl_) {}
-  KernelTag(const GemmPlan& pl, int cl) : name(nullptr), plan(&pl), cluster(cl) {}
+  KernelTag(const GemmPlan& pl, int cl, double fl, int sp) : name(nullptr), plan(&pl), cluster(cl), flops(fl), span(sp) {}
 };
 
 // Launch configuration; `at` receives its attributes.  With `pdl` the grid may become resident while its predecessor
@@ -184,11 +193,14 @@ template <typename... KArgs, typename... Args>
   cudaLaunchAttribute at[2];
   const cudaLaunchConfig_t cfg = launch_cfg(grid, block, smem, s, k.cluster, k.pdl && c->pdl, at);
   const bool timed = c->prof == 2 || (c->prof == 1 && k.plan);
+  // SPAN_CLOSE continues the record its main grid opened (launch_pp208 launches the two back to back)
+  const bool opens = timed && k.span != SPAN_CLOSE;
   gm_ctx::ProfRec r;
-  if (timed) {
+  if (opens) {
     r.name = c->prof == 2 ? (k.plan ? gemm_name(*k.plan) : k.name) : nullptr;
     r.kind = k.plan ? k.plan->kind : -1;
-    r.flops = k.plan ? k.plan->flops : 0.0;
+    r.flops = k.flops;
+    r.launches = 1;
     CU_OK(c, cudaEventCreate(&r.e0));
     CU_OK(c, cudaEventCreate(&r.e1));
     CU_OK(c, cudaEventRecord(r.e0, s));
@@ -196,53 +208,83 @@ template <typename... KArgs, typename... Args>
   const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
   if (e != cudaSuccess) {
     cudaGetLastError();   // a launch error is not sticky: leave no trace of it for the caller's next runtime call
-    if (timed) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
+    if (opens) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
+    else if (timed) cudaEventRecord(c->prof_recs.back().e1, s);   // close the main grid's record on its own
     return fail(c, GM_ERR_CUDA, "%s launch failed: %s", k.plan ? gemm_name(*k.plan) : k.name, cudaGetErrorString(e));
   }
   c->launches++;
   if (timed) {
-    c->prof_recs.push_back(r);
-    CU_OK(c, cudaEventRecord(r.e1, s));
+    if (opens) c->prof_recs.push_back(r);
+    gm_ctx::ProfRec& rec = c->prof_recs.back();
+    if (!opens) { rec.launches++; rec.flops += k.flops; }
+    if (k.span != SPAN_OPEN) CU_OK(c, cudaEventRecord(rec.e1, s));
   }
   return GM_OK;
 }
 
+// One grid of a plan's product: all of it (the default), or the main or companion share of a two-grid plan (launch_pp208):
+// m-tiles [m_tile0, m_tile0 + m_tiles), at most `clusters` clusters, B through tmB (the companion's 2-CTA B shares).
+struct GridPart {
+  int m_tile0 = 0, m_tiles = 0;   // m_tiles 0: all of the plan's
+  int clusters = 0;               // 0: as many as the device holds at once
+  int span = SPAN_OWN;
+  const CUtensorMap* tmB = nullptr;
+};
+
+// The instance's function, configured on the current device at its first use: the opt-in to > 48 KB dynamic shared
+// memory is per (function, device); so is the number of clusters that fit at once (*mc; 0 unclustered)
 template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false,
-          int CL = kGemmCluster<BN, AMN, BMN>>
-static int launch_inst(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
+          int CL = kGemmCluster<BN, AMN, BMN>, int ROLE = PDL_SINGLE>
+static int inst_clusters(gm_ctx* c, const GemmPlan& pl, cudaStream_t s, int* mc) {
   using Cfg = GemmCfg<BN, !AMN, PP>;
-  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP, CL>;
-  // the opt-in to > 48 KB dynamic shared memory is per (function, device); so is the number of clusters that fit at once
+  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP, CL, ROLE>;
   static bool configured[64] = {};
   static int max_clusters[64] = {};
   int dev = 0;
   CU_OK(c, cudaGetDevice(&dev));
   const bool cached = dev >= 0 && dev < 64;
-  int mc = cached ? max_clusters[dev] : 0;
+  *mc = cached ? max_clusters[dev] : 0;
   if (!cached || !configured[dev]) {
     CU_OK(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     if (CL > 1) {
       cudaLaunchAttribute at[2];
       const cudaLaunchConfig_t cfg = launch_cfg(dim3(CL), dim3(kGemmThreads), Cfg::SMEM_BYTES, s, CL, false, at);
-      CU_OK(c, cudaOccupancyMaxActiveClusters(&mc, kern, &cfg));
-      if (mc < 1) return fail(c, GM_ERR_CUDA, "%s: no %d-CTA cluster fits on device %d", gemm_name(pl), CL, dev);
+      CU_OK(c, cudaOccupancyMaxActiveClusters(mc, kern, &cfg));
+      if (*mc < 1) return fail(c, GM_ERR_CUDA, "%s: no %d-CTA cluster fits on device %d", gemm_name(pl), CL, dev);
     }
-    if (cached) { max_clusters[dev] = mc; configured[dev] = true; }
+    if (cached) { max_clusters[dev] = *mc; configured[dev] = true; }
   }
+  return GM_OK;
+}
+
+template <int BN, bool AMN, bool BMN, int EPI = kEpiUniversal, bool SPLIT = false, bool PP = false,
+          int CL = kGemmCluster<BN, AMN, BMN>, int ROLE = PDL_SINGLE>
+static int launch_inst(gm_ctx* c, const GemmPlan& pl, cudaStream_t s, const GridPart& part = GridPart()) {
+  using Cfg = GemmCfg<BN, !AMN, PP>;
+  auto kern = gemm_wgmma_kernel<BN, AMN, BMN, EPI, SPLIT, PP, CL, ROLE>;
+  int mc = 0;
+  if (int rc = inst_clusters<BN, AMN, BMN, EPI, SPLIT, PP, CL, ROLE>(c, pl, s, &mc)) return rc;
+  GemmParams prm = pl.p;
+  double flops = pl.flops;
+  if (part.m_tiles > 0) {
+    prm.m_tile0 = part.m_tile0;
+    prm.m_tiles = part.m_tiles;
+    const int end = (part.m_tile0 + part.m_tiles) * BM, rows = (end < prm.M ? end : prm.M) - part.m_tile0 * BM;
+    flops = pl.flops * double(rows) / double(prm.M);
+  }
+  if (part.clusters > 0 && part.clusters < mc) mc = part.clusters;
   dim3 grid(pl.grid);
   if (CL > 1) {
     // persistent: one cluster per item, up to the clusters the device holds at once (a GPC need not hold a multiple of CL
     // SMs).  K-major clusters group CL m-tiles, MN-major ones pair n-tiles (of an even count)
-    const GemmParams& q = pl.p;
-    const int items = (BMN ? q.m_tiles * (q.n_tiles / CL) : cdiv(q.m_tiles, CL) * q.n_tiles) * q.splits;
+    const int items = (BMN ? prm.m_tiles * (prm.n_tiles / CL) : cdiv(prm.m_tiles, CL) * prm.n_tiles) * prm.splits;
     grid = dim3(CL * (items < mc ? items : mc));
   }
-  GemmParams prm = pl.p;
   prm.tma_store = pl.tmc_state == 1 ? 1 : 0;
   // fp32 rows take float4 stores only where every row of every split starts on 16 bytes (ldc = 30: row 1 is at byte 120)
   prm.f32_vec = prm.epi == EPI_F32 && !(reinterpret_cast<uintptr_t>(prm.part) & 15) && prm.ldp % 4 == 0 && prm.part_stride % 4 == 0;
-  return launch(c, KernelTag(pl, CL), kern, grid, kGemmThreads, Cfg::SMEM_BYTES, s, pl.tmA, pl.tmB, pl.tmC, pl.tmA2, pl.tmB2,
-                pl.tmBt, pl.tmB2t, prm);
+  return launch(c, KernelTag(pl, CL, flops, part.span), kern, grid, kGemmThreads, Cfg::SMEM_BYTES, s, pl.tmA,
+                part.tmB ? *part.tmB : pl.tmB, pl.tmC, pl.tmA2, pl.tmB2, pl.tmBt, pl.tmB2t, prm);
 }
 
 // TN kind: the 256-wide tile, or the 208-wide one as 2-CTA clusters over n-tile pairs (an even n-tile count, plan_gemm)
@@ -262,6 +304,56 @@ static int launch_split(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   else return launch_inst<BN, AMN, BMN, kEpiUniversal, true>(c, pl, s);
 }
 
+// Per-SM rate of the 2-CTA ping-pong instance (a companion grid) over that of the 4-CTA one: 2-CTA clusters load B once
+// per 64-row half for two m-tiles, 43 008 instead of 29 696 B per 128 rows and k-block.  Measured on an H100 SXM at 700 W
+// (DESIGN §5) with the whole GEMM as 66 2-CTA clusters against 30 4-CTA clusters at B = 65536: 0.72 for d1 on 2B rows,
+// 0.79 for g2 and dx.  The lower one, rounded down; every train-step split is the same for rates from 0.7 to 1.
+constexpr double kCompanionRate = 0.7;
+
+// Two-grid split of a K-major 208-wide ping-pong plan.  30 4-CTA clusters fit on an H100 SXM: 120 SMs, since some GPCs
+// hold 4k + 2 SMs, and the last of a plan's rounds of 30 items is mostly empty (512 items: 17.07 rounds run as 18).  So a
+// plan of two or more rounds runs m-tiles [0, 4 g) as the main grid of 4-CTA clusters and m-tiles [4 g, m_tiles) in
+// pairs as a companion grid of 2-CTA clusters on the SMs left over, (num_sms - 4 main_clusters) / 2 clusters.  g makes
+// the two grids finish together, at the companion's rate kCompanionRate; among equal finishes the largest g.  Returns 0
+// (one grid) where that finishes no sooner.  Every (m-tile, n-tile) keeps its k order, warp, lane and epilogue code, so
+// outputs are bit-identical to the single grid's.
+static int companion_groups(const GemmParams& p, int main_clusters, int comp_clusters) {
+  if (comp_clusters < 1 || main_clusters < 1 || p.splits != 1) return 0;
+  const int single = cdiv(cdiv(p.m_tiles, 4) * p.n_tiles, main_clusters);
+  if (single < 2) return 0;
+  int best = 0;
+  double best_t = single;
+  for (int g = 1; 4 * g < p.m_tiles; ++g) {
+    const double t_main = cdiv(g * p.n_tiles, main_clusters);
+    const double t_comp = cdiv(cdiv(p.m_tiles - 4 * g, 2) * p.n_tiles, comp_clusters) / kCompanionRate;
+    const double t = t_main > t_comp ? t_main : t_comp;
+    if (t < best_t || (best && t == best_t)) { best = g; best_t = t; }
+  }
+  return best;
+}
+
+// A ping-pong plan: one grid of 4-CTA clusters, or a main and a companion grid (companion_groups; PDL_* for their order)
+template <int EPI>
+static int launch_pp208(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
+  int mc4 = 0;
+  if (int rc = inst_clusters<208, false, false, EPI, false, true, 4>(c, pl, s, &mc4)) return rc;
+  // the companion overlaps the main grid only through programmatic dependent launch
+  const int g = c->pdl && !pl.one_grid ? companion_groups(pl.p, mc4, (c->num_sms - 4 * mc4) / 2) : 0;
+  if (g == 0) return launch_inst<208, false, false, EPI, false, true, 4>(c, pl, s);
+  const bool timed = c->prof != 0;
+  GridPart main;
+  main.m_tiles = 4 * g;
+  main.span = timed ? SPAN_OPEN : SPAN_OWN;
+  if (int rc = launch_inst<208, false, false, EPI, false, true, 4, PDL_MAIN>(c, pl, s, main)) return rc;
+  GridPart comp;
+  comp.m_tile0 = 4 * g;
+  comp.m_tiles = pl.p.m_tiles - 4 * g;
+  comp.clusters = (c->num_sms - 4 * mc4) / 2;
+  comp.span = timed ? SPAN_CLOSE : SPAN_OWN;
+  comp.tmB = &pl.tmBc;
+  return launch_inst<208, false, false, EPI, false, true, 2, PDL_COMPANION>(c, pl, s, comp);
+}
+
 // K-major 128x208 kernel: the compile-time-specialised instance of the plan's epilogue signature when the train steps use
 // that signature, else the universal instance.  The specialised instances run their consumer warpgroups in ping-pong, so
 // each half-tile's epilogue hides under the other warpgroup's wgmma; the 4-CTA cluster's multicast keeps the B feed of
@@ -269,7 +361,7 @@ static int launch_split(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
 static int launch_nt208(gm_ctx* c, const GemmPlan& pl, cudaStream_t s) {
   const GemmParams& p = pl.p;
   if (p.epi != EPI_BF16) return launch_inst<208, false, false>(c, pl, s);
-#define NT208(S) case S: return launch_inst<208, false, false, S, false, true>(c, pl, s)
+#define NT208(S) case S: return launch_pp208<S>(c, pl, s)
   switch (epi_sig(p)) {
     NT208(epi_sig(ACT_RELU, AUX_NONE, true, DOT_NONE));
     NT208(epi_sig(ACT_SIGMOID, AUX_NONE, true, DOT_NONE));
@@ -338,6 +430,7 @@ static int plan_gemm(gm_ctx* c, GemmPlan* pl, int mode, int M, int N, int K, con
     rc = make_tmap(c, &pl->tmB, B, K, N, ldb, BK, boxn);
     if (rc) return rc;
     if (boxn_t && (rc = make_tmap(c, &pl->tmBt, B, K, N, ldb, BK, boxn_t))) return rc;
+    if (boxn_t && c->plan_lo == 0 && (rc = make_tmap(c, &pl->tmBc, B, K, N, ldb, BK, b_share_rows(208, 2, 0)))) return rc;
   } else {
     // K (batch rows) need not be a multiple of 64: rows past the extent are TMA zero-fill.  Wide outputs take the 208-wide
     // tile, run as 2-CTA clusters over n-tile pairs, wherever it needs an even number of n-tiles and no more than the
@@ -479,7 +572,7 @@ extern "C" int gm_prof_report(gm_ctx* c, char* buf, int buflen) {
       cudaEventElapsedTime(&t, r.e0, r.e1);
       auto it = agg.find(r.name);
       if (it == agg.end()) { order.push_back(r.name); it = agg.emplace(r.name, std::make_pair(0ll, 0.0)).first; }
-      it->second.first++; it->second.second += t;
+      it->second.first += r.launches; it->second.second += t;
     }
     cudaEventDestroy(r.e0); cudaEventDestroy(r.e1);
   }
@@ -504,7 +597,7 @@ extern "C" int gm_prof_collect(gm_ctx* c, double* ms, double* flops, long long* 
     if (r.kind >= 0) {
       float t = 0.f;
       cudaEventElapsedTime(&t, r.e0, r.e1);
-      ms[r.kind] += t; flops[r.kind] += r.flops; count[r.kind]++;
+      ms[r.kind] += t; flops[r.kind] += r.flops; count[r.kind] += r.launches;
     }
     cudaEventDestroy(r.e0);
     cudaEventDestroy(r.e1);
@@ -549,6 +642,7 @@ extern "C" int gm_gemm_bf16(gm_ctx* c, const gm_gemm_desc* d, gm_stream stream) 
   }
   int rc = plan_gemm(c, &pl, d->mode, d->M, d->N, d->K, d->A_dev, d->lda, d->B_dev, d->ldb, ncover, f32 ? 64 : 1);
   if (rc) return rc;
+  pl.one_grid = true;
   GemmParams& p = pl.p;
   if (!f32) {
     p.epi = EPI_BF16;

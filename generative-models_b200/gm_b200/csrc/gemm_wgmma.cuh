@@ -109,7 +109,28 @@ struct GemmParams {
   int nparts, kb_part;
   long long lo_off;
   float act_slope;      // ACT_LRELU
+  // ---- companion grid of a two-grid K-major plan (launch_pp208): it takes m-tiles [m_tile0, m_tile0 + m_tiles)
+  int m_tile0;
 };
+// Programmatic dependent launch of a grid (the kernel's ROLE): PDL_SINGLE lets its dependent launch at once and waits for
+// its predecessor after the prologue.  A plan split into a main grid and a companion grid launched right behind it
+// (launch_pp208):
+//  * PDL_MAIN waits for its predecessor before it lets the companion launch.  The companion launches only once every
+//    main CTA has executed griddepcontrol.launch_dependents (or exited), so when it starts, the kernel that wrote both
+//    grids' inputs has completed and its writes are visible in L2 (CUDA Programming Guide, "Programmatic Dependent Launch
+//    and Synchronization"; PTX ISA, griddepcontrol).
+//  * PDL_COMPANION therefore does not wait before its first load, and so takes the SMs the resident main grid leaves free.
+//    It waits before it exits: griddepcontrol.wait returns once the prerequisite grid (the main grid) has completed and
+//    its writes are visible, and the next kernel in the stream waits only for the grid right before it (the companion),
+//    so that kernel's wait covers the main grid too.
+//    Every load it makes is served from L2, which the predecessor's writes reached before it completed: the operands
+//    arrive through the TMA, aux rows through cp.async.cg or ld.global.nc, bias and row-dot weights through ld.global.nc,
+//    and the cluster barrier after barrier init (barrier.cluster.wait, acquire) invalidates the SM's L1 before the first
+//    of them (CCTL.IVALL in the SASS, ahead of every LDG and UTMALDG).
+// ROLE is a template argument, so a single grid issues launch_dependents without waiting for a parameter load: read from
+// GemmParams, the role put a constant-cache miss ahead of it in every GEMM, and the CUDA-graph small-batch step took 1%
+// longer (DESIGN §5).
+enum : int { PDL_SINGLE = 0, PDL_MAIN = 1, PDL_COMPANION = 2 };
 
 inline int epi_sig(const GemmParams& p) { return epi_sig(p.act, p.aux_mode, p.bias != nullptr, p.dot); }
 
@@ -180,10 +201,11 @@ constexpr int kTnTail = 16;
 // EPI: the fused epilogue's signature (epi_sig), or kEpiUniversal.
 // PINGPONG: the consumer warpgroups run the 64-row halves of each tile as half-items of their own (see the consumer loop)
 // CL: CTAs per cluster; with MN-major operands the cluster's CTAs take adjacent n-tiles of one m-tile.
+// ROLE: PDL_SINGLE, or the main (PDL_MAIN) or companion (PDL_COMPANION) grid of a two-grid ping-pong plan.
 // tmBt / tmB2t: the 16-column tail boxes of tmB / tmB2 (MN-major 208-wide kernel), or the shorter B shares of a
 // K-major cluster (b_share_rows)
 template <int BN, bool A_MN, bool B_MN, int EPI = kEpiUniversal, bool SPLIT = false, bool PINGPONG = false,
-          int CL = kGemmCluster<BN, A_MN, B_MN>>
+          int CL = kGemmCluster<BN, A_MN, B_MN>, int ROLE = PDL_SINGLE>
 // 384 threads, one block per SM: 168 registers per thread at launch, redistributed by setmaxnreg
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -205,6 +227,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // K-major: each CTA's share of the B tile starts on a 1024-byte swizzle atom, so the B descriptor is the same as for
   // one box.  MN-major: each CTA's share of the A tile is one whole 64-column box, so the A descriptor is unchanged.
   static_assert(CL == 1 || CL == 2 || CL == 4, "cluster size");
+  static_assert(ROLE == PDL_SINGLE || (PINGPONG && !SPLIT && CL == (ROLE == PDL_MAIN ? 4 : 2)), "two-grid plans: ping-pong only");
+  constexpr int kMTile0 = ROLE == PDL_COMPANION;   // the companion's m-tiles start at p.m_tile0
   static_assert(CL == 1 || (!B_MN && BN % 8 == 0 && BK * 2 == 128 && b_share_rows(BN, CL, CL - 1) > 0) ||
                 (B_MN && kTail && BM / CL == 64), "multicast share");
   // K-major cluster: ranks below kBigShares load their B share through tmB / tmB2, the others through tmBt / tmB2t
@@ -220,7 +244,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0);   // provably warp-uniform (wgmma issue)
   const int lane = threadIdx.x & 31;
 
-  griddep_launch();   // the next grid may start its prologue as soon as SMs free up
+  // the next grid may start its prologue as soon as SMs free up (a main grid lets its companion launch only further down)
+  if constexpr (ROLE != PDL_MAIN) griddep_launch();
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
@@ -238,18 +263,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // the barriers are initialised in every CTA of the cluster before any peer arrives on them or multicasts into them
   if constexpr (CL > 1) cluster_sync();
   else __syncthreads();
-  griddep_wait();     // barrier init above overlapped the previous grid's tail
+  // barrier init above overlapped the previous grid's tail
+  if constexpr (ROLE != PDL_COMPANION) griddep_wait();
+  if constexpr (ROLE == PDL_MAIN) griddep_launch();
 
   // Work items walk (split, m-group, n-group) with one item per cluster.  K-major: CTA rank r of a cluster takes m-tile
   // CL * group + r of the item's n-tile; m-tiles are rounded up to whole groups: a CTA on a tile past M loads its share
   // of B, computes on zero-filled A rows and stores nothing (every store is guarded by row < M or clipped at the tensor
   // extent), so all CTAs walk the same k-blocks through the ring.  MN-major (n_tiles a multiple of CL): rank r takes
   // n-tile CL * group + r of the item's m-tile; both CTAs share split and m-tile, so they walk the same k-blocks too.
+  // The companion grid of a two-grid plan (ROLE) starts its m-tiles at p.m_tile0.
   constexpr bool kPairN = CL > 1 && B_MN;
   const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
   const int n_groups = kPairN ? p.n_tiles / CL : p.n_tiles;
   const int tiles = (kPairN ? p.m_tiles : (p.m_tiles + CL - 1) / CL) * n_groups;
-  auto m0_of = [&](int rem) { return ((rem / n_groups) * (kPairN ? 1 : CL) + (kPairN ? 0 : rank)) * BM; };
+  auto m0_of = [&](int rem) { return (kMTile0 * p.m_tile0 + (rem / n_groups) * (kPairN ? 1 : CL) + (kPairN ? 0 : rank)) * BM; };
   auto n_tile_of = [&](int rem) { return (rem % n_groups) * (kPairN ? CL : 1) + (kPairN ? rank : 0); };
   const int total = tiles * p.splits;
   const int first = blockIdx.x / CL, stride = gridDim.x / CL;
@@ -257,7 +285,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // k-blocks enter the ring one half after the other.  The second half is skipped in all CTAs of the cluster when rank
   // 0's first row of it is past M (the other ranks' rows are higher still), so the peers keep walking the same k-blocks.
   auto halves_of = [&](int rem) -> int {
-    if constexpr (PP) return (rem / p.n_tiles) * CL * BM + Cfg::A_ROWS < p.M ? 2 : 1;
+    if constexpr (PP) return (kMTile0 * p.m_tile0 + (rem / p.n_tiles) * CL) * BM + Cfg::A_ROWS < p.M ? 2 : 1;
     else return 1;
   };
   // A k-block's stage and phase follow from the running count `it` of k-blocks issued, in (item, half-item, k-block)
@@ -803,6 +831,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // no CTA exits while a peer may still arrive on its barriers (its multicasts have all landed: every stage was consumed)
   if constexpr (CL > 1) cluster_sync();
   else __syncthreads();
+  if constexpr (ROLE == PDL_COMPANION) griddep_wait();   // the main grid has completed before the companion does (PDL_*)
 }
 
 }  // namespace gm

@@ -89,6 +89,9 @@ int gm_ctx_num_sms(const gm_ctx* ctx);
  * out_kind 1: fp32 C_dev (ldc floats; transposed store if transpose), split-K
  *             partials summed by the library into C_dev.  Only the logical
  *             block ([M, N], or [N, M] transposed) is written.
+ * A call launches one GEMM kernel, plus one that sums the partials when an
+ * fp32 product is split over K.  (The train-step engines may run a K-major
+ * GEMM as two grids.)
  * Refused with GM_ERR_ARG before any launch: mode outside 0..1; mode 1 with a
  * bf16 output; act outside 0..3 or aux_mode outside 0..3; aux_mode without
  * aux_dev or the reverse; an fp32 output with any epilogue field (out_cols
