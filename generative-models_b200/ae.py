@@ -16,7 +16,7 @@ from utils import *  # noqa: F401,F403
 
 from gm_b200 import AdamHP, AeEngine, GmError
 from gm_b200.gan_api import (to_cuda, builtin_step, has_custom_compute_batch, refuse_multi_rank, compute_batch_loop,
-                             compute_batch_evaluate, slot_ring, EngineCall, GradHandoff, grow_engine)
+                             compute_batch_evaluate, engine_call, GradHandoff, grow_engine)
 
 
 class Encoder(nn.Module):
@@ -29,19 +29,14 @@ class Encoder(nn.Module):
     def forward(self, x):
         eng, attached = _engine_of(self, "Encoder", x.shape[0])
         if attached and torch.is_grad_enabled():   # the code relu(linear(x)) and its backward on the CUDA kernels
-            ring, n = slot_ring(eng, "Encoder", eng.SLOTS), x.shape[0]
+            n = x.shape[0]
 
-            def forward(x):
-                slot, gen = ring.take()
-                return eng.encoder_forward(slot, x), (slot, gen)
-
-            def backward(handle, grads, need_dx):
+            def backward(slot, grads, need_dx):
                 if need_dx:
                     raise RuntimeError("the gradient with respect to the encoder's input is not computed")
-                ring.check(*handle)
-                g = eng.encoder_backward(handle[0], n, grads[0])
-                return None, [g["encoder.linear.weight"], g["encoder.linear.bias"]]
-            return EngineCall.apply(to_cuda(x).float(), forward, backward, self.linear.weight, self.linear.bias)
+                return eng.encoder_backward(slot, n, grads[0]), None
+            return engine_call(eng, "Encoder", eng.SLOTS, to_cuda(x).float(), self.named_parameters("encoder"),
+                               eng.encoder_forward, backward)
         return eng.encode(to_cuda(x).float())
 
 
@@ -55,17 +50,13 @@ class Decoder(nn.Module):
     def forward(self, encoder_output):
         eng, attached = _engine_of(self, "Decoder", encoder_output.shape[0])
         if attached and torch.is_grad_enabled():   # sigmoid(linear(code)) and its backward, with dL/dcode when the code requires grad
-            ring, n = slot_ring(eng, "Decoder", eng.SLOTS), encoder_output.shape[0]
+            n = encoder_output.shape[0]
 
-            def forward(code):
-                slot, gen = ring.take()
-                return eng.decoder_forward(slot, code), (slot, gen)
-
-            def backward(handle, grads, need_dcode):
-                ring.check(*handle)
-                g, dcode = eng.decoder_backward(handle[0], n, grads[0])
-                return (dcode if need_dcode else None), [g["decoder.linear.weight"], g["decoder.linear.bias"]]
-            return EngineCall.apply(to_cuda(encoder_output).float(), forward, backward, self.linear.weight, self.linear.bias)
+            def backward(slot, grads, need_dcode):
+                g, dcode = eng.decoder_backward(slot, n, grads[0])
+                return g, (dcode if need_dcode else None)
+            return engine_call(eng, "Decoder", eng.SLOTS, to_cuda(encoder_output).float(), self.named_parameters("decoder"),
+                               eng.decoder_forward, backward)
         return eng.decode(to_cuda(encoder_output).float())
 
 

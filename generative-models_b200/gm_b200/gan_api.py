@@ -526,6 +526,25 @@ class EngineCall(torch.autograd.Function):
         return (dx, None, None, *param_grads)
 
 
+def engine_call(eng, what, slots, x, named, fwd, bwd):
+    """x through one grad-mode call of eng's `what` module on a slot of its SlotRing (made with `slots` slots):
+    fwd(slot, x) runs the forward kernels and returns the outputs; bwd(slot, upstream gradients, need_dx) runs the
+    backward ones once the slot is checked and returns ({parameter name: gradient}, dL/dx or None).  named: the module's
+    (name, parameter) pairs, named as bwd's gradients are (module.named_parameters("encoder") for encoder.* keys)."""
+    ring = slot_ring(eng, what, slots)
+    names, params = zip(*named)
+
+    def forward(x):
+        slot, gen = ring.take()
+        return fwd(slot, x), (slot, gen)
+
+    def backward(handle, grads, need_dx):
+        ring.check(*handle)
+        g, dx = bwd(handle[0], grads, need_dx)
+        return dx, [g[k] for k in names]
+    return EngineCall.apply(x, forward, backward, *params)
+
+
 class GradHandoff(torch.autograd.Function):
     """A loss whose backward() adds gradients the fused kernels already computed, times the upstream, to the parameters'
     .grad (the reference calls loss.backward() then optimizer.step(), src/ns_gan.py:138-139).  pairs: (parameter, its
